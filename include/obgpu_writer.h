@@ -123,6 +123,30 @@ typedef struct obgpu_macro_spec {
 int obgpu_writer_build_macro_blocks(const void *micro_image, const int64_t *offsets, const int64_t *sizes, int32_t n_blocks,
                                     const obgpu_macro_spec *spec, void *out, int64_t out_cap, int64_t *out_size,
                                     int32_t *n_macro, int32_t *first_micro, int32_t first_micro_cap);
+/* The same with the FixedHeader's compressor_type_ (OBGPU_COMPRESSOR_*). The micro-blocks are taken as they are, in stored
+ * form (obgpu_writer_compress_blocks): a macro block records the compressor, it does not apply it. With NONE every block must
+ * have data_zlength_ == data_length_ (OBGPU_INVALID_ARGUMENT otherwise); other compressors: OBGPU_NOT_SUPPORTED.
+ * obgpu_writer_build_macro_blocks is this call with OBGPU_COMPRESSOR_NONE. */
+int obgpu_writer_build_macro_blocks_ex(const void *micro_image, const int64_t *offsets, const int64_t *sizes, int32_t n_blocks,
+                                       const obgpu_macro_spec *spec, void *out, int64_t out_cap, int64_t *out_size,
+                                       int32_t *n_macro, int32_t *first_micro, int32_t first_micro_cap, int32_t compressor_type);
+
+/* =============================================================================================
+ * Compressed micro-blocks (ObMicroBlockWriter / ObMicroBlockEncoder::build_block -> ObMicroBlockCompressor::compress): the
+ * 64-byte ObMicroBlockHeader stays plain, the payload behind it is compressed on its own, data_zlength_ is the stored
+ * payload size and data_length_ the decoded one; data_checksum_ is the crc32c of the STORED payload bytes.
+ * ============================================================================================= */
+/* One LZ4 block (lz4 block format: no frame, no size prefix; what LZ4_compress_default's output decodes like): greedy, 64 KiB
+ * window, end-of-block rules of the format kept. out == NULL: only *out_len (never more than src_len + src_len / 255 + 16). */
+int obgpu_writer_lz4_compress(const void *src, int64_t src_len, void *out, int64_t out_cap, int64_t *out_len);
+/* Re-frames n plain micro-blocks (data_zlength_ == data_length_) into stored form with `compressor` (OBGPU_COMPRESSOR_LZ4 /
+ * LZ4_1_9_1; NONE copies): the payload is compressed and kept raw when that is not smaller; a compressed block gets
+ * data_zlength_, data_checksum_ (crc32c of the stored bytes) and a recomputed header checksum. Block i goes to
+ * out[out_offsets[i], out_offsets[i] + out_sizes[i]), offsets multiples of align (a power of two; 1: back to back).
+ * out_cap >= sum over i of (sizes[i] rounded up to align) always suffices; *out_size = bytes used. */
+int obgpu_writer_compress_blocks(const void *image, const int64_t *offsets, const int64_t *sizes, int32_t n_blocks, int32_t compressor,
+                                 int64_t align, void *out, int64_t out_cap, int64_t *out_offsets, int64_t *out_sizes,
+                                 int64_t *out_size);
 
 int obgpu_writer_set_cs_stream_encoding(int32_t mode);
 /* The codec bytes alone (no ObIntegerStreamMeta) for count values of width_bytes (low bytes of vals[i]); type 0 =

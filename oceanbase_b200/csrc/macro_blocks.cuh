@@ -7,8 +7,10 @@
 //             micro_block_data_offset_; the walk must end at micro_block_data_offset_ + micro_block_data_size_ with row_count_ rows
 //   realign : one CTA per micro-block copies it to a 128-byte aligned slot of a new image (unaligned source words through
 //             funnel shifts, 16-byte stores, zero padding) -- one read + one write of the data, at HBM speed, once per cache fill
-// 16 bytes per micro-block (offset, size) and 4 per macro block come back to the host for obgpu_batch_open's tables; the block
-// bytes never touch the CPU. Compressed payloads (compressor_type_ != NONE) and encrypted blocks are refused.
+// Macro blocks whose compressor_type_ is LZ4 / LZ4_1_9_1 hold micro-blocks in stored form: the walk's (offset, stored size)
+// pairs go to open_stored_blocks (lz4_blocks.cuh), which decodes the compressed ones into their slots and realigns the raw
+// ones with the kernel below. 16 bytes per micro-block (offset, size) and 4 per macro block come back to the host for
+// obgpu_batch_open's tables; the block bytes never touch the CPU. Other compressors and encrypted blocks are refused.
 #pragma once
 
 namespace mb {
@@ -21,7 +23,7 @@ __device__ __forceinline__ uint32_t ld32u(const uint8_t *p) {   // unaligned lit
 __device__ __forceinline__ uint64_t ld64u(const uint8_t *p) { return (uint64_t)ld32u(p) | ((uint64_t)ld32u(p + 4) << 32); }
 
 struct Fixed {
-  int32_t micro_count, data_off, data_size, row_count;
+  int32_t micro_count, data_off, data_size, row_count, compressor;
 };
 
 __device__ __forceinline__ int32_t parse_headers(const uint8_t *m, int64_t macro_size, Fixed &f) {
@@ -42,6 +44,7 @@ __device__ __forceinline__ int32_t parse_headers(const uint8_t *m, int64_t macro
   f.data_size = (int32_t)ld32u(h + 60);
   const int64_t data_checksum = (int64_t)ld64u(h + 80), encrypt_id = (int64_t)ld64u(h + 88), master_key = (int64_t)ld64u(h + 96);
   const uint32_t compressor = h[104];
+  f.compressor = (int32_t)compressor;
   if (!(version >= 1 && version <= 2 && magic == 1007 && tablet != 0 && logical >= 0 && rowkey_cnt >= 0 && row_store_type >= 0 &&
         f.row_count > 0 && occupy > 0 && f.micro_count > 0 && f.data_off > 0 && f.data_size > 0 && data_checksum >= 0 && encrypt_id >= 0 &&
         master_key >= -1 && compressor > 0))
@@ -50,7 +53,8 @@ __device__ __forceinline__ int32_t parse_headers(const uint8_t *m, int64_t macro
   if (f.data_off != 24 + 128 + type_cols * 8 + (int64_t)column_count * 8 + 1) return kStBadFixed;
   if ((int64_t)f.data_off + f.data_size > macro_size || occupy != f.data_off + f.data_size) return kStBadFixed;
   if ((int64_t)f.micro_count * 64 > f.data_size) return kStBadFixed;   // a micro-block is at least its 64-byte header
-  if (compressor != 1 /*NONE_COMPRESSOR*/ || encrypt_id != 0) return kStCompressed;
+  if ((compressor != OBGPU_COMPRESSOR_NONE && compressor != OBGPU_COMPRESSOR_LZ4 && compressor != OBGPU_COMPRESSOR_LZ4_1_9_1) || encrypt_id != 0)
+    return kStCompressed;
   return kStOk;
 }
 
@@ -80,6 +84,7 @@ __global__ void obgpu_macro_walk_kernel(const uint8_t *image, int64_t macro_size
     const uint32_t magic = (uint32_t)h[0] | ((uint32_t)h[1] << 8);
     const int64_t sz = (int64_t)ld32u(h + 4) + (int32_t)ld32u(h + 44);   // header_size_ + data_zlength_
     if (magic != 1005u || sz < 64 || at + sz > end) { ok = false; break; }
+    if (f.compressor == OBGPU_COMPRESSOR_NONE && ld32u(h + 40) != ld32u(h + 44)) { ok = false; break; }   // NONE: stored raw
     src_off[first[i] + k] = (int64_t)i * macro_size + at;
     sizes[first[i] + k] = sz;
     rows += ld32u(h + 16);
@@ -122,6 +127,9 @@ __global__ void __launch_bounds__(kCopyThreads) obgpu_macro_realign_kernel(const
 
 }  // namespace mb
 
+static int open_stored_blocks(obgpu_ctx *ctx, const uint8_t *d_image, int64_t image_size, const int64_t *d_src, const int64_t *d_zsize,
+                              int32_t n, int32_t compressor, obgpu_batch **out);   // lz4_blocks.cuh
+
 extern "C" {
 
 int obgpu_batch_open_macro_blocks(obgpu_ctx *ctx, const void *macro_image, int64_t image_size, int64_t macro_block_size, int32_t n_macro_blocks,
@@ -142,10 +150,10 @@ int obgpu_batch_open_macro_blocks(obgpu_ctx *ctx, const void *macro_image, int64
     return OBGPU_INVALID_ARGUMENT;
   }
   int ret = OBGPU_SUCCESS;
-  void *d_small = nullptr, *d_tab = nullptr, *d_out = nullptr;
+  void *d_small = nullptr, *d_tab = nullptr;
   std::vector<int32_t> counts((size_t)n_macro_blocks + 1);
-  std::vector<int64_t> first((size_t)n_macro_blocks + 1), src, sizes, dst;
-  int64_t n_micro = 0, out_bytes = 0;
+  std::vector<int64_t> first((size_t)n_macro_blocks + 1);
+  int64_t n_micro = 0;
   auto fail = [&](int code, const char *what) { if (what) ctx->err = what; ret = code; };
   do {
     if (cudaMallocAsync(&d_small, ((size_t)n_macro_blocks + 1) * 12 + 64, ctx->stream) != cudaSuccess) { fail(OBGPU_ALLOCATE_MEMORY_FAILED, "macro survey tables"); break; }
@@ -164,35 +172,24 @@ int obgpu_batch_open_macro_blocks(obgpu_ctx *ctx, const void *macro_image, int64
     for (int32_t i = 0; i < n_macro_blocks; ++i) { first[(size_t)i] = n_micro; n_micro += counts[(size_t)i]; }
     first[(size_t)n_macro_blocks] = n_micro;
     if (n_micro <= 0 || n_micro > 0x7fffffff) { fail(OBGPU_INVALID_DATA, "macro blocks hold no micro-block"); break; }
-    if (cudaMallocAsync(&d_tab, (size_t)n_micro * 24 + 64, ctx->stream) != cudaSuccess) { fail(OBGPU_ALLOCATE_MEMORY_FAILED, "micro-block tables"); break; }
-    int64_t *d_src = (int64_t *)d_tab, *d_sizes = d_src + n_micro, *d_dst = d_sizes + n_micro;
+    if (cudaMallocAsync(&d_tab, (size_t)n_micro * 16 + 64, ctx->stream) != cudaSuccess) { fail(OBGPU_ALLOCATE_MEMORY_FAILED, "micro-block tables"); break; }
+    int64_t *d_src = (int64_t *)d_tab, *d_sizes = d_src + n_micro;
     cudaMemcpyAsync(d_first, first.data(), ((size_t)n_macro_blocks + 1) * 8, cudaMemcpyHostToDevice, ctx->stream);
     mb::obgpu_macro_walk_kernel<<<(unsigned)((n_macro_blocks + 63) / 64), 64, 0, ctx->stream>>>(d_macro, macro_block_size, n_macro_blocks, d_first, d_src, d_sizes, d_status);
     ctx->launches++;
-    src.resize((size_t)n_micro); sizes.resize((size_t)n_micro); dst.resize((size_t)n_micro);
     int32_t st = 0;
-    if (cudaMemcpyAsync(sizes.data(), d_sizes, (size_t)n_micro * 8, cudaMemcpyDeviceToHost, ctx->stream) != cudaSuccess ||
-        cudaMemcpyAsync(&st, d_status, 4, cudaMemcpyDeviceToHost, ctx->stream) != cudaSuccess ||
+    if (cudaMemcpyAsync(&st, d_status, 4, cudaMemcpyDeviceToHost, ctx->stream) != cudaSuccess ||
         cudaStreamSynchronize(ctx->stream) != cudaSuccess) { fail(OBGPU_ERR_SYS, "macro walk"); break; }
     if (st != mb::kStOk) { fail(OBGPU_INVALID_DATA, "micro-block chain of a macro block is inconsistent"); break; }
-    for (int64_t k = 0; k < n_micro; ++k) { dst[(size_t)k] = out_bytes; out_bytes += (sizes[(size_t)k] + 127) & ~127ll; }
-    if (cudaMallocAsync(&d_out, (size_t)out_bytes + 64, ctx->stream) != cudaSuccess) { fail(OBGPU_ALLOCATE_MEMORY_FAILED, "realigned image"); break; }
-    cudaMemsetAsync((uint8_t *)d_out + out_bytes, 0, 64, ctx->stream);
-    cudaMemcpyAsync(d_dst, dst.data(), (size_t)n_micro * 8, cudaMemcpyHostToDevice, ctx->stream);
-    mb::obgpu_macro_realign_kernel<<<(unsigned)n_micro, mb::kCopyThreads, 0, ctx->stream>>>(d_macro, image_size, d_src, d_sizes, d_dst, (uint8_t *)d_out);
-    ctx->launches++;
-    if (cudaStreamSynchronize(ctx->stream) != cudaSuccess) { fail(OBGPU_ERR_SYS, "macro realign"); break; }   // dst (host vector) was the copy source
+    // NONE macro blocks were checked by the walk (every block raw); LZ4 admits raw and compressed blocks alike
     obgpu_batch *b = nullptr;
-    ret = obgpu_batch_open(ctx, d_out, out_bytes, dst.data(), sizes.data(), (int32_t)n_micro, 1, nullptr, &b);
+    ret = open_stored_blocks(ctx, d_macro, image_size, d_src, d_sizes, (int32_t)n_micro, OBGPU_COMPRESSOR_LZ4, &b);
     if (ret != OBGPU_SUCCESS) break;
-    b->own_image = true;   // the realigned image lives and dies with the batch
-    d_out = nullptr;
     *out = b;
     if (n_micro_out) *n_micro_out = (int32_t)n_micro;
   } while (0);
   if (d_small) cudaFreeAsync(d_small, ctx->stream);
   if (d_tab) cudaFreeAsync(d_tab, ctx->stream);
-  if (d_out) cudaFreeAsync(d_out, ctx->stream);
   if (tmp_image) cudaFreeAsync(tmp_image, ctx->stream);
   return ret;
 }

@@ -2426,10 +2426,27 @@ static_assert(sizeof(MacroFixedHeader) == 128, "FixedHeader is 128 bytes");
 int obgpu_writer_build_macro_blocks(const void *micro_image, const int64_t *offsets, const int64_t *sizes, int32_t n_blocks,
                                     const obgpu_macro_spec *spec, void *out, int64_t out_cap, int64_t *out_size, int32_t *n_macro,
                                     int32_t *first_micro, int32_t first_micro_cap) {
+  return obgpu_writer_build_macro_blocks_ex(micro_image, offsets, sizes, n_blocks, spec, out, out_cap, out_size, n_macro, first_micro,
+                                            first_micro_cap, OBGPU_COMPRESSOR_NONE);
+}
+
+int obgpu_writer_build_macro_blocks_ex(const void *micro_image, const int64_t *offsets, const int64_t *sizes, int32_t n_blocks,
+                                       const obgpu_macro_spec *spec, void *out, int64_t out_cap, int64_t *out_size, int32_t *n_macro,
+                                       int32_t *first_micro, int32_t first_micro_cap, int32_t compressor_type) {
   if (!micro_image || !offsets || !sizes || n_blocks <= 0 || !spec || !out || !out_size || !n_macro || spec->tablet_id == 0 ||
       spec->n_cols <= 0 || spec->rowkey_col_cnt < 0 || spec->rowkey_col_cnt > spec->n_cols || !spec->col_metas ||
       (spec->header_version != 1 && spec->header_version != 2) || spec->macro_block_size < 4096 || spec->macro_block_size > 0x7fffffffll)
     return OBGPU_INVALID_ARGUMENT;
+  if (compressor_type != OBGPU_COMPRESSOR_NONE && compressor_type != OBGPU_COMPRESSOR_LZ4 && compressor_type != OBGPU_COMPRESSOR_LZ4_1_9_1)
+    return OBGPU_NOT_SUPPORTED;
+  for (int32_t b = 0; b < n_blocks; ++b) {   // with NONE every micro-block must be stored raw
+    if (sizes[b] < 64 || offsets[b] < 0) return OBGPU_INVALID_ARGUMENT;
+    const uint8_t *mb = (const uint8_t *)micro_image + offsets[b];
+    int32_t len, zlen;
+    memcpy(&len, mb + 40, 4);
+    memcpy(&zlen, mb + 44, 4);
+    if (compressor_type == OBGPU_COMPRESSOR_NONE && len != zlen) return OBGPU_INVALID_ARGUMENT;
+  }
   const int64_t n_type_cols = spec->header_version == 2 ? spec->rowkey_col_cnt : spec->n_cols;
   // get_serialize_size: fixed header + ObObjMeta[] + ObOrderType[] + int64 checksum per column + is_normal_cg_
   const int64_t mh_size = (int64_t)sizeof(MacroFixedHeader) + n_type_cols * 4 + n_type_cols * 4 + (int64_t)spec->n_cols * 8 + 1;
@@ -2455,7 +2472,7 @@ int obgpu_writer_build_macro_blocks(const void *micro_image, const int64_t *offs
     fh.micro_block_data_offset_ = (int32_t)data_base;
     fh.encrypt_id_ = 0;
     fh.master_key_id_ = 0;   // the spec's store desc has no encryption (FixedHeader::reset leaves -1 only until init)
-    fh.compressor_type_ = 1;  // NONE_COMPRESSOR
+    fh.compressor_type_ = (uint8_t)compressor_type;   // ObCompressorType: the micro payloads are in stored form already
     int64_t len = data_base;
     uint64_t data_ck = 0;
     while (b < n_blocks) {
@@ -2523,6 +2540,147 @@ int obgpu_writer_stream_encode(int32_t type, int32_t width_bytes, const uint64_t
   if (!out) return OBGPU_SUCCESS;
   if ((int64_t)enc.size() > out_cap) return OBGPU_BUF_NOT_ENOUGH;
   if (!enc.empty()) memcpy(out, enc.data(), enc.size());
+  return OBGPU_SUCCESS;
+}
+
+}  // extern "C"
+
+// ---- LZ4 block format (lz4_Block_format.md): what ObLZ4Compressor::compress writes per micro-block payload -------------------
+// Greedy single-pass compressor: 4-byte hash -> last position (64 Ki entries), offsets below 64 KiB, no backward extension.
+// End-of-block rules of the format: the last 5 bytes are literals (a match ends at n - 5 at the latest) and the last match
+// starts at least 12 bytes before the end; the block ends with a literal-only sequence.
+namespace {
+inline uint32_t rd32le(const uint8_t *p) { uint32_t v; memcpy(&v, p, 4); return v; }
+
+void lz4_put_len(std::vector<uint8_t> &o, int64_t extra) {   // length extension: 255 ... 255, remainder
+  for (; extra >= 255; extra -= 255) o.push_back(255);
+  o.push_back((uint8_t)extra);
+}
+
+void lz4_compress_block(const uint8_t *src, int64_t n, std::vector<uint8_t> &o) {
+  constexpr int64_t kLastLiterals = 5, kMfLimit = 12, kMaxOffset = 65535;
+  o.clear();
+  o.reserve((size_t)(n + n / 255 + 16));
+  int64_t anchor = 0, ip = 0;
+  auto emit = [&](int64_t lit_end, int64_t offset, int64_t mlen) {   // mlen 0: the last, literal-only sequence
+    const int64_t lit = lit_end - anchor, ml = mlen ? mlen - 4 : 0;
+    o.push_back((uint8_t)((std::min<int64_t>(lit, 15) << 4) | std::min<int64_t>(ml, 15)));
+    if (lit >= 15) lz4_put_len(o, lit - 15);
+    o.insert(o.end(), src + anchor, src + lit_end);
+    if (!mlen) return;
+    o.push_back((uint8_t)(offset & 0xff));
+    o.push_back((uint8_t)(offset >> 8));
+    if (ml >= 15) lz4_put_len(o, ml - 15);
+  };
+  if (n > kMfLimit) {
+    std::vector<int32_t> table(1u << 16, -1);
+    const int64_t match_end_limit = n - kLastLiterals;
+    while (ip <= n - kMfLimit) {
+      const uint32_t seq = rd32le(src + ip);
+      const uint32_t h = (seq * 2654435761u) >> 16;
+      const int64_t ref = table[h];
+      table[h] = (int32_t)ip;
+      if (ref >= 0 && ip - ref <= kMaxOffset && rd32le(src + ref) == seq) {
+        int64_t len = 4;
+        while (ip + len < match_end_limit && src[ref + len] == src[ip + len]) ++len;
+        emit(ip, ip - ref, len);
+        ip += len;
+        anchor = ip;
+      } else {
+        ++ip;
+      }
+    }
+  }
+  emit(n, 0, 0);
+}
+
+// ObMicroBlockHeader header checksum (ob_micro_block_header.cpp:203-233) over the 64-byte header as stored
+int16_t micro_header_checksum(const uint8_t *p) {
+  int16_t cs = 0;
+  auto rd = [&](int off, int w) { int64_t v = 0; memcpy(&v, p + off, (size_t)w); return v; };
+  auto f64 = [&](int64_t v) { for (int k = 0; k < 4; ++k) cs = (int16_t)(cs ^ ((v >> (k * 16)) & 0xFFFF)); };
+  cs = (int16_t)(cs ^ (int16_t)rd(0, 2));     // magic_
+  cs = (int16_t)(cs ^ (int16_t)rd(2, 2));     // version_
+  cs = (int16_t)(cs ^ (int16_t)p[20]);        // row_store_type_
+  cs = (int16_t)(cs ^ (int16_t)p[21]);        // opt_
+  f64(rd(10, 2));                             // column_count_, rowkey_column_count_ (32-bit folds of 16-bit values)
+  f64(rd(12, 2));
+  f64(rd(14, 2) & 1);
+  f64(rd(22, 2));                             // opt2_
+  f64(rd(4, 4));                              // header_size_
+  f64(rd(16, 4));                             // row_count_
+  f64(rd(24, 4));                             // row_data_offset_
+  f64((int32_t)rd(28, 4));                    // original_length_
+  f64(rd(32, 8));                             // max_merged_trans_version_
+  f64((int32_t)rd(40, 4));                    // data_length_
+  f64((int32_t)rd(44, 4));                    // data_zlength_
+  f64(rd(48, 8));                             // data_checksum_
+  return cs;
+}
+}  // namespace
+
+extern "C" {
+
+int obgpu_writer_lz4_compress(const void *src, int64_t src_len, void *out, int64_t out_cap, int64_t *out_len) {
+  if ((!src && src_len > 0) || src_len < 0 || src_len > 0x7e000000ll || !out_len) return OBGPU_INVALID_ARGUMENT;
+  std::vector<uint8_t> o;
+  lz4_compress_block((const uint8_t *)src, src_len, o);
+  *out_len = (int64_t)o.size();
+  if (!out) return OBGPU_SUCCESS;
+  if ((int64_t)o.size() > out_cap) return OBGPU_BUF_NOT_ENOUGH;
+  memcpy(out, o.data(), o.size());
+  return OBGPU_SUCCESS;
+}
+
+int obgpu_writer_compress_blocks(const void *image, const int64_t *offsets, const int64_t *sizes, int32_t n_blocks, int32_t compressor,
+                                 int64_t align, void *out, int64_t out_cap, int64_t *out_offsets, int64_t *out_sizes,
+                                 int64_t *out_size) {
+  if (!image || !offsets || !sizes || n_blocks <= 0 || !out || !out_offsets || !out_sizes || !out_size || align < 1 ||
+      (align & (align - 1)) != 0)
+    return OBGPU_INVALID_ARGUMENT;
+  if (compressor != OBGPU_COMPRESSOR_NONE && compressor != OBGPU_COMPRESSOR_LZ4 && compressor != OBGPU_COMPRESSOR_LZ4_1_9_1)
+    return OBGPU_NOT_SUPPORTED;
+  const uint8_t *img = (const uint8_t *)image;
+  uint8_t *o = (uint8_t *)out;
+  std::vector<uint8_t> z;
+  int64_t at = 0;
+  for (int32_t b = 0; b < n_blocks; ++b) {
+    const uint8_t *blk = img + offsets[b];
+    uint32_t hs;
+    int32_t len, zlen;
+    if (sizes[b] < 64 || offsets[b] < 0) return OBGPU_INVALID_ARGUMENT;
+    memcpy(&hs, blk + 4, 4);
+    memcpy(&len, blk + 40, 4);
+    memcpy(&zlen, blk + 44, 4);
+    if (hs < 64 || len != zlen || (int64_t)hs + len != sizes[b]) return OBGPU_INVALID_DATA;   // plain, well-framed blocks only
+    at = (at + align - 1) & ~(align - 1);
+    bool keep_raw = compressor == OBGPU_COMPRESSOR_NONE;
+    if (!keep_raw) {
+      lz4_compress_block(blk + hs, len, z);
+      keep_raw = (int64_t)z.size() >= len;   // a block that does not shrink is stored raw (data_zlength_ == data_length_)
+    }
+    const int64_t stored = keep_raw ? sizes[b] : (int64_t)hs + (int64_t)z.size();
+    if (at + stored > out_cap) return OBGPU_BUF_NOT_ENOUGH;
+    uint8_t *d = o + at;
+    memcpy(d, blk, hs);
+    if (keep_raw) {
+      memcpy(d + hs, blk + hs, (size_t)len);
+    } else {
+      memcpy(d + hs, z.data(), z.size());
+      const int32_t zl = (int32_t)z.size();
+      const int64_t ck = (int64_t)crc32c_update(0, z.data(), z.size());   // data_checksum_: crc over the stored bytes
+      memcpy(d + 44, &zl, 4);
+      memcpy(d + 48, &ck, 8);
+      int16_t zero = 0;
+      memcpy(d + 8, &zero, 2);
+      const int16_t hc = micro_header_checksum(d);
+      memcpy(d + 8, &hc, 2);
+    }
+    out_offsets[b] = at;
+    out_sizes[b] = stored;
+    at += stored;
+  }
+  *out_size = at;
   return OBGPU_SUCCESS;
 }
 

@@ -123,8 +123,8 @@ class ScanContext:
         return (lib.obgpu_ctx_last_error(self._h) or b"").decode()
 
     def open_batch(self, table, device_image_ptr: Optional[int] = None, host_view: bool = True,
-                   image_size: Optional[int] = None) -> "PageBatch":
-        return PageBatch(self, table, device_image_ptr, host_view, image_size)
+                   image_size: Optional[int] = None, compressor: Optional[int] = None) -> "PageBatch":
+        return PageBatch(self, table, device_image_ptr, host_view, image_size, compressor)
 
     def bitmap_to_row_ids(self, bitmap: np.ndarray, start: int, to: int, limit: int, id_offset: int = 0):
         """common::ObBitmap::get_row_ids. Returns (row_ids, next_from)."""
@@ -151,16 +151,28 @@ class PageBatch:
     """obgpu_batch: N micro-blocks resident in HBM."""
 
     def __init__(self, ctx: ScanContext, table, device_image_ptr: Optional[int] = None, host_view: bool = True,
-                 image_size: Optional[int] = None):
+                 image_size: Optional[int] = None, compressor: Optional[int] = None):
         """host_view=False: a device-resident image is opened without a host copy of it (table.image may then be
-        None; the headers are surveyed on the device)."""
+        None; the headers are surveyed on the device).
+        compressor (capi.COMPRESSOR_*): the blocks of `table` are in stored form (sstable.compress_table) and are decoded on
+        the device by obgpu_batch_open_compressed into an image the batch owns (device_image()); None: plain blocks."""
         self.ctx = ctx
         self.table = table
         self._h = C.c_void_p()
         img = table.image
         offs = np.ascontiguousarray(table.offsets, dtype=np.int64)
         sizes = np.ascontiguousarray(table.sizes, dtype=np.int64)
-        if device_image_ptr is None:
+        if compressor is not None:
+            if device_image_ptr is None:
+                img = np.ascontiguousarray(img, dtype=np.uint8)
+                code = lib.obgpu_batch_open_compressed(ctx._h, img.ctypes.data, img.size, offs.ctypes.data, sizes.ctypes.data,
+                                                       len(offs), 0, int(compressor), C.byref(self._h))
+            else:
+                size = int(image_size) if image_size is not None else img.size
+                code = lib.obgpu_batch_open_compressed(ctx._h, C.c_void_p(device_image_ptr), size, offs.ctypes.data,
+                                                       sizes.ctypes.data, len(offs), 1, int(compressor), C.byref(self._h))
+            check(code, "obgpu_batch_open_compressed", ctx._h)
+        elif device_image_ptr is None:
             code = lib.obgpu_batch_open(ctx._h, img.ctypes.data, img.size, offs.ctypes.data, sizes.ctypes.data,
                                         len(offs), 0, None, C.byref(self._h))
         else:
@@ -168,7 +180,8 @@ class PageBatch:
             code = lib.obgpu_batch_open(ctx._h, C.c_void_p(device_image_ptr), size, offs.ctypes.data,
                                         sizes.ctypes.data, len(offs), 1,
                                         img.ctypes.data if (host_view and img is not None) else None, C.byref(self._h))
-        check(code, "obgpu_batch_open", ctx._h)
+        if compressor is None:
+            check(code, "obgpu_batch_open", ctx._h)
         self.n_blocks = len(offs)
         tr = C.c_int64(0)
         check(lib.obgpu_batch_total_rows(self._h, C.byref(tr)), "obgpu_batch_total_rows", ctx._h)
@@ -197,6 +210,13 @@ class PageBatch:
         check(lib.obgpu_batch_total_rows(self._h, C.byref(tr)), "obgpu_batch_total_rows", ctx._h)
         self.total_rows = tr.value
         return self
+
+    def device_image(self):
+        """(device address, bytes) of the image the batch's blocks live in (obgpu_batch_device_image). For a batch that owns
+        its image (host image, macro blocks, compressed blocks) scan(string_base=device_image()[0]) yields device addresses."""
+        p, n = C.c_void_p(), C.c_int64(0)
+        check(lib.obgpu_batch_device_image(self._h, C.byref(p), C.byref(n)), "obgpu_batch_device_image", self.ctx._h)
+        return p.value or 0, n.value
 
     def block_info(self, i):
         rc, cc = C.c_int64(0), C.c_int32(0)

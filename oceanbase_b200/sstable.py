@@ -144,8 +144,12 @@ class MacroImage:
 
 def build_macro_blocks(table: TableImage, col_types: Sequence[int], rowkey_cnt: int, tablet_id: int = 200001, logical_version: int = 1,
                        first_data_seq: int = 0, header_version: int = 1, is_cg: bool = False, macro_block_size: int = 2 << 20,
-                       col_orders: Optional[Sequence[int]] = None) -> MacroImage:
-    """ObMacroBlock::write_micro_block / write_macro_header over the micro-blocks of `table`."""
+                       col_orders: Optional[Sequence[int]] = None, compressor: Optional[int] = None) -> MacroImage:
+    """ObMacroBlock::write_micro_block / write_macro_header over the micro-blocks of `table`.
+    compressor (capi.COMPRESSOR_*): the plain blocks are compressed first (compress_table) and the macro headers record it."""
+    if compressor is not None and compressor != capi.COMPRESSOR_NONE:
+        table = compress_table(table, compressor)
+    comp = capi.COMPRESSOR_NONE if compressor is None else int(compressor)
     n_cols = len(col_types)
     metas = np.zeros((n_cols, 4), dtype=np.uint8)
     metas[:, 0] = col_types
@@ -161,10 +165,39 @@ def build_macro_blocks(table: TableImage, col_types: Sequence[int], rowkey_cnt: 
     out = np.zeros(min(est, table.n_blocks) * macro_block_size, dtype=np.uint8)
     first = np.zeros(table.n_blocks + 1, dtype=np.int32)
     size, nm = C.c_int64(0), C.c_int32(0)
-    check(lib.obgpu_writer_build_macro_blocks(img.ctypes.data, off.ctypes.data, sz.ctypes.data, table.n_blocks, C.byref(spec),
-                                              out.ctypes.data, out.size, C.byref(size), C.byref(nm), first.ctypes.data, first.size),
-          "obgpu_writer_build_macro_blocks")
+    check(lib.obgpu_writer_build_macro_blocks_ex(img.ctypes.data, off.ctypes.data, sz.ctypes.data, table.n_blocks, C.byref(spec),
+                                                 out.ctypes.data, out.size, C.byref(size), C.byref(nm), first.ctypes.data, first.size,
+                                                 comp), "obgpu_writer_build_macro_blocks_ex")
     return MacroImage(out[:size.value], macro_block_size, nm.value, first[:nm.value + 1].copy())
+
+
+# ---- compressed micro-blocks (ObMicroBlockCompressor: plain header, payload compressed on its own) ----------------------------
+def lz4_compress(data) -> np.ndarray:
+    """One LZ4 block (block format, no frame) of `data` by the writer's compressor."""
+    src = np.ascontiguousarray(np.frombuffer(bytes(data), dtype=np.uint8) if not isinstance(data, np.ndarray) else data, dtype=np.uint8)
+    n = C.c_int64(0)
+    check(lib.obgpu_writer_lz4_compress(src.ctypes.data, src.size, None, 0, C.byref(n)), "obgpu_writer_lz4_compress(size)")
+    out = np.zeros(max(n.value, 1), dtype=np.uint8)
+    check(lib.obgpu_writer_lz4_compress(src.ctypes.data, src.size, out.ctypes.data, out.size, C.byref(n)), "obgpu_writer_lz4_compress")
+    return out[:n.value]
+
+
+def compress_table(table: TableImage, compressor: int, align: int = 1) -> TableImage:
+    """The blocks of `table` in stored form: each payload compressed with `compressor` (capi.COMPRESSOR_*) and kept raw when
+    that is not smaller (data_zlength_, data_checksum_ and the header checksum follow). align=1: blocks back to back, at any
+    byte offset, as inside a macro block."""
+    img = np.ascontiguousarray(table.image)
+    off = np.ascontiguousarray(table.offsets, dtype=np.int64)
+    sz = np.ascontiguousarray(table.sizes, dtype=np.int64)
+    cap = int(((sz + align - 1) // align * align).sum()) + align
+    out = np.zeros(cap, dtype=np.uint8)
+    o_off = np.zeros(table.n_blocks, dtype=np.int64)
+    o_sz = np.zeros(table.n_blocks, dtype=np.int64)
+    used = C.c_int64(0)
+    check(lib.obgpu_writer_compress_blocks(img.ctypes.data, off.ctypes.data, sz.ctypes.data, table.n_blocks, int(compressor), align,
+                                           out.ctypes.data, out.size, o_off.ctypes.data, o_sz.ctypes.data, C.byref(used)),
+          "obgpu_writer_compress_blocks")
+    return TableImage(out[:used.value], o_off, o_sz, table.total_rows, table.n_cols)
 
 
 # ---- skip index: aggregate rows (include/obgpu_skip_index.h) -------------------------------------------------
