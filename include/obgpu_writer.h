@@ -125,8 +125,8 @@ int obgpu_writer_build_macro_blocks(const void *micro_image, const int64_t *offs
                                     int32_t *n_macro, int32_t *first_micro, int32_t first_micro_cap);
 /* The same with the FixedHeader's compressor_type_ (OBGPU_COMPRESSOR_*). The micro-blocks are taken as they are, in stored
  * form (obgpu_writer_compress_blocks): a macro block records the compressor, it does not apply it. With NONE every block must
- * have data_zlength_ == data_length_ (OBGPU_INVALID_ARGUMENT otherwise); other compressors: OBGPU_NOT_SUPPORTED.
- * obgpu_writer_build_macro_blocks is this call with OBGPU_COMPRESSOR_NONE. */
+ * have data_zlength_ == data_length_ (OBGPU_INVALID_ARGUMENT otherwise); LZ4 / LZ4_1_9_1 / ZSTD_1_3_8 record that compressor;
+ * other compressors: OBGPU_NOT_SUPPORTED. obgpu_writer_build_macro_blocks is this call with OBGPU_COMPRESSOR_NONE. */
 int obgpu_writer_build_macro_blocks_ex(const void *micro_image, const int64_t *offsets, const int64_t *sizes, int32_t n_blocks,
                                        const obgpu_macro_spec *spec, void *out, int64_t out_cap, int64_t *out_size,
                                        int32_t *n_macro, int32_t *first_micro, int32_t first_micro_cap, int32_t compressor_type);
@@ -139,8 +139,13 @@ int obgpu_writer_build_macro_blocks_ex(const void *micro_image, const int64_t *o
 /* One LZ4 block (lz4 block format: no frame, no size prefix; what LZ4_compress_default's output decodes like): greedy, 64 KiB
  * window, end-of-block rules of the format kept. out == NULL: only *out_len (never more than src_len + src_len / 255 + 16). */
 int obgpu_writer_lz4_compress(const void *src, int64_t src_len, void *out, int64_t out_cap, int64_t *out_len);
+/* One zstd frame (RFC 8878; what ZSTD_decompressDCtx and ObZstdCompressor_1_3_8::decompress read): Single_Segment with
+ * Frame_Content_Size, no checksum, no dictionary; blocks of <= 128 KiB matched by the LZ4 compressor's greedy matcher; Raw
+ * literals; sequences in Predefined mode (FSE from the RFC's default distributions); a block that does not shrink is a Raw
+ * block. out == NULL: only *out_len (never more than src_len + 3 * (src_len / 128 KiB + 1) + 13). */
+int obgpu_writer_zstd_compress(const void *src, int64_t src_len, void *out, int64_t out_cap, int64_t *out_len);
 /* Re-frames n plain micro-blocks (data_zlength_ == data_length_) into stored form with `compressor` (OBGPU_COMPRESSOR_LZ4 /
- * LZ4_1_9_1; NONE copies): the payload is compressed and kept raw when that is not smaller; a compressed block gets
+ * LZ4_1_9_1: an LZ4 block; ZSTD_1_3_8: a zstd frame, obgpu_writer_zstd_compress; NONE copies): the payload is compressed and kept raw when that is not smaller; a compressed block gets
  * data_zlength_, data_checksum_ (crc32c of the stored bytes) and a recomputed header checksum. Block i goes to
  * out[out_offsets[i], out_offsets[i] + out_sizes[i]), offsets multiples of align (a power of two; 1: back to back).
  * out_cap >= sum over i of (sizes[i] rounded up to align) always suffices; *out_size = bytes used. */

@@ -186,6 +186,30 @@ __global__ void __launch_bounds__(kWarps * 32) obgpu_lz4_blocks_kernel(const uin
 
 }  // namespace lz4dev
 
+static void launch_zstd_blocks(obgpu_ctx *ctx, bool blocks, const uint8_t *in, const int64_t *in_off, const int64_t *in_len, uint8_t *out,
+                               const int64_t *out_off, const int64_t *out_len, int32_t n, int32_t *blk_status,
+                               int32_t *any_status);   // zstd_blocks.cuh
+
+static void launch_decode(obgpu_ctx *ctx, int32_t compressor, bool blocks, const uint8_t *in, const int64_t *in_off, const int64_t *in_len,
+                          uint8_t *out, const int64_t *out_off, const int64_t *out_len, int32_t n, int32_t *blk_status, int32_t *any_status) {
+  if (compressor == OBGPU_COMPRESSOR_ZSTD_1_3_8) {
+    launch_zstd_blocks(ctx, blocks, in, in_off, in_len, out, out_off, out_len, n, blk_status, any_status);
+    return;
+  }
+  const unsigned grid = (unsigned)((n + lz4dev::kWarps - 1) / lz4dev::kWarps);
+  if (blocks)
+    lz4dev::obgpu_lz4_blocks_kernel<true><<<grid, lz4dev::kWarps * 32, 0, ctx->stream>>>(in, in_off, in_len, out, out_off, out_len, n,
+                                                                                        blk_status, any_status);
+  else
+    lz4dev::obgpu_lz4_blocks_kernel<false><<<grid, lz4dev::kWarps * 32, 0, ctx->stream>>>(in, in_off, in_len, out, out_off, out_len, n,
+                                                                                         blk_status, any_status);
+  ctx->launches++;
+}
+
+static bool device_compressor(int32_t c) {
+  return c == OBGPU_COMPRESSOR_NONE || c == OBGPU_COMPRESSOR_LZ4 || c == OBGPU_COMPRESSOR_LZ4_1_9_1 || c == OBGPU_COMPRESSOR_ZSTD_1_3_8;
+}
+
 // Stored micro-blocks d_image[d_src[i], + d_zsize[i]) (device tables) -> page batch owning the decoded, realigned image.
 // The one routine behind obgpu_batch_open_macro_blocks and obgpu_batch_open_compressed.
 static int open_stored_blocks(obgpu_ctx *ctx, const uint8_t *d_image, int64_t image_size, const int64_t *d_src, const int64_t *d_zsize,
@@ -246,17 +270,16 @@ static int open_stored_blocks(obgpu_ctx *ctx, const uint8_t *d_image, int64_t im
                                                                                          (uint8_t *)d_out);
       ctx->launches++;
     }
-    if (nz) {
-      lz4dev::obgpu_lz4_blocks_kernel<true><<<(unsigned)((nz + lz4dev::kWarps - 1) / lz4dev::kWarps), lz4dev::kWarps * 32, 0, ctx->stream>>>(
-          d_image, d_lz, d_lz + nz, (uint8_t *)d_out, d_lz + 2 * nz, d_lz + 3 * nz, (int32_t)nz, d_blk_status, d_status);
-      ctx->launches++;
-    }
+    if (nz)
+      launch_decode(ctx, compressor, true, d_image, d_lz, d_lz + nz, (uint8_t *)d_out, d_lz + 2 * nz, d_lz + 3 * nz, (int32_t)nz, d_blk_status,
+                    d_status);
     // the host tables were copy sources: synchronise before they go out of scope
     if (cudaGetLastError() != cudaSuccess || cudaMemcpyAsync(&st, d_status, 4, cudaMemcpyDeviceToHost, ctx->stream) != cudaSuccess ||
         cudaStreamSynchronize(ctx->stream) != cudaSuccess) { fail(OBGPU_ERR_SYS, "stored-block decode"); break; }
     if (st != lz4dev::kStOk) {
       fail(OBGPU_INVALID_DATA, st == lz4dev::kStBadChecksum ? "checksum of a compressed micro-block does not match"
-                                                            : "LZ4 payload of a micro-block is malformed");
+                               : compressor == OBGPU_COMPRESSOR_ZSTD_1_3_8 ? "zstd payload of a micro-block is malformed"
+                                                                           : "LZ4 payload of a micro-block is malformed");
       break;
     }
     obgpu_batch *b = nullptr;
@@ -277,7 +300,7 @@ extern "C" {
 int obgpu_batch_open_compressed(obgpu_ctx *ctx, const void *image, int64_t image_size, const int64_t *offsets, const int64_t *sizes,
                                 int32_t n_blocks, int32_t image_on_device, int32_t compressor_type, obgpu_batch **out) {
   if (!ctx || !image || !offsets || !sizes || !out || n_blocks <= 0 || image_size <= 0) return OBGPU_INVALID_ARGUMENT;
-  if (compressor_type != OBGPU_COMPRESSOR_NONE && compressor_type != OBGPU_COMPRESSOR_LZ4 && compressor_type != OBGPU_COMPRESSOR_LZ4_1_9_1) {
+  if (!device_compressor(compressor_type)) {
     ctx->err = "compressor not handled by the device path";
     return OBGPU_NOT_SUPPORTED;
   }
@@ -326,8 +349,11 @@ int obgpu_batch_device_image(const obgpu_batch *batch, const void **image, int64
   return OBGPU_SUCCESS;
 }
 
-int obgpu_lz4_decompress(obgpu_ctx *ctx, const void *d_in, const int64_t *in_off, const int64_t *in_len, void *d_out, const int64_t *out_off,
-                         const int64_t *out_len, int32_t n, int32_t *status) {
+}  // extern "C"
+
+// n independent streams of one codec in device memory (obgpu_lz4_decompress, obgpu_zstd_decompress)
+static int decompress_streams(obgpu_ctx *ctx, const void *d_in, const int64_t *in_off, const int64_t *in_len, void *d_out, const int64_t *out_off,
+                              const int64_t *out_len, int32_t n, int32_t *status, int32_t compressor) {
   if (!ctx || !d_in || !in_off || !in_len || !d_out || !out_off || !out_len || n <= 0 || !status) return OBGPU_INVALID_ARGUMENT;
   for (int32_t i = 0; i < n; ++i)
     if (in_off[i] < 0 || in_len[i] < 0 || out_off[i] < 0 || out_len[i] < 0) return OBGPU_INVALID_ARGUMENT;
@@ -340,22 +366,30 @@ int obgpu_lz4_decompress(obgpu_ctx *ctx, const void *d_in, const int64_t *in_off
   memcpy(tab.data() + 2 * (size_t)n, out_off, (size_t)n * 8);
   memcpy(tab.data() + 3 * (size_t)n, out_len, (size_t)n * 8);
   do {
-    if (cudaMallocAsync(&d_tab, (size_t)n * 36 + 64, ctx->stream) != cudaSuccess) { ctx->err = "lz4 tables"; ret = OBGPU_ALLOCATE_MEMORY_FAILED; break; }
+    if (cudaMallocAsync(&d_tab, (size_t)n * 36 + 64, ctx->stream) != cudaSuccess) { ctx->err = "stream tables"; ret = OBGPU_ALLOCATE_MEMORY_FAILED; break; }
     int64_t *d = (int64_t *)d_tab;
     int32_t *d_st = (int32_t *)(d + 4 * (size_t)n), *d_any = d_st + n;
     cudaMemcpyAsync(d, tab.data(), (size_t)n * 32, cudaMemcpyHostToDevice, ctx->stream);
     cudaMemsetAsync(d_any, 0, 4, ctx->stream);
-    lz4dev::obgpu_lz4_blocks_kernel<false><<<(unsigned)((n + lz4dev::kWarps - 1) / lz4dev::kWarps), lz4dev::kWarps * 32, 0, ctx->stream>>>(
-        (const uint8_t *)d_in, d, d + n, (uint8_t *)d_out, d + 2 * n, d + 3 * n, n, d_st, d_any);
-    ctx->launches++;
+    launch_decode(ctx, compressor, false, (const uint8_t *)d_in, d, d + n, (uint8_t *)d_out, d + 2 * n, d + 3 * n, n, d_st, d_any);
     int32_t any = 0;
     if (cudaGetLastError() != cudaSuccess || cudaMemcpyAsync(status, d_st, (size_t)n * 4, cudaMemcpyDeviceToHost, ctx->stream) != cudaSuccess ||
         cudaMemcpyAsync(&any, d_any, 4, cudaMemcpyDeviceToHost, ctx->stream) != cudaSuccess ||
-        cudaStreamSynchronize(ctx->stream) != cudaSuccess) { ctx->err = "lz4 decode"; ret = OBGPU_ERR_SYS; break; }
-    if (any != lz4dev::kStOk) { ctx->err = "an LZ4 block is malformed"; ret = OBGPU_INVALID_DATA; }
+        cudaStreamSynchronize(ctx->stream) != cudaSuccess) { ctx->err = "stream decode"; ret = OBGPU_ERR_SYS; break; }
+    if (any != lz4dev::kStOk) {
+      ctx->err = compressor == OBGPU_COMPRESSOR_ZSTD_1_3_8 ? "a zstd frame is malformed" : "an LZ4 block is malformed";
+      ret = OBGPU_INVALID_DATA;
+    }
   } while (0);
   if (d_tab) cudaFreeAsync(d_tab, ctx->stream);
   return ret;
+}
+
+extern "C" {
+
+int obgpu_lz4_decompress(obgpu_ctx *ctx, const void *d_in, const int64_t *in_off, const int64_t *in_len, void *d_out, const int64_t *out_off,
+                         const int64_t *out_len, int32_t n, int32_t *status) {
+  return decompress_streams(ctx, d_in, in_off, in_len, d_out, out_off, out_len, n, status, OBGPU_COMPRESSOR_LZ4);
 }
 
 }  // extern "C"

@@ -7,9 +7,10 @@
 //             micro_block_data_offset_; the walk must end at micro_block_data_offset_ + micro_block_data_size_ with row_count_ rows
 //   realign : one CTA per micro-block copies it to a 128-byte aligned slot of a new image (unaligned source words through
 //             funnel shifts, 16-byte stores, zero padding) -- one read + one write of the data, at HBM speed, once per cache fill
-// Macro blocks whose compressor_type_ is LZ4 / LZ4_1_9_1 hold micro-blocks in stored form: the walk's (offset, stored size)
-// pairs go to open_stored_blocks (lz4_blocks.cuh), which decodes the compressed ones into their slots and realigns the raw
-// ones with the kernel below. 16 bytes per micro-block (offset, size) and 4 per macro block come back to the host for
+// Macro blocks whose compressor_type_ is LZ4 / LZ4_1_9_1 / ZSTD_1_3_8 hold micro-blocks in stored form: the walk's (offset,
+// stored size) pairs go to open_stored_blocks (lz4_blocks.cuh), which decodes the compressed ones into their slots and
+// realigns the raw ones with the kernel below; the survey reports each macro block's compressor, and the ones of one open
+// must agree. 16 bytes per micro-block (offset, size) and 4 per macro block come back to the host for
 // obgpu_batch_open's tables; the block bytes never touch the CPU. Other compressors and encrypted blocks are refused.
 #pragma once
 
@@ -53,17 +54,20 @@ __device__ __forceinline__ int32_t parse_headers(const uint8_t *m, int64_t macro
   if (f.data_off != 24 + 128 + type_cols * 8 + (int64_t)column_count * 8 + 1) return kStBadFixed;
   if ((int64_t)f.data_off + f.data_size > macro_size || occupy != f.data_off + f.data_size) return kStBadFixed;
   if ((int64_t)f.micro_count * 64 > f.data_size) return kStBadFixed;   // a micro-block is at least its 64-byte header
-  if ((compressor != OBGPU_COMPRESSOR_NONE && compressor != OBGPU_COMPRESSOR_LZ4 && compressor != OBGPU_COMPRESSOR_LZ4_1_9_1) || encrypt_id != 0)
+  if ((compressor != OBGPU_COMPRESSOR_NONE && compressor != OBGPU_COMPRESSOR_LZ4 && compressor != OBGPU_COMPRESSOR_LZ4_1_9_1 &&
+       compressor != OBGPU_COMPRESSOR_ZSTD_1_3_8) || encrypt_id != 0)
     return kStCompressed;
   return kStOk;
 }
 
-__global__ void obgpu_macro_survey_kernel(const uint8_t *image, int64_t macro_size, int32_t n_macro, int32_t *counts, int32_t *status) {
+__global__ void obgpu_macro_survey_kernel(const uint8_t *image, int64_t macro_size, int32_t n_macro, int32_t *counts, int32_t *comps,
+                                          int32_t *status) {
   const int32_t i = (int32_t)(blockIdx.x * blockDim.x + threadIdx.x);
   if (i >= n_macro) return;
   Fixed f;
   const int32_t st = parse_headers(image + (int64_t)i * macro_size, macro_size, f);
   counts[i] = st == kStOk ? f.micro_count : 0;
+  comps[i] = st == kStOk ? f.compressor : 0;
   if (st != kStOk) atomicMax(status, st);
 }
 
@@ -128,7 +132,7 @@ __global__ void __launch_bounds__(kCopyThreads) obgpu_macro_realign_kernel(const
 }  // namespace mb
 
 static int open_stored_blocks(obgpu_ctx *ctx, const uint8_t *d_image, int64_t image_size, const int64_t *d_src, const int64_t *d_zsize,
-                              int32_t n, int32_t compressor, obgpu_batch **out);   // lz4_blocks.cuh
+                              int32_t n, int32_t compressor, obgpu_batch **out);   // lz4_blocks.cuh (decoders: lz4 / zstd_blocks.cuh)
 
 extern "C" {
 
@@ -151,24 +155,38 @@ int obgpu_batch_open_macro_blocks(obgpu_ctx *ctx, const void *macro_image, int64
   }
   int ret = OBGPU_SUCCESS;
   void *d_small = nullptr, *d_tab = nullptr;
-  std::vector<int32_t> counts((size_t)n_macro_blocks + 1);
+  std::vector<int32_t> counts((size_t)n_macro_blocks + 1), comps((size_t)n_macro_blocks);
   std::vector<int64_t> first((size_t)n_macro_blocks + 1);
   int64_t n_micro = 0;
   auto fail = [&](int code, const char *what) { if (what) ctx->err = what; ret = code; };
   do {
-    if (cudaMallocAsync(&d_small, ((size_t)n_macro_blocks + 1) * 12 + 64, ctx->stream) != cudaSuccess) { fail(OBGPU_ALLOCATE_MEMORY_FAILED, "macro survey tables"); break; }
+    // [counts i32 x n][status i32][first i64 x (n + 1), 16-byte aligned][compressor i32 x n]
+    const size_t first_at = (((size_t)n_macro_blocks + 1) * 4 + 15) / 16 * 16, comps_at = first_at + ((size_t)n_macro_blocks + 1) * 8;
+    if (cudaMallocAsync(&d_small, comps_at + (size_t)n_macro_blocks * 4 + 64, ctx->stream) != cudaSuccess) { fail(OBGPU_ALLOCATE_MEMORY_FAILED, "macro survey tables"); break; }
     int32_t *d_counts = (int32_t *)d_small, *d_status = d_counts + n_macro_blocks;
-    int64_t *d_first = (int64_t *)((uint8_t *)d_small + (((size_t)n_macro_blocks + 1) * 4 + 15) / 16 * 16);
+    int64_t *d_first = (int64_t *)((uint8_t *)d_small + first_at);
+    int32_t *d_comps = (int32_t *)((uint8_t *)d_small + comps_at);
     cudaMemsetAsync(d_status, 0, 4, ctx->stream);
-    mb::obgpu_macro_survey_kernel<<<(unsigned)((n_macro_blocks + 127) / 128), 128, 0, ctx->stream>>>(d_macro, macro_block_size, n_macro_blocks, d_counts, d_status);
+    mb::obgpu_macro_survey_kernel<<<(unsigned)((n_macro_blocks + 127) / 128), 128, 0, ctx->stream>>>(d_macro, macro_block_size, n_macro_blocks, d_counts,
+                                                                                                     d_comps, d_status);
     ctx->launches++;
     if (cudaMemcpyAsync(counts.data(), d_counts, ((size_t)n_macro_blocks + 1) * 4, cudaMemcpyDeviceToHost, ctx->stream) != cudaSuccess ||
+        cudaMemcpyAsync(comps.data(), d_comps, (size_t)n_macro_blocks * 4, cudaMemcpyDeviceToHost, ctx->stream) != cudaSuccess ||
         cudaStreamSynchronize(ctx->stream) != cudaSuccess) { fail(OBGPU_ERR_SYS, "macro survey"); break; }
     if (counts[(size_t)n_macro_blocks] != mb::kStOk) {
       fail(counts[(size_t)n_macro_blocks] == mb::kStCompressed ? OBGPU_NOT_SUPPORTED : OBGPU_INVALID_DATA,
            counts[(size_t)n_macro_blocks] == mb::kStCompressed ? "compressed or encrypted macro block" : "macro block header is invalid");
       break;
     }
+    // one SSTable has one compressor: the macro blocks that are not NONE must agree (NONE ones hold raw blocks only)
+    int32_t compressor = OBGPU_COMPRESSOR_NONE;
+    bool mixed = false;
+    for (int32_t c : comps)
+      if (c != OBGPU_COMPRESSOR_NONE) {
+        mixed = mixed || (compressor != OBGPU_COMPRESSOR_NONE && c != compressor);
+        compressor = c;
+      }
+    if (mixed) { fail(OBGPU_NOT_SUPPORTED, "macro blocks of one open use different compressors"); break; }
     for (int32_t i = 0; i < n_macro_blocks; ++i) { first[(size_t)i] = n_micro; n_micro += counts[(size_t)i]; }
     first[(size_t)n_macro_blocks] = n_micro;
     if (n_micro <= 0 || n_micro > 0x7fffffff) { fail(OBGPU_INVALID_DATA, "macro blocks hold no micro-block"); break; }
@@ -181,9 +199,9 @@ int obgpu_batch_open_macro_blocks(obgpu_ctx *ctx, const void *macro_image, int64
     if (cudaMemcpyAsync(&st, d_status, 4, cudaMemcpyDeviceToHost, ctx->stream) != cudaSuccess ||
         cudaStreamSynchronize(ctx->stream) != cudaSuccess) { fail(OBGPU_ERR_SYS, "macro walk"); break; }
     if (st != mb::kStOk) { fail(OBGPU_INVALID_DATA, "micro-block chain of a macro block is inconsistent"); break; }
-    // NONE macro blocks were checked by the walk (every block raw); LZ4 admits raw and compressed blocks alike
+    // NONE macro blocks were checked by the walk (every block raw); the others admit raw and compressed blocks alike
     obgpu_batch *b = nullptr;
-    ret = open_stored_blocks(ctx, d_macro, image_size, d_src, d_sizes, (int32_t)n_micro, OBGPU_COMPRESSOR_LZ4, &b);
+    ret = open_stored_blocks(ctx, d_macro, image_size, d_src, d_sizes, (int32_t)n_micro, compressor, &b);
     if (ret != OBGPU_SUCCESS) break;
     *out = b;
     if (n_micro_out) *n_micro_out = (int32_t)n_micro;

@@ -3660,6 +3660,7 @@ int obgpu_project_datums(obgpu_batch *batch, int32_t block, int32_t col, const i
 #include "merge_streamed.cuh"
 #include "encode_kernels.cuh"   // phase B: merged columns -> SSTable bytes + column checksums
 #include "lz4_blocks.cuh"       // LZ4-compressed micro-blocks decoded at open (page batches, macro blocks)
+#include "zstd_blocks.cuh"      // zstd-compressed micro-blocks: the decoder behind the same open
 
 // ---- host-buffer scan pipeline (include/obgpu_pipeline.h) ------------------------------------------------
 #include "host_pipeline.h"

@@ -1,4 +1,5 @@
-"""Cost of opening LZ4-compressed micro-blocks on the device vs opening the plain image of the same table.
+"""Cost of opening LZ4-compressed (default) or zstd-compressed (--compressor zstd) micro-blocks on the device vs opening the
+plain image of the same table.
 
 Table: seeded RAW int64 key + RAW small ints + RAW 9-byte strings, ~1 GB plain (the writer's LZ4 stores it ~1.5x smaller).
 Measured with CUDA events on the ctx stream (median of --reps after one warm-up), for
@@ -7,7 +8,12 @@ Measured with CUDA events on the ctx stream (median of --reps after one warm-up)
   kernel : obgpu_lz4_decompress over the compressed payloads alone (decoded GB/s from the block sizes; no checksum)
 and the H2D bytes of each host open. The question: opening from host memory, do the H2D bytes saved pay for the decode?
 
-  python tools/bench_decompress.py [--rows N] [--reps R] [--out FILE]
+--compressor zstd (compressor 6, zstd_1.3.8; default --rows 8M): the same opens for blocks from the writer's zstd compressor
+and from libzstd at levels 1 and 3 (libzstd.so.1 through ctypes), obgpu_zstd_decompress alone on each, the ratios, and a
+CPU baseline: libzstd's ZSTD_decompressDCtx over the same payloads on --cpu-threads threads (one call per micro-block, what
+the reference does), timed with a host clock.
+
+  python tools/bench_decompress.py [--compressor lz4|zstd] [--rows N] [--reps R] [--cpu-threads T] [--out FILE]
 """
 import argparse
 import ctypes as C
@@ -66,13 +72,138 @@ def timed(fn, reps):
     return float(np.median(out))
 
 
+def stored_sizes(stored):
+    zl = stored.image.view(np.uint8)
+    zlen = np.array([int(zl[o + 44:o + 48].view(np.int32)[0]) for o in stored.offsets], dtype=np.int64)
+    dlen = np.array([int(zl[o + 40:o + 44].view(np.int32)[0]) for o in stored.offsets], dtype=np.int64)
+    return zlen, dlen
+
+
+def reframe_libzstd(table, level):
+    """The table's blocks with payloads compressed by libzstd at `level` (kept raw when not smaller), checksums fixed."""
+    sys.path.insert(0, os.path.join(ROOT, "tests"))
+    sys.path.insert(0, os.path.join(ROOT, "tests", "golden"))
+    import make_zstd_golden as golden
+    from test_gpu_lz4_blocks import _reframe_with
+    z = golden.libzstd()
+    if z is None:
+        return None
+    zs = golden.Zstd(z)
+    return _reframe_with(table, lambda p: zs.compress(p, level))
+
+
+def zstd_main(a):
+    import concurrent.futures as cf
+    import torch
+    import oceanbase_b200 as ob
+    from oceanbase_b200 import capi
+    from oceanbase_b200.capi import lib
+    from oceanbase_b200.sstable import compress_table
+    sys.path.insert(0, os.path.join(ROOT, "tests", "golden"))
+    import make_zstd_golden as golden
+    rows = a.rows or 8_000_000
+    t0 = time.time()
+    table = make_table(rows, a.rpb)
+    variants = {"writer": compress_table(table, capi.COMPRESSOR_ZSTD_1_3_8), "libzstd1": reframe_libzstd(table, 1),
+                "libzstd3": reframe_libzstd(table, 3)}
+    build_s = time.time() - t0
+    ctx = ob.ScanContext(0, stream=torch.cuda.current_stream().cuda_stream)
+    pinned_plain = torch.from_numpy(table.image).pin_memory()
+    plain_h = type(table)(pinned_plain.numpy(), table.offsets, table.sizes, table.total_rows, table.n_cols)
+    dev_plain = pinned_plain.cuda()
+    torch.cuda.synchronize()
+    res = {"open_host_plain_ms": timed(lambda: ob.PageBatch(ctx, plain_h), a.reps),
+           "open_device_plain_ms": timed(lambda: ob.PageBatch(ctx, table, device_image_ptr=dev_plain.data_ptr(), host_view=False,
+                                                              image_size=table.image.size), a.reps)}
+    z = golden.libzstd()
+    for name, stored in variants.items():
+        if stored is None:
+            res[name] = "not measured (libzstd.so.1 not present)"
+            continue
+        pinned = torch.from_numpy(stored.image).pin_memory()
+        st_h = type(stored)(pinned.numpy(), stored.offsets, stored.sizes, stored.total_rows, stored.n_cols)
+        dev = pinned.cuda()
+        torch.cuda.synchronize()
+        r = {"open_host_ms": timed(lambda: ob.PageBatch(ctx, st_h, compressor=capi.COMPRESSOR_ZSTD_1_3_8), a.reps),
+             "open_device_ms": timed(lambda: ob.PageBatch(ctx, stored, device_image_ptr=dev.data_ptr(), image_size=stored.image.size,
+                                                          compressor=capi.COMPRESSOR_ZSTD_1_3_8), a.reps)}
+        zlen, dlen = stored_sizes(stored)
+        comp = zlen < dlen
+        idx = np.nonzero(comp)[0]
+        in_off = (stored.offsets[idx] + 64).astype(np.int64)
+        in_len = zlen[idx].astype(np.int64)
+        out_len = dlen[idx].astype(np.int64)
+        out_off = np.concatenate([[0], np.cumsum(out_len)[:-1]]).astype(np.int64)
+        d_out = torch.empty(int(out_len.sum()), dtype=torch.uint8, device="cuda")
+        stv = np.zeros(len(idx), dtype=np.int32)
+        ks = []
+        for rep in range(a.reps + 1):
+            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            e0.record()
+            code = lib.obgpu_zstd_decompress(ctx._h, C.c_void_p(dev.data_ptr()), in_off.ctypes.data, in_len.ctypes.data,
+                                             C.c_void_p(d_out.data_ptr()), out_off.ctypes.data, out_len.ctypes.data, len(idx), stv.ctypes.data)
+            e1.record()
+            e1.synchronize()
+            assert code == 0 and (stv == 0).all()
+            if rep:
+                ks.append(e0.elapsed_time(e1))
+        r["zstd_decompress_ms"] = float(np.median(ks))
+        r["zstd_decoded_gbps"] = float(out_len.sum()) / (r["zstd_decompress_ms"] * 1e-3) / 1e9
+        r.update({"compressed_blocks": int(comp.sum()), "stored_bytes": int(stored.image.size),
+                  "ratio": float(table.image.size) / float(stored.image.size),
+                  "payload_ratio": float(out_len.sum()) / float(max(in_len.sum(), 1))})
+        if z is None:
+            r["cpu_libzstd"] = "not measured (libzstd.so.1 not present)"
+        else:   # CPU baseline: one ZSTD_decompressDCtx per compressed payload, --cpu-threads threads (ctypes drops the GIL)
+            img = stored.image
+            chunks = np.array_split(np.arange(len(idx)), a.cpu_threads)
+            outbuf = np.empty(int(out_len.sum()), dtype=np.uint8)
+
+            def work(ks_):
+                d = z.ZSTD_createDCtx()
+                base = img.ctypes.data
+                for k in ks_:
+                    n = z.ZSTD_decompressDCtx(d, C.c_void_p(outbuf.ctypes.data + int(out_off[k])), int(out_len[k]),
+                                              C.cast(C.c_void_p(base + int(in_off[k])), C.c_char_p), int(in_len[k]))
+                    assert n == out_len[k]
+                return len(ks_)
+            with cf.ThreadPoolExecutor(a.cpu_threads) as ex:
+                list(ex.map(work, chunks))   # warm-up
+                cpu = []
+                for _ in range(a.reps):
+                    t1 = time.perf_counter()
+                    list(ex.map(work, chunks))
+                    cpu.append((time.perf_counter() - t1) * 1e3)
+            r["cpu_libzstd_ms"] = float(np.median(cpu))
+            r["cpu_libzstd_decoded_gbps"] = float(out_len.sum()) / (r["cpu_libzstd_ms"] * 1e-3) / 1e9
+            r["cpu_threads"] = a.cpu_threads
+        res[name] = r
+        del dev, pinned
+    name, power = card()
+    res.update({"compressor": "zstd_1.3.8", "card": name, "power_limit_and_max_sm_clock": power, "rows": rows, "rows_per_block": a.rpb,
+                "n_blocks": int(table.n_blocks), "plain_bytes": int(table.image.size), "table_build_s": build_s, "reps": a.reps,
+                "libzstd": z.ZSTD_versionString().decode() if z is not None else "not present"})
+    ctx.close()
+    return res
+
+
 def main():
     ap = argparse.ArgumentParser()
-    ap.add_argument("--rows", type=int, default=76_000_000)
+    ap.add_argument("--compressor", choices=["lz4", "zstd"], default="lz4")
+    ap.add_argument("--rows", type=int, default=None)
     ap.add_argument("--rpb", type=int, default=700)
     ap.add_argument("--reps", type=int, default=3)
+    ap.add_argument("--cpu-threads", type=int, default=os.cpu_count() or 1)
     ap.add_argument("--out", default=None)
     a = ap.parse_args()
+    if a.compressor == "zstd":
+        line = json.dumps(zstd_main(a))
+        print(line)
+        if a.out:
+            with open(a.out, "w") as f:
+                f.write(line + "\n")
+        return
+    a.rows = a.rows or 76_000_000
     import torch
     import oceanbase_b200 as ob
     from oceanbase_b200 import capi
