@@ -5,23 +5,20 @@
 //             (ob_macro_block_common_header.cpp:54-69, ob_sstable_macro_block_header.cpp:118-140) -> micro_block_count_
 //   walk    : one thread per macro block follows the micro headers (header_size_ + data_zlength_ each) from
 //             micro_block_data_offset_; the walk must end at micro_block_data_offset_ + micro_block_data_size_ with row_count_ rows
-//   realign : one CTA per micro-block copies it to a 128-byte aligned slot of a new image (unaligned source words through
-//             funnel shifts, 16-byte stores, zero padding) -- one read + one write of the data, at HBM speed, once per cache fill
-// Macro blocks whose compressor_type_ is LZ4 / LZ4_1_9_1 / ZSTD_1_3_8 hold micro-blocks in stored form: the walk's (offset,
-// stored size) pairs go to open_stored_blocks (lz4_blocks.cuh), which decodes the compressed ones into their slots and
-// realigns the raw ones with the kernel below; the survey reports each macro block's compressor, and the ones of one open
-// must agree. 16 bytes per micro-block (offset, size) and 4 per macro block come back to the host for
-// obgpu_batch_open's tables; the block bytes never touch the CPU. Other compressors and encrypted blocks are refused.
+//   open    : the walk's (offset, stored size) pairs go to open_stored_blocks (stored_blocks.cuh), which copies every raw
+//             micro-block to a 128-byte aligned slot of a new image (obgpu_macro_realign_kernel) and decodes the compressed ones
+//             (compressor_type_ LZ4 / LZ4_1_9_1 / ZSTD_1_3_8) into theirs -- once per cache fill
+// The survey reports each macro block's compressor, and the ones of one open must agree. 16 bytes per micro-block (offset,
+// size) and 4 per macro block come back to the host for obgpu_batch_open's tables; the block bytes never touch the CPU. Other
+// compressors and encrypted blocks are refused.
 #pragma once
 
 namespace mb {
 
 constexpr int32_t kStOk = 0, kStBadCommon = 1, kStBadFixed = 2, kStBadWalk = 3, kStCompressed = 4;
 
-__device__ __forceinline__ uint32_t ld32u(const uint8_t *p) {   // unaligned little-endian loads
-  return (uint32_t)p[0] | ((uint32_t)p[1] << 8) | ((uint32_t)p[2] << 16) | ((uint32_t)p[3] << 24);
-}
-__device__ __forceinline__ uint64_t ld64u(const uint8_t *p) { return (uint64_t)ld32u(p) | ((uint64_t)ld32u(p + 4) << 32); }
+using sb::ld32u;
+using sb::ld64u;
 
 struct Fixed {
   int32_t micro_count, data_off, data_size, row_count, compressor;
@@ -54,9 +51,7 @@ __device__ __forceinline__ int32_t parse_headers(const uint8_t *m, int64_t macro
   if (f.data_off != 24 + 128 + type_cols * 8 + (int64_t)column_count * 8 + 1) return kStBadFixed;
   if ((int64_t)f.data_off + f.data_size > macro_size || occupy != f.data_off + f.data_size) return kStBadFixed;
   if ((int64_t)f.micro_count * 64 > f.data_size) return kStBadFixed;   // a micro-block is at least its 64-byte header
-  if ((compressor != OBGPU_COMPRESSOR_NONE && compressor != OBGPU_COMPRESSOR_LZ4 && compressor != OBGPU_COMPRESSOR_LZ4_1_9_1 &&
-       compressor != OBGPU_COMPRESSOR_ZSTD_1_3_8) || encrypt_id != 0)
-    return kStCompressed;
+  if (!obf::stored_compressor(f.compressor) || encrypt_id != 0) return kStCompressed;
   return kStOk;
 }
 
@@ -97,42 +92,7 @@ __global__ void obgpu_macro_walk_kernel(const uint8_t *image, int64_t macro_size
   if (!ok || at != end || rows != f.row_count) atomicMax(status, kStBadWalk);
 }
 
-constexpr int kCopyThreads = 128;
-__global__ void __launch_bounds__(kCopyThreads) obgpu_macro_realign_kernel(const uint8_t *image, int64_t image_size, const int64_t *src_off,
-                                                                            const int64_t *sizes, const int64_t *dst_off, uint8_t *out) {
-  const int64_t blk = blockIdx.x;
-  const int64_t src = src_off[blk], sz = sizes[blk];
-  const int64_t slot = (sz + 127) & ~127ll;
-  uint4 *dst = reinterpret_cast<uint4 *>(out + dst_off[blk]);
-  const uint32_t sh = (uint32_t)(src & 3) * 8u;
-  const uint32_t *w = reinterpret_cast<const uint32_t *>(image + (src & ~3ll));
-  const int64_t w_cap = (image_size - (src & ~3ll)) >> 2;   // whole words readable from w
-  for (int64_t j = threadIdx.x; j < slot / 16; j += kCopyThreads) {
-    uint32_t v[5];
-#pragma unroll
-    for (int k = 0; k < 5; ++k) {
-      const int64_t idx = j * 4 + k;
-      v[k] = idx < w_cap ? __ldg(w + idx) : 0u;
-    }
-    uint32_t o[4];
-#pragma unroll
-    for (int k = 0; k < 4; ++k) o[k] = __funnelshift_r(v[k], v[k + 1], sh);
-    const int64_t left = sz - j * 16;   // bytes of this chunk that belong to the block
-    if (left < 16) {
-#pragma unroll
-      for (int k = 0; k < 4; ++k) {
-        const int64_t lb = left - 4 * k;
-        o[k] = lb >= 4 ? o[k] : (lb <= 0 ? 0u : (o[k] & (0xffffffffu >> (32 - 8 * (int)lb))));
-      }
-    }
-    dst[j] = make_uint4(o[0], o[1], o[2], o[3]);
-  }
-}
-
 }  // namespace mb
-
-static int open_stored_blocks(obgpu_ctx *ctx, const uint8_t *d_image, int64_t image_size, const int64_t *d_src, const int64_t *d_zsize,
-                              int32_t n, int32_t compressor, obgpu_batch **out);   // lz4_blocks.cuh (decoders: lz4 / zstd_blocks.cuh)
 
 extern "C" {
 
@@ -142,18 +102,10 @@ int obgpu_batch_open_macro_blocks(obgpu_ctx *ctx, const void *macro_image, int64
       image_size < macro_block_size * (int64_t)n_macro_blocks)
     return OBGPU_INVALID_ARGUMENT;
   cudaSetDevice(ctx->device);
-  const uint8_t *d_macro = (const uint8_t *)macro_image;
-  void *tmp_image = nullptr;
-  if (!image_on_device) {
-    CUDA_TRY(ctx, cudaMallocAsync(&tmp_image, (size_t)image_size, ctx->stream));
-    cudaError_t e = cudaMemcpyAsync(tmp_image, macro_image, (size_t)image_size, cudaMemcpyHostToDevice, ctx->stream);
-    if (e != cudaSuccess) { ctx->err = cudaGetErrorString(e); cudaFreeAsync(tmp_image, ctx->stream); return OBGPU_ERR_SYS; }
-    d_macro = (const uint8_t *)tmp_image;
-  } else if (((uintptr_t)macro_image & 15u) != 0) {
-    ctx->err = "device-resident macro blocks must be 16-byte aligned";
-    return OBGPU_INVALID_ARGUMENT;
-  }
-  int ret = OBGPU_SUCCESS;
+  DeviceImage img;
+  int ret = stage_image(ctx, macro_image, image_size, image_on_device, "device-resident macro blocks must be 16-byte aligned", img);
+  if (ret != OBGPU_SUCCESS) return ret;
+  const uint8_t *d_macro = img.d;
   void *d_small = nullptr, *d_tab = nullptr;
   std::vector<int32_t> counts((size_t)n_macro_blocks + 1), comps((size_t)n_macro_blocks);
   std::vector<int64_t> first((size_t)n_macro_blocks + 1);
@@ -208,7 +160,7 @@ int obgpu_batch_open_macro_blocks(obgpu_ctx *ctx, const void *macro_image, int64
   } while (0);
   if (d_small) cudaFreeAsync(d_small, ctx->stream);
   if (d_tab) cudaFreeAsync(d_tab, ctx->stream);
-  if (tmp_image) cudaFreeAsync(tmp_image, ctx->stream);
+  if (img.tmp) cudaFreeAsync(img.tmp, ctx->stream);
   return ret;
 }
 

@@ -13,6 +13,8 @@
 #pragma once
 #include <stdint.h>
 
+#include "../../include/obgpu_scan.h"   // OBGPU_COMPRESSOR_*
+
 #if defined(__CUDACC__)
 #define OBF_HD __host__ __device__ __forceinline__
 #else
@@ -136,7 +138,28 @@ enum CSColAttr : uint8_t { CS_IS_FIXED_LENGTH = 0x01, CS_HAS_NULL_OR_NOP_BITMAP 
 enum IntStreamAttr : uint8_t { IS_USE_BASE = 0x1, IS_REPLACE_NULL_VALUE = 0x2, IS_DECIMAL_INT = 0x4 };
 enum IntStreamType : uint8_t { IS_RAW = 1 };   // the other codecs need the CPU transformer (not handled)
 constexpr uint8_t INTEGER_STREAM_META_V2 = 1;
-constexpr uint8_t COMPRESSOR_NONE = 1;         // common::ObCompressorType::NONE_COMPRESSOR
+
+// ObCompressorType values whose micro-blocks the library writes and opens in stored form: NONE, and the payload codecs the
+// device decodes (stored_blocks.cuh)
+OBF_HD bool stored_compressor(int32_t c) {
+  return c == OBGPU_COMPRESSOR_NONE || c == OBGPU_COMPRESSOR_LZ4 || c == OBGPU_COMPRESSOR_LZ4_1_9_1 || c == OBGPU_COMPRESSOR_ZSTD_1_3_8;
+}
+
+// ObMicroBlockHeader header checksum (ob_micro_block_header.cpp:203-233) of a 64-byte header as stored: the XOR of the 16-bit
+// halves of its fields, header_checksum_ (bytes 8-9) left out; the signed 32-bit fields are sign-extended to 64 bits first.
+OBF_HD int16_t micro_header_checksum(const uint8_t *h) {
+  auto le = [h](int off, int bytes) {   // unaligned little-endian load
+    uint64_t v = 0;
+    for (int k = bytes - 1; k >= 0; --k) v = (v << 8) | h[off + k];
+    return v;
+  };
+  auto i32 = [&](int off) { return (uint64_t)(int64_t)(int32_t)le(off, 4); };
+  const uint64_t x = le(0, 2) ^ le(2, 2) ^ h[20] ^ h[21]                  // magic_, version_, row_store_type_, opt_
+                     ^ le(10, 2) ^ le(12, 2) ^ (le(14, 2) & 1) ^ le(22, 2)  // column_count_, rowkey_column_count_, has_column_checksum, opt2_
+                     ^ le(4, 4) ^ le(16, 4) ^ le(24, 4) ^ i32(28)          // header_size_, row_count_, row_data_offset_, original_length_
+                     ^ le(32, 8) ^ i32(40) ^ i32(44) ^ le(48, 8);          // max_merged_trans_version_, data_length_, data_zlength_, data_checksum_
+  return (int16_t)(uint16_t)(x ^ (x >> 16) ^ (x >> 32) ^ (x >> 48));
+}
 
 static_assert(sizeof(MicroBlockHeader) == 64, "micro header must be 64 bytes");
 static_assert(sizeof(ColumnHeader) == 16, "column header must be 16 bytes");

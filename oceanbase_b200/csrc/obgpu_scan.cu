@@ -3644,7 +3644,6 @@ int obgpu_project_datums(obgpu_batch *batch, int32_t block, int32_t col, const i
 }  // extern "C"
 
 // ---- ObCGBitmap: range bitmaps shared by the column groups of a table ----------------------------------------------------
-#include "macro_blocks.cuh"   // macro blocks (disk format) -> page batch, parsed and re-laid on the device
 #include "cg_bitmap.cuh"
 
 // ---- string cells as bytes (dense heap): scan results and the per-block entry ------------------------------------------
@@ -3659,8 +3658,8 @@ int obgpu_project_datums(obgpu_batch *batch, int32_t block, int32_t col, const i
 #include "merge_exchange.cuh"
 #include "merge_streamed.cuh"
 #include "encode_kernels.cuh"   // phase B: merged columns -> SSTable bytes + column checksums
-#include "lz4_blocks.cuh"       // LZ4-compressed micro-blocks decoded at open (page batches, macro blocks)
-#include "zstd_blocks.cuh"      // zstd-compressed micro-blocks: the decoder behind the same open
+#include "stored_blocks.cuh"    // stored (raw, LZ4- or zstd-compressed) micro-blocks -> page batch, decoded on the device
+#include "macro_blocks.cuh"     // macro blocks (disk format) -> page batch, parsed on the device
 
 // ---- host-buffer scan pipeline (include/obgpu_pipeline.h) ------------------------------------------------
 #include "host_pipeline.h"

@@ -1,4 +1,4 @@
-// One zstd frame (RFC 8878) -> exactly n_out bytes: the decoder behind zstd_blocks.cuh (ObZstdCompressor_1_3_8::decompress,
+// One zstd frame (RFC 8878) -> exactly n_out bytes: the decoder behind stored_blocks.cuh (ObZstdCompressor_1_3_8::decompress,
 // ZSTD_decompressDCtx into a buffer of data_length_ bytes, per micro-block payload in the reference).
 // Self-contained and __host__ __device__: the same code runs in a warp on the device and single-threaded in a CPU build.
 //   lanes   : every lane runs the serial walk (headers, bit readers, FSE states) on the same bytes, so the warp stays converged
