@@ -83,9 +83,6 @@ __device__ __forceinline__ uint32_t area_bytes(uint32_t rows, uint32_t max_len) 
 }
 
 // ---- span columns ---------------------------------------------------------------------------------------------------------------
-__device__ __forceinline__ bool is_mat_type(uint32_t t) {
-  return t == COL_STRING_DIFF || t == COL_HEX_PACKING || t == COL_STRING_PREFIX || t == COL_COLUMN_EQUAL || t == COL_COLUMN_SUBSTR;
-}
 __device__ __forceinline__ bool is_span_type(uint32_t t) { return t == COL_COLUMN_EQUAL || t == COL_COLUMN_SUBSTR; }
 
 struct SpanCol {
@@ -254,7 +251,7 @@ __global__ void __launch_bounds__(256) mat_probe_kernel(const uint8_t *image, co
   if (!b.ok || b.is_cs) return;
   for (uint32_t c = 0; c < b.column_count; ++c) {
     const uint32_t t = (ld32(s, b.header_size + 16u * c) >> 8) & 0xffu;
-    if (is_mat_type(t)) { atomicOr(flag, MF_ANY); return; }
+    if (obf::rebuilt_at_open(t)) { atomicOr(flag, MF_ANY); return; }
   }
 }
 
@@ -272,7 +269,7 @@ __global__ void __launch_bounds__(128) mat_survey_kernel(const uint8_t *image, c
   if (b.ok && !b.is_cs) {
     for (uint32_t c = 0; c < b.column_count; ++c) {
       const uint32_t w0 = ld32(s, b.header_size + 16u * c), t = (w0 >> 8) & 0xffu;
-      if (!is_mat_type(t)) continue;
+      if (!obf::rebuilt_at_open(t)) continue;
       uint64_t need;
       if (is_span_type(t)) {
         need = span_area_need(s, b, (int)c, lane);
@@ -317,7 +314,7 @@ __global__ void __launch_bounds__(128) mat_rewrite_kernel(const uint8_t *image, 
   for (uint32_t c = 0; c < b.column_count; ++c) {
     const uint32_t ch = b.header_size + 16u * c;
     const uint32_t t = (ld32(s, ch) >> 8) & 0xffu;
-    if (!is_mat_type(t)) continue;
+    if (!obf::rebuilt_at_open(t)) continue;
     if (is_span_type(t)) {   // the column header of the copy says where the area is
       const uint32_t need = span_area_need(s, b, (int)c, lane);
       if (need == 0) continue;

@@ -161,6 +161,38 @@ OBF_HD int16_t micro_header_checksum(const uint8_t *h) {
   return (int16_t)(uint16_t)(x ^ (x >> 16) ^ (x >> 32) ^ (x >> 48));
 }
 
+// What check_micro_header found wrong with a micro-block header
+enum MicroHeaderVerdict : uint32_t { HDR_OK = 0, HDR_INVALID = 1, HDR_ROW_STORE = 2, HDR_EXTENT = 3, HDR_TOO_MANY_ROWS = 4 };
+struct MicroHeaderFacts {
+  uint32_t header_size, rows, ncol;
+  bool is_cs;
+};
+
+// The header rules a page-batch open applies to a block of `size` bytes, first failure wins: ObMicroBlockHeader::is_valid
+// (ob_micro_block_header.cpp:53-61); a row store type the device path decodes (PAX or CS); the column headers, and a PAX block's
+// row data, start inside the block, which holds at least one row (get_micro_metas bounds); at most 65535 rows. The facts are read
+// from the header whatever the verdict.
+OBF_HD uint32_t check_micro_header(const uint8_t *h, uint32_t size, MicroHeaderFacts &f) {
+  auto le = [h](int off, int bytes) {   // unaligned little-endian load
+    uint32_t v = 0;
+    for (int k = bytes - 1; k >= 0; --k) v = (v << 8) | h[off + k];
+    return v;
+  };
+  const int16_t magic = (int16_t)le(0, 2), version = (int16_t)le(2, 2);
+  const uint32_t nkey = le(12, 2), rst = h[20], row_data_off = le(24, 4);
+  f.header_size = le(4, 4);
+  f.ncol = le(10, 2);
+  f.rows = le(16, 4);
+  f.is_cs = rst == CS_ENCODING_ROW_STORE;
+  if (magic != MICRO_BLOCK_HEADER_MAGIC || version < 1 || version > 3 || f.ncol < nkey || rst >= MAX_ROW_STORE) return HDR_INVALID;
+  if (rst != ENCODING_ROW_STORE && rst != SELECTIVE_ENCODING_ROW_STORE && !f.is_cs) return HDR_ROW_STORE;
+  if (f.header_size < 64 || (uint64_t)f.header_size + (f.is_cs ? 12ull + 4ull * f.ncol : 16ull * f.ncol) > size ||
+      (!f.is_cs && row_data_off > size) || f.rows == 0)
+    return HDR_EXTENT;
+  if (f.rows > 65535u) return HDR_TOO_MANY_ROWS;
+  return HDR_OK;
+}
+
 static_assert(sizeof(MicroBlockHeader) == 64, "micro header must be 64 bytes");
 static_assert(sizeof(ColumnHeader) == 16, "column header must be 16 bytes");
 static_assert(sizeof(DictMetaHeader) == 9, "dict meta header must be 9 bytes");
@@ -182,6 +214,12 @@ enum ColType : int8_t {
   COL_COLUMN_SUBSTR = 9,
   COL_MAX_TYPE = 10,
 };
+
+// Column types whose strings a page batch materialises at open (mat_codecs.cuh): rebuilt by the decoder (STRING_DIFF, HEX_PACKING,
+// STRING_PREFIX) or taken from another column (COLUMN_EQUAL, COLUMN_SUBSTR)
+OBF_HD bool rebuilt_at_open(uint32_t t) {
+  return t == COL_STRING_DIFF || t == COL_HEX_PACKING || t == COL_STRING_PREFIX || t == COL_COLUMN_EQUAL || t == COL_COLUMN_SUBSTR;
+}
 
 // ObColumnHeader::Attribute  ob_block_sstable_struct.h:218-226
 enum ColAttr : int8_t {

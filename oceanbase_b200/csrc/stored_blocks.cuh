@@ -267,14 +267,10 @@ static int open_stored_blocks(obgpu_ctx *ctx, const uint8_t *d_image, int64_t im
         cudaStreamSynchronize(ctx->stream) != cudaSuccess) { fail(OBGPU_ERR_SYS, "stored-block survey"); break; }
     if (st != sb::kStOk) { fail(OBGPU_INVALID_DATA, "micro-block header of a stored block is invalid"); break; }
     // slots + the two work lists: raw -> realign copy, compressed -> decoder
-    int64_t out_bytes = 0;
+    const int64_t out_bytes = (int64_t)slot_layout(dsize.data(), n, dst.data());
     std::vector<int64_t> raw_tab, lz_tab;   // raw: [src][size][dst], compressed: [src][zsize][dst][dsize]
     std::vector<int32_t> raw_idx, lz_idx;
-    for (int32_t i = 0; i < n; ++i) {
-      dst[(size_t)i] = out_bytes;
-      out_bytes += (dsize[(size_t)i] + 127) & ~127ll;
-      (kind[(size_t)i] ? lz_idx : raw_idx).push_back(i);
-    }
+    for (int32_t i = 0; i < n; ++i) (kind[(size_t)i] ? lz_idx : raw_idx).push_back(i);
     const size_t nr = raw_idx.size(), nz = lz_idx.size();
     raw_tab.resize(nr * 3);
     lz_tab.resize(nz * 4);
