@@ -1011,6 +1011,26 @@ __device__ __forceinline__ void dict_str(const uint8_t *s, const ColDesc &d, uin
                                 : (uint32_t)ld_bytes(s, d.dict_payload + ref * ib, ib) - off;
 }
 
+// Shared-window twins of dict_int / dict_str: `sbit` is 8 * the shared-window address of the staged block (or of the
+// staged column region, shifted so block offsets resolve into it).
+__device__ __forceinline__ uint64_t dict_int_s(uint32_t sbit, const ColDesc &d, uint32_t ref) {
+  const uint32_t dbits = d.dict_data_size * 8u, at = sbit + d.dict_payload * 8u + ref * dbits;
+  const uint64_t v = (dbits <= 32u ? (uint64_t)sbits32(at, dbits) : sbits(at, dbits)) + d.base;
+  return d.sign_fix ? sign_fix(d.int_mask, v) : v;
+}
+__device__ __forceinline__ void dict_str_s(uint32_t sbit, const ColDesc &d, uint32_t ref, uint32_t &cell, uint32_t &len) {
+  if (d.dict_fixed) {
+    len = d.dict_data_size;
+    cell = d.dict_payload + ref * len;
+    return;
+  }
+  const uint32_t ib8 = d.dict_data_size * 8u, ibit = sbit + d.dict_payload * 8u;
+  const uint32_t off = ref == 0 ? 0u : sbits32(ibit + (ref - 1u) * ib8, ib8);
+  const uint32_t end = ref == d.dict_count - 1u ? d.dict_end - d.dict_var : sbits32(ibit + ref * ib8, ib8);
+  cell = d.dict_var + off;
+  len = end - off;
+}
+
 // ---- integer-class cell (generic path) -----------------------------------------------------------
 // Returns the 64-bit value image the reference would MEMCPY into the datum (low elem_len bytes
 // significant); is_null set for NULL (and NOP) cells.
