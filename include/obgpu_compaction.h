@@ -209,6 +209,20 @@ int obgpu_encoded_fetch(obgpu_encoded *enc, void *host_image, int64_t image_cap,
 int obgpu_encoded_device_image(obgpu_encoded *enc, const void **dev_image, const int64_t **dev_offsets, const uint32_t **dev_sizes);
 /* Column checksums (K16) of the encoded rows, n_cols values in host memory. */
 int obgpu_encoded_column_checksums(obgpu_encoded *enc, int64_t *host_checksums);
+/* obgpu_writer_compress_blocks on the device. Block i is d_image[d_offsets[i], + d_sizes[i]): a plain micro-block
+ * (header_size_ >= 64, data_zlength_ == data_length_, header_size_ + data_length_ == size), or size 0 = a block left to the
+ * host writer (output size 0, nothing written). Offsets and sizes are device arrays, exactly what
+ * obgpu_encoded_device_image returns. Output: block i at d_out_offsets[i] (aligned as the writer aligns), d_out_sizes[i]
+ * bytes, in STORED form, byte for byte what obgpu_writer_compress_blocks writes for the same block; *out_size (host)
+ * = total bytes. d_out == NULL: *out_size = the capacity the call needs, sum of align_up(d_sizes[i], align) (stored <=
+ * plain, so it always suffices), and nothing else is done (the writer's size-query idiom).
+ * OBGPU_INVALID_ARGUMENT: bad pointers, n_blocks <= 0, align not a power of two in [1, 4096], an offset not a multiple of 16;
+ * OBGPU_NOT_SUPPORTED: a compressor other than NONE, LZ4, LZ4_1_9_1 or ZSTD_1_3_8, or a block above 0x7f000000 bytes;
+ * OBGPU_BUF_NOT_ENOUGH: out_cap below the capacity (nothing written); OBGPU_INVALID_DATA: a block that is not plain.
+ * The padding between blocks is zeroed. */
+int obgpu_compress_blocks(obgpu_ctx *ctx, const void *d_image, const int64_t *d_offsets, const uint32_t *d_sizes,
+                          int32_t n_blocks, int32_t compressor, int32_t align, void *d_out, int64_t out_cap,
+                          int64_t *d_out_offsets, uint32_t *d_out_sizes, int64_t *out_size);
 void obgpu_encoded_free(obgpu_encoded *enc);
 /* Column checksums of plain device columns (no encode). */
 int obgpu_column_checksums(obgpu_ctx *ctx, const obgpu_encode_col *cols, int32_t n_cols, int64_t total_rows, int64_t *host_checksums);

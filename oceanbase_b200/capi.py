@@ -248,6 +248,7 @@ def declared_signatures():
         "obgpu_encoded_device_image": (C.c_int, [vp, P(vp), P(vp), P(vp)]),
         "obgpu_encoded_column_checksums": (C.c_int, [vp, vp]),
         "obgpu_encoded_free": (None, [vp]),
+        "obgpu_compress_blocks": (C.c_int, [vp, vp, vp, vp, i32, i32, i32, vp, i64, vp, vp, P(i64)]),
         "obgpu_column_checksums": (C.c_int, [vp, P(EncodeCol), i32, i64, vp]),
         # include/obgpu_skip_index.h
         "obgpu_batch_set_agg_rows": (C.c_int, [vp, vp, vp]),

@@ -313,6 +313,11 @@ class Encoded:
         check(lib.obgpu_encoded_device_image(self._h, C.byref(a), C.byref(b), C.byref(c)), "obgpu_encoded_device_image", self.ctx._h)
         return a.value, b.value, c.value
 
+    def compress(self, compressor: int, align: int = 128) -> "Compressed":
+        """The blocks in stored form, compressed on the device (compress_blocks over device_image())."""
+        img, off, sz = self.device_image()
+        return compress_blocks(self.ctx, img, off, sz, self.info().n_blocks, compressor, align, keep=self)
+
     def column_checksums(self) -> np.ndarray:
         out = np.zeros(self.n_cols, dtype=np.int64)
         check(lib.obgpu_encoded_column_checksums(self._h, out.ctypes.data), "obgpu_encoded_column_checksums", self.ctx._h)
@@ -329,6 +334,41 @@ class Encoded:
             self.free()
         except Exception:
             pass
+
+
+class Compressed:
+    """Micro-blocks in stored form on the device (obgpu_compress_blocks): byte for byte what obgpu_writer_compress_blocks
+    writes for the same plain blocks; a size of 0 marks a block left to the host writer."""
+
+    def __init__(self, image, offsets, sizes, size, keep=None):
+        self.image, self.offsets, self.sizes, self.image_size, self._keep = image, offsets, sizes, size, keep
+
+    def fetch(self):
+        """(image uint8, offsets int64, sizes int64), the form Encoded.fetch returns."""
+        return (self.image[:self.image_size].cpu().numpy(), self.offsets.cpu().numpy(),
+                self.sizes.cpu().numpy().view(np.uint32).astype(np.int64))
+
+    def device_image(self):
+        """(device pointer of the image, of the int64 offsets, of the uint32 sizes) -- valid while this object lives."""
+        return self.image.data_ptr(), self.offsets.data_ptr(), self.sizes.data_ptr()
+
+
+def compress_blocks(ctx, dev_image: int, dev_offsets: int, dev_sizes: int, n_blocks: int, compressor: int, align: int = 128,
+                    keep=None) -> Compressed:
+    """Plain micro-blocks dev_image[dev_offsets[i], + dev_sizes[i]) (device pointers: int64 offsets, uint32 sizes, 0 = no
+    block) -> stored form with `compressor`, compressed on the device into an output buffer torch allocates."""
+    import torch
+    cap = C.c_int64()
+    check(lib.obgpu_compress_blocks(ctx._h, dev_image, dev_offsets, dev_sizes, n_blocks, compressor, align, None, 0, None, None,
+                                    C.byref(cap)), "obgpu_compress_blocks", ctx._h)
+    dev = torch.device("cuda", ctx.device)
+    out = torch.empty(max(cap.value, 1), dtype=torch.uint8, device=dev)
+    off = torch.empty(n_blocks, dtype=torch.int64, device=dev)
+    sz = torch.empty(n_blocks, dtype=torch.int32, device=dev)
+    size = C.c_int64()
+    check(lib.obgpu_compress_blocks(ctx._h, dev_image, dev_offsets, dev_sizes, n_blocks, compressor, align, out.data_ptr(), cap.value,
+                                    off.data_ptr(), sz.data_ptr(), C.byref(size)), "obgpu_compress_blocks", ctx._h)
+    return Compressed(out, off, sz, size.value, keep)
 
 
 def _encode_cols(cols):

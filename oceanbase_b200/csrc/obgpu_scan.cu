@@ -3155,6 +3155,7 @@ int obgpu_project_datums(obgpu_batch *batch, int32_t block, int32_t col, const i
 #include "merge_streamed.cuh"
 #include "encode_kernels.cuh"   // phase B: merged columns -> SSTable bytes + column checksums
 #include "stored_blocks.cuh"    // stored (raw, LZ4- or zstd-compressed) micro-blocks -> page batch, decoded on the device
+#include "stored_compress.cuh"  // plain micro-blocks -> stored (LZ4- or zstd-compressed) form, compressed on the device
 #include "macro_blocks.cuh"     // macro blocks (disk format) -> page batch, parsed on the device
 
 // ---- host-buffer scan pipeline (include/obgpu_pipeline.h) ------------------------------------------------

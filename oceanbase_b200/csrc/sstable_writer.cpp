@@ -25,6 +25,7 @@
 #include <vector>
 
 #include "../../include/obgpu_writer.h"
+#include "ob_compress_format.h"
 #include "ob_format.h"
 #include "stream_codecs_host.h"
 
@@ -2507,7 +2508,8 @@ int obgpu_writer_stream_encode(int32_t type, int32_t width_bytes, const uint64_t
 // ---- LZ4 block format (lz4_Block_format.md): what ObLZ4Compressor::compress writes per micro-block payload -------------------
 // Greedy single-pass compressor: 4-byte hash -> last position (64 Ki entries), offsets below 64 KiB, no backward extension.
 // End-of-block rules of the format: the last 5 bytes are literals (a match ends at n - 5 at the latest) and the last match
-// starts at least 12 bytes before the end; the block ends with a literal-only sequence.
+// starts at least 12 bytes before the end; the block ends with a literal-only sequence. The constants, the zstd tables and
+// the zstd headers / bitstream are ob_compress_format.h's, which the device compressor (stored_compress.cuh) shares.
 namespace {
 inline uint32_t rd32le(const uint8_t *p) { uint32_t v; memcpy(&v, p, 4); return v; }
 
@@ -2519,17 +2521,16 @@ void lz4_put_len(std::vector<uint8_t> &o, int64_t extra) {   // length extension
 // The greedy matcher: emit(at, offset, length) for each match, in order (match length >= 4, offset <= 65535).
 template <class Emit>
 void greedy_matches(const uint8_t *src, int64_t n, Emit emit) {
-  constexpr int64_t kLastLiterals = 5, kMfLimit = 12, kMaxOffset = 65535;
-  if (n <= kMfLimit) return;
-  std::vector<int32_t> table(1u << 16, -1);
-  const int64_t match_end_limit = n - kLastLiterals;
+  if (n <= obz::kMfLimit) return;
+  std::vector<int32_t> table(obz::kHashEntries, -1);
+  const int64_t match_end_limit = n - obz::kLastLiterals;
   int64_t ip = 0;
-  while (ip <= n - kMfLimit) {
+  while (ip <= n - obz::kMfLimit) {
     const uint32_t seq = rd32le(src + ip);
-    const uint32_t h = (seq * 2654435761u) >> 16;
+    const uint32_t h = obz::hash4(seq);
     const int64_t ref = table[h];
     table[h] = (int32_t)ip;
-    if (ref >= 0 && ip - ref <= kMaxOffset && rd32le(src + ref) == seq) {
+    if (ref >= 0 && ip - ref <= obz::kMaxOffset && rd32le(src + ref) == seq) {
       int64_t len = 4;
       while (ip + len < match_end_limit && src[ref + len] == src[ip + len]) ++len;
       emit(ip, ip - ref, len);
@@ -2565,92 +2566,15 @@ void lz4_compress_block(const uint8_t *src, int64_t n, std::vector<uint8_t> &o) 
 // One frame: Single_Segment, Frame_Content_Size, no checksum, no dictionary. Blocks of <= 128 KiB matched on their own by
 // greedy_matches; Raw literals; sequences in Predefined mode for LL / OF / ML, FSE-coded from the RFC's default
 // distributions (FSE_buildCTable / ZSTD_encodeSequences order); a block that does not shrink is a Raw block.
-struct FseEnc {   // FSE encoding table of one predefined distribution
-  int log = 0;
-  std::vector<uint16_t> state;
-  std::vector<int32_t> dnb, dfs;   // per symbol: deltaNbBits, deltaFindState
-  FseEnc(const int16_t *norm, int nsym, int lg) : log(lg), state((size_t)1 << lg), dnb((size_t)nsym), dfs((size_t)nsym) {
-    const int size = 1 << lg, mask = size - 1, step = (size >> 1) + (size >> 3) + 3;
-    std::vector<int> sym((size_t)size), cumul((size_t)nsym + 1);
-    int high = size - 1;
-    for (int s = 0; s < nsym; ++s) {
-      if (norm[s] == -1) {
-        cumul[(size_t)s + 1] = cumul[(size_t)s] + 1;
-        sym[(size_t)high--] = s;
-      } else {
-        cumul[(size_t)s + 1] = cumul[(size_t)s] + norm[s];
-      }
-    }
-    int pos = 0;
-    for (int s = 0; s < nsym; ++s)
-      for (int i = 0; i < norm[s]; ++i) {
-        sym[(size_t)pos] = s;
-        do pos = (pos + step) & mask; while (pos > high);
-      }
-    for (int u = 0; u < size; ++u) state[(size_t)cumul[(size_t)sym[(size_t)u]]++] = (uint16_t)(size + u);
-    int total = 0;
-    for (int s = 0; s < nsym; ++s) {
-      const int c = norm[s];
-      if (c == -1 || c == 1) {
-        dnb[(size_t)s] = (lg << 16) - size;
-        dfs[(size_t)s] = total - 1;
-        ++total;
-      } else if (c > 1) {
-        const int max_bits_out = lg - (31 - __builtin_clz((uint32_t)(c - 1)));
-        dnb[(size_t)s] = (max_bits_out << 16) - (c << max_bits_out);
-        dfs[(size_t)s] = total - c;
-        total += c;
-      }
-    }
-  }
-};
-
-struct BitWriter {   // forward little-endian bit accumulator (the decoder reads the stream backward)
+struct ByteSink {   // obz byte sink over a vector
   std::vector<uint8_t> &o;
-  uint64_t acc = 0;
-  int nb = 0;
-  explicit BitWriter(std::vector<uint8_t> &out) : o(out) {}
-  void add(uint64_t v, int k) {
-    acc |= (v & ((1ull << k) - 1)) << nb;
-    nb += k;
-    for (; nb >= 8; nb -= 8, acc >>= 8) o.push_back((uint8_t)acc);
-  }
-  void close() {   // the end mark: one 1 bit, then padding to the byte
-    add(1, 1);
-    if (nb) o.push_back((uint8_t)acc);
-  }
+  void put(uint8_t b) { o.push_back(b); }
 };
-
-int zstd_code(uint32_t v, bool ml) {   // largest Literals_Length / Match_Length code whose baseline is <= v
-  static const uint32_t ll_base[36] = {0, 1, 2, 3, 4, 5, 6, 7, 8, 9, 10, 11, 12, 13, 14, 15, 16, 18, 20, 22, 24, 28, 32, 40, 48, 64,
-                                       128, 256, 512, 1024, 2048, 4096, 8192, 16384, 32768, 65536};
-  static const uint32_t ml_base[53] = {3, 4, 5, 6, 7, 8, 9, 10, 11, 12, 13, 14, 15, 16, 17, 18, 19, 20, 21, 22, 23, 24, 25, 26, 27, 28,
-                                       29, 30, 31, 32, 33, 34, 35, 37, 39, 41, 43, 47, 51, 59, 67, 83, 99, 131, 259, 515, 1027, 2051,
-                                       4099, 8195, 16387, 32771, 65539};
-  const uint32_t *b = ml ? ml_base : ll_base;
-  int c = (ml ? 53 : 36) - 1;
-  while (b[c] > v) --c;
-  return c;
-}
-int zstd_extra_bits(int c, bool ml) {
-  static const uint8_t ll_bits[36] = {0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 1, 1, 1, 1, 2, 2, 3, 3, 4, 6, 7, 8, 9, 10, 11, 12,
-                                      13, 14, 15, 16};
-  return ml ? (c < 32 ? 0 : c < 36 ? 1 : c < 38 ? 2 : c < 40 ? 3 : c < 42 ? 4 : c == 42 ? 5 : c - 36) : ll_bits[c];
-}
-
-const FseEnc &zstd_predefined(int which) {   // 0 LL, 1 OF, 2 ML (RFC 8878 3.1.1.3.2.2)
-  static const int16_t ll[36] = {4, 3, 2, 2, 2, 2, 2, 2, 2, 2, 2, 2, 2, 1, 1, 1, 2, 2, 2, 2, 2, 2, 2, 2, 2, 3, 2, 1, 1, 1, 1, 1, -1, -1, -1, -1};
-  static const int16_t of[29] = {1, 1, 1, 1, 1, 1, 2, 2, 2, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1, -1, -1, -1, -1, -1};
-  static const int16_t ml[53] = {1, 4, 3, 2, 2, 2, 2, 2, 2, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1,
-                                 1, 1, 1, 1, 1, 1, 1, 1, 1, 1, -1, -1, -1, -1, -1, -1, -1};
-  static const FseEnc t[3] = {FseEnc(ll, 36, 6), FseEnc(of, 29, 5), FseEnc(ml, 53, 6)};
-  return t[which];
-}
 
 // the Block_Content of one Compressed_Block for src[0, n) (n <= 128 KiB)
 void zstd_compressed_block(const uint8_t *src, int64_t n, std::vector<uint8_t> &o) {
-  struct Seq { uint32_t ll, off, ml; };
-  std::vector<Seq> seqs;
+  static const obz::FseSet fse = [] { obz::FseSet f; obz::fse_build_predefined(f); return f; }();
+  std::vector<obz::Seq> seqs;
   std::vector<uint8_t> lits;
   int64_t anchor = 0;
   greedy_matches(src, n, [&](int64_t at, int64_t offset, int64_t len) {
@@ -2660,90 +2584,24 @@ void zstd_compressed_block(const uint8_t *src, int64_t n, std::vector<uint8_t> &
   });
   lits.insert(lits.end(), src + anchor, src + n);
   o.clear();
-  const uint32_t nl = (uint32_t)lits.size();   // Raw literals header: 1, 2 or 3 bytes
-  if (nl < 32) {
-    o.push_back((uint8_t)(nl << 3));
-  } else if (nl < 4096) {
-    o.push_back((uint8_t)((1u << 2) | ((nl & 15) << 4)));
-    o.push_back((uint8_t)(nl >> 4));
-  } else {
-    o.push_back((uint8_t)((3u << 2) | ((nl & 15) << 4)));
-    o.push_back((uint8_t)(nl >> 4));
-    o.push_back((uint8_t)(nl >> 12));
-  }
+  ByteSink sink{o};
+  obz::zstd_literals_header(sink, (uint32_t)lits.size());
   o.insert(o.end(), lits.begin(), lits.end());
-  const size_t ns = seqs.size();
-  if (ns < 128) {
-    o.push_back((uint8_t)ns);
-  } else if (ns < 0x7f00) {
-    o.push_back((uint8_t)((ns >> 8) + 128));
-    o.push_back((uint8_t)ns);
-  } else {
-    o.push_back(255);
-    o.push_back((uint8_t)(ns - 0x7f00));
-    o.push_back((uint8_t)((ns - 0x7f00) >> 8));
-  }
-  if (ns == 0) return;
-  o.push_back(0);   // Symbol_Compression_Modes: Predefined x 3
-  const FseEnc &tll = zstd_predefined(0), &tof = zstd_predefined(1), &tml = zstd_predefined(2);
-  std::vector<int> llc(ns), mlc(ns), ofc(ns);
-  for (size_t k = 0; k < ns; ++k) {
-    llc[k] = zstd_code(seqs[k].ll, false);
-    mlc[k] = zstd_code(seqs[k].ml, true);
-    ofc[k] = 31 - __builtin_clz(seqs[k].off + 3);   // Offset_Value = offset + 3: no repeat codes
-  }
-  BitWriter bw(o);
-  auto init = [&](const FseEnc &t, int s) {
-    const uint32_t nbo = (uint32_t)((t.dnb[(size_t)s] + (1 << 15)) >> 16);
-    const uint32_t v = (nbo << 16) - (uint32_t)t.dnb[(size_t)s];
-    return (uint32_t)t.state[(size_t)((v >> nbo) + (uint32_t)t.dfs[(size_t)s])];
-  };
-  auto encode = [&](const FseEnc &t, uint32_t &st, int s) {
-    const uint32_t nbo = (st + (uint32_t)t.dnb[(size_t)s]) >> 16;
-    bw.add(st, (int)nbo);
-    st = t.state[(size_t)((st >> nbo) + (uint32_t)t.dfs[(size_t)s])];
-  };
-  auto extras = [&](size_t k) {
-    const int lb = zstd_extra_bits(llc[k], false), mb = zstd_extra_bits(mlc[k], true);
-    bw.add(seqs[k].ll, lb);   // the baselines' low bits are zero: the extra bits are the value's low bits
-    bw.add(seqs[k].ml - 3, mb);
-    bw.add(seqs[k].off + 3, ofc[k]);
-  };
-  uint32_t sml = init(tml, mlc[ns - 1]), sof = init(tof, ofc[ns - 1]), sll = init(tll, llc[ns - 1]);
-  extras(ns - 1);
-  for (size_t k = ns - 1; k-- > 0;) {
-    encode(tof, sof, ofc[k]);
-    encode(tml, sml, mlc[k]);
-    encode(tll, sll, llc[k]);
-    extras(k);
-  }
-  bw.add(sml, tml.log);
-  bw.add(sof, tof.log);
-  bw.add(sll, tll.log);
-  bw.close();
+  obz::zstd_sequences(sink, seqs.data(), (uint32_t)seqs.size(), fse);
 }
 
 void zstd_compress_frame(const uint8_t *src, int64_t n, std::vector<uint8_t> &o) {
-  constexpr int64_t kBlock = 128 * 1024;
   o.clear();
-  o.reserve((size_t)(n + n / kBlock * 3 + 32));
-  const uint8_t magic[4] = {0x28, 0xb5, 0x2f, 0xfd};
-  o.insert(o.end(), magic, magic + 4);
-  const int fcs_bytes = n < 256 ? 1 : n < 65536 + 256 ? 2 : n <= 0xffffffffll ? 4 : 8;
-  o.push_back((uint8_t)(((fcs_bytes == 1 ? 0 : fcs_bytes == 2 ? 1 : fcs_bytes == 4 ? 2 : 3) << 6) | 0x20));   // Single_Segment
-  const uint64_t fcs = (uint64_t)n - (fcs_bytes == 2 ? 256 : 0);
-  for (int k = 0; k < fcs_bytes; ++k) o.push_back((uint8_t)(fcs >> (8 * k)));
+  o.reserve((size_t)(n + n / obz::kZstdBlock * 3 + 32));
+  ByteSink sink{o};
+  obz::zstd_frame_header(sink, n);
   std::vector<uint8_t> blk;
   int64_t at = 0;
   do {
-    const int64_t len = std::min<int64_t>(kBlock, n - at);
-    const uint32_t last = at + len == n ? 1u : 0u;
+    const int64_t len = std::min<int64_t>(obz::kZstdBlock, n - at);
     if (len > 0) zstd_compressed_block(src + at, len, blk);
     const bool raw = len == 0 || (int64_t)blk.size() >= len;
-    const uint32_t bh = last | ((raw ? 0u : 2u) << 1) | ((uint32_t)(raw ? len : (int64_t)blk.size()) << 3);
-    o.push_back((uint8_t)bh);
-    o.push_back((uint8_t)(bh >> 8));
-    o.push_back((uint8_t)(bh >> 16));
+    obz::zstd_block_header(sink, at + len == n, raw, (uint32_t)(raw ? len : (int64_t)blk.size()));
     if (raw) o.insert(o.end(), src + at, src + at + len);
     else o.insert(o.end(), blk.begin(), blk.end());
     at += len;

@@ -1,5 +1,7 @@
 #include "ob_gpu_partition_merger.h"
 
+#include <cuda_runtime_api.h>   // the device buffer of a compressed group (obgpu_compress_blocks writes into caller memory)
+
 #include <algorithm>
 
 namespace oceanbase {
@@ -111,9 +113,43 @@ int ObGpuPartitionMajorMerger::get_next_rows(int64_t max_rows, ObGpuMergedRows &
   return ret;
 }
 
+// The device blocks of one encoded group in stored form (obgpu_compress_blocks into a temporary device buffer), fetched to the
+// host as the group's image, offsets and sizes; blocks of size 0 stay size 0.
+static int fetch_compressed(obgpu_ctx *ctx, obgpu_encoded *enc, int32_t n_blocks, int32_t compressor, int32_t align,
+                            ObGpuEncodedColumnGroup &o) {
+  const void *img = nullptr;
+  const int64_t *off = nullptr;
+  const uint32_t *sz = nullptr;
+  int ret = obgpu_encoded_device_image(enc, &img, &off, &sz);
+  int64_t cap = 0, used = 0;
+  if (OB_SUCCESS == ret) ret = obgpu_compress_blocks(ctx, img, off, sz, n_blocks, compressor, align, nullptr, 0, nullptr, nullptr, &cap);
+  void *d_out = nullptr, *d_tab = nullptr;
+  if (OB_SUCCESS == ret && (cudaMalloc(&d_out, (size_t)std::max<int64_t>(cap, 1)) != cudaSuccess ||
+                            cudaMalloc(&d_tab, (size_t)n_blocks * 12) != cudaSuccess))
+    ret = OBGPU_ALLOCATE_MEMORY_FAILED;
+  int64_t *d_off = (int64_t *)d_tab;
+  uint32_t *d_sz = (uint32_t *)(d_off + n_blocks);
+  if (OB_SUCCESS == ret) ret = obgpu_compress_blocks(ctx, img, off, sz, n_blocks, compressor, align, d_out, cap, d_off, d_sz, &used);
+  std::vector<uint32_t> sizes((size_t)n_blocks);
+  if (OB_SUCCESS == ret) {   // obgpu_compress_blocks has synchronised its stream: the output is complete
+    o.image_.resize((size_t)used);
+    o.offsets_.resize((size_t)n_blocks);
+    o.sizes_.resize((size_t)n_blocks);
+    if (cudaMemcpy(o.image_.data(), d_out, (size_t)used, cudaMemcpyDeviceToHost) != cudaSuccess ||
+        cudaMemcpy(o.offsets_.data(), d_off, (size_t)n_blocks * 8, cudaMemcpyDeviceToHost) != cudaSuccess ||
+        cudaMemcpy(sizes.data(), d_sz, (size_t)n_blocks * 4, cudaMemcpyDeviceToHost) != cudaSuccess)
+      ret = OBGPU_ERR_SYS;
+    for (size_t b = 0; b < sizes.size(); ++b) o.sizes_[b] = sizes[b];
+  }
+  if (d_out) cudaFree(d_out);
+  if (d_tab) cudaFree(d_tab);
+  return ret;
+}
+
 int ObGpuPartitionMajorMerger::write_column_groups(const std::vector<ObGpuColumnGroup> &groups, int64_t rows_per_block, int32_t align,
-                                                   std::vector<ObGpuEncodedColumnGroup> &out) {
+                                                   std::vector<ObGpuEncodedColumnGroup> &out, int32_t compressor) {
   int ret = OB_SUCCESS;
+  const bool compress = compressor != OBGPU_COMPRESSOR_NONE;
   if (!merged_) {
     ret = OB_NOT_INIT;
   } else if (groups.empty() || rows_per_block <= 0 || info_.out_rows <= 0) {
@@ -137,11 +173,15 @@ int ObGpuPartitionMajorMerger::write_column_groups(const std::vector<ObGpuColumn
     if (OB_SUCCESS != ret) break;
     o.row_count_ = info.total_rows;
     o.host_encoded_blocks_ = info.n_host_blocks;
-    o.offsets_.resize((size_t)info.n_blocks);
-    o.sizes_.resize((size_t)info.n_blocks);
-    o.image_.resize((size_t)info.image_size);
     o.column_checksums_.resize(cg.cols_.size());
-    ret = obgpu_encoded_fetch(enc[g], o.image_.data(), info.image_size, o.offsets_.data(), o.sizes_.data(), info.n_blocks);
+    if (compress) {
+      ret = fetch_compressed(ctx_, enc[g], info.n_blocks, compressor, align, o);
+    } else {
+      o.offsets_.resize((size_t)info.n_blocks);
+      o.sizes_.resize((size_t)info.n_blocks);
+      o.image_.resize((size_t)info.image_size);
+      ret = obgpu_encoded_fetch(enc[g], o.image_.data(), info.image_size, o.offsets_.data(), o.sizes_.data(), info.n_blocks);
+    }
     if (OB_SUCCESS == ret) ret = obgpu_encoded_column_checksums(enc[g], o.column_checksums_.data());
     if (OB_SUCCESS == ret && info.n_host_blocks > 0) {
       // the blocks the device left out (ObRawEncoder stores a NULL-dominated column as var-length cells): their rows come
@@ -175,6 +215,13 @@ int ObGpuPartitionMajorMerger::write_column_groups(const std::vector<ObGpuColumn
             image.resize(at + (size_t)bound);
             int64_t sz = 0;
             ret = obgpu_writer_encode_block(in.data(), (int32_t)nc, cg.rowkey_col_cnt_, 0, n, image.data() + at, bound, &sz);
+            if (OB_SUCCESS == ret && compress) {   // the host writer's compressor, which the device's matches byte for byte
+              std::vector<uint8_t> plain(image.begin() + (std::ptrdiff_t)at, image.begin() + (std::ptrdiff_t)(at + (size_t)sz));
+              const int64_t zero = 0;
+              int64_t zoff = 0, zsz = 0, used = 0;
+              ret = obgpu_writer_compress_blocks(plain.data(), &zero, &sz, 1, compressor, 1, image.data() + at, bound, &zoff, &zsz, &used);
+              sz = zsz;
+            }
             if (OB_SUCCESS == ret) { image.resize(at + (size_t)sz); o.sizes_[(size_t)b] = sz; }
           }
         }

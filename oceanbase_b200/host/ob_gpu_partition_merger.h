@@ -89,8 +89,12 @@ public:
   // the merged stream -- produced once by merge_partition -- is replayed into the writer of every column group. Here a
   // writer is the device encoder (obgpu_merge_result_encode): the rows never leave the device as rows, each group comes back
   // as reference-format micro-blocks (every column RAW) + its column checksums. rows_per_block cuts the blocks.
+  // compressor (ObCompressorType: OBGPU_COMPRESSOR_LZ4 / LZ4_1_9_1 / ZSTD_1_3_8): every group comes back in STORED form
+  // (ObMicroBlockCompressor): the device's blocks compressed on the device (obgpu_compress_blocks) before the fetch, the
+  // blocks left to the host writer compressed by obgpu_writer_compress_blocks; byte for byte obgpu_writer_compress_blocks
+  // over the plain image. OBGPU_COMPRESSOR_NONE: plain blocks.
   int write_column_groups(const std::vector<ObGpuColumnGroup> &groups, int64_t rows_per_block, int32_t align,
-                          std::vector<ObGpuEncodedColumnGroup> &out);
+                          std::vector<ObGpuEncodedColumnGroup> &out, int32_t compressor = OBGPU_COMPRESSOR_NONE);
   void reset();
 
 private:
