@@ -1819,6 +1819,15 @@ extern "C" {
 
 const char *obgpu_version(void) { return "obgpu_scan 0.1 (sm_90a, cuda " "12.9" ")"; }
 
+#ifdef OBGPU_PIPE_CLOCKS
+// Instrumented builds only: copies the pipe kernels' cycle sums (g_pipe_clocks, scan_small.cuh) to out[6] and zeroes them.
+int obgpu_pipe_clocks(unsigned long long *out) {
+  if (cudaMemcpyFromSymbol(out, g_pipe_clocks, sizeof(g_pipe_clocks)) != cudaSuccess) return OBGPU_ERR_SYS;
+  static const unsigned long long zero[6] = {0};
+  return cudaMemcpyToSymbol(g_pipe_clocks, zero, sizeof(g_pipe_clocks)) == cudaSuccess ? OBGPU_SUCCESS : OBGPU_ERR_SYS;
+}
+#endif
+
 int obgpu_ctx_create(int device, obgpu_ctx **out) {
   if (!out) return OBGPU_INVALID_ARGUMENT;
   int n = 0;

@@ -14,7 +14,9 @@
 //                               as obgpu_count_kernel (K4 / K6 / K9 / K14)
 //   obgpu_project_pipe_kernel : stages the block's bitmap words and the projected columns' byte ranges; a projected
 //                               VARCHAR dictionary column needs only its refs and its offset array (VEC_DISCRETE
-//                               output is pointers into the caller's block: the dictionary's bytes are never read)
+//                               output is pointers into the caller's block: the dictionary's bytes are never read).
+//                               "Flat" columns (project_flat) are decoded in one pass over (column, selected row)
+//                               items, the others column after column
 #pragma once
 
 __device__ __forceinline__ void cp_async16(uint32_t saddr, const void *g) {
@@ -28,6 +30,27 @@ __device__ __forceinline__ void cp_async4(uint32_t saddr, const void *g) {
 }
 __device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
 __device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.wait_group 0;" ::: "memory"); }
+
+// Where a warp's pipeline iteration goes (tools/scan_kernel_split.py builds a separate library with -DOBGPU_PIPE_CLOCKS; the
+// product library never carries the stamps): per kernel, summed over the warps in clock64 cycles,
+// [wait for regions(b) / meta(b + 1) | issue regions(b + 1) + meta(b + 2) | everything, loop start to end].
+#ifdef OBGPU_PIPE_CLOCKS
+__device__ unsigned long long g_pipe_clocks[2][3];
+#define PIPE_CLOCK_START() const long long pclk_t0 = clock64(); long long pclk_wait = 0, pclk_issue = 0, pclk_a = 0, pclk_b = 0
+#define PIPE_CLOCK_AT(v) v = clock64()
+#define PIPE_CLOCK_ADD(acc, from) acc += clock64() - (from)
+#define PIPE_CLOCK_STOP(k)                                                                   \
+  if (lane == 0) {                                                                           \
+    atomicAdd(&g_pipe_clocks[k][0], (unsigned long long)pclk_wait);                          \
+    atomicAdd(&g_pipe_clocks[k][1], (unsigned long long)pclk_issue);                         \
+    atomicAdd(&g_pipe_clocks[k][2], (unsigned long long)(clock64() - pclk_t0));              \
+  }
+#else
+#define PIPE_CLOCK_START()
+#define PIPE_CLOCK_AT(v)
+#define PIPE_CLOCK_ADD(acc, from)
+#define PIPE_CLOCK_STOP(k)
+#endif
 
 constexpr int kPipeMaxFilterCols = 8;
 constexpr uint32_t kCountHdrBytes = 64u;   // count region slot: deltas + flags | regions
@@ -274,17 +297,22 @@ __global__ void __launch_bounds__(kThreads) obgpu_count_pipe_kernel(const __grid
   issue_meta(blk + nwarps_total, 1);
   cp_async_commit();
   int it = 0;
+  PIPE_CLOCK_START();
   for (; blk < p.n_blocks; blk += nwarps_total, ++it) {
     const int ms = it % 3, rsl = it & 1;
+    PIPE_CLOCK_AT(pclk_a);
     cp_async_wait_all();
     mbar_wait(bars + rsl, (uint32_t)(it >> 1) & 1u);
     __syncwarp();
+    PIPE_CLOCK_ADD(pclk_wait, pclk_a);
+    PIPE_CLOCK_AT(pclk_b);
     const int b2 = blk + 2 * nwarps_total;
     if (p.blk_const != nullptr && b2 < p.n_blocks) v_next2 = p.blk_const[b2];
     issue_regions(blk + nwarps_total, (it + 1) % 3, rsl ^ 1, v_next);
     cp_async_commit();
     issue_meta(b2, (it + 2) % 3);
     cp_async_commit();
+    PIPE_CLOCK_ADD(pclk_issue, pclk_b);
 
     // ---- block `blk` from shared memory -------------------------------------------------------------------------
     const uint8_t *m = meta0 + (uint32_t)ms * p.pc_meta_bytes;
@@ -415,6 +443,7 @@ __global__ void __launch_bounds__(kThreads) obgpu_count_pipe_kernel(const __grid
     if (lane == 0) p.counts[blk] = cnt;
     __syncwarp();   // every lane is done with this iteration's slots before the next iteration refills them
   }
+  PIPE_CLOCK_STOP(0);
   cp_async_wait_all();
 }
 
@@ -447,6 +476,112 @@ __device__ __forceinline__ void project_str_dict_shallow(const ScanParams &p, co
   if (saw_null) p.has_null[pc] = 1;
 }
 #undef ROW
+
+// "Flat" projected columns: a row's output is one ref / value load plus at most two dictionary loads, with no per-block
+// table to build first -- K_BITS without ext bits, sign fix or replaced NULLs, K_DICT over a fixed-width integer
+// dictionary, K_DICT over a variable-length string dictionary (pointer + length, as project_str_dict_shallow). Lane pc turns
+// the column's plan into a FlatCol entry once per block, written over the plan itself in the block's meta slot (no extra
+// shared memory: a table of its own per warp made the kernel slower, fewer warps fit an SM); the list of flat columns goes over the
+// block record at the slot's start, already copied to registers. Then the lanes walk all (column, selected row) items together.
+enum : uint8_t { FLAT_BITS = 0, FLAT_INT_DICT = 1, FLAT_STR_DICT = 2 };
+struct FlatCol {
+  uint64_t add;        // K_BITS / integer dictionary: the plan's base; string dictionary: string address of its var data
+  uint64_t mask;       // integer dictionary with sign fix: int_mask, else 0
+  uint8_t *out;        // output at the block's first selected row
+  int32_t *olen;       // string dictionary: lengths at the block's first selected row
+  uint32_t vbit, width, stride;   // value / ref of row r at staged bit vbit + r * stride, width bits
+  uint32_t dcount, dbit, dbits;   // dictionary: entries, staged bit of entry 0 (string: END offsets), bits per entry
+  uint32_t last_end;   // string dictionary: END of the last entry, relative to the var data
+  uint8_t kind, elem_len, pc, pad_;
+};
+static_assert(sizeof(FlatCol) <= sizeof(ColDesc), "a flat entry replaces its column's plan");
+static_assert(kMetaPlans >= kMaxProj, "the flat column list (one byte per column) fits before the plans");
+
+__device__ __forceinline__ bool flat_kind(const ColDesc &d) {
+  if (d.kind == K_BITS) return d.sc != 5 && d.ext_bit == 0 && !d.sign_fix && !d.var_is_last;
+  if (d.kind == K_DICT) return d.sc == 5 ? !d.dict_fixed : d.dict_data_size <= 8u;
+  return false;
+}
+
+// Entry of projected column pc (flat_kind) from its plan and its staged byte ranges (slot deltas d0, d1). Not inlined: once
+// per block, and inlined into obgpu_project_pipe_kernel it costs the kernel spills at 64 registers.
+// dst overlays the plan d: the entry is built in registers and stored with memcpy, whose byte stores may alias any type, so
+// no load of the plan can move past them.
+__device__ __noinline__ void flat_fill(const ScanParams &p, const ColDesc &d, int pc, uint32_t rs_addr, int32_t d0, int32_t d1,
+                                       int64_t base, uint64_t blk_addr, void *dst) {
+  FlatCol f;
+  const uint32_t s0 = (rs_addr + (uint32_t)d0) * 8u;
+  uint32_t rbit = s0, ibit = s0;
+  f.kind = d.kind == K_BITS ? FLAT_BITS : d.sc == 5 ? FLAT_STR_DICT : FLAT_INT_DICT;
+  if (f.kind == FLAT_STR_DICT && d0 != d1) {
+    // which delta belongs to the refs: with two ranges they are ordered by block offset (proj_ranges)
+    const uint32_t s1 = (rs_addr + (uint32_t)d1) * 8u;
+    if ((d.val_bit >> 3) < d.dict_payload) ibit = s1;
+    else rbit = s1;
+  }
+  f.elem_len = f.kind == FLAT_STR_DICT ? 8u : d.elem_len;
+  f.pc = (uint8_t)pc;
+  f.pad_ = 0;
+  f.out = reinterpret_cast<uint8_t *>(p.out_data[pc]) + base * (int64_t)f.elem_len;
+  f.olen = f.kind == FLAT_STR_DICT ? p.out_lens[pc] + base : nullptr;
+  f.vbit = rbit + d.val_bit;
+  f.width = d.width;
+  f.stride = d.stride;
+  f.dcount = d.dict_count;
+  f.dbit = ibit + d.dict_payload * 8u;
+  f.dbits = d.dict_data_size * 8u;
+  f.last_end = d.dict_end - d.dict_var;
+  f.add = f.kind == FLAT_STR_DICT ? blk_addr + d.dict_var : d.base;
+  f.mask = f.kind == FLAT_INT_DICT && d.sign_fix ? d.int_mask : 0ull;
+  memcpy(dst, &f, sizeof(FlatCol));
+}
+
+// Item k = f * cnt + j (flat column f, selected row j); lane l starts at item l and steps by 32.
+// Flat column f is the entry over plan cols[f] of `plans`.
+__device__ __forceinline__ void project_flat(const ScanParams &p, const ColDesc *plans, const uint8_t *cols, uint32_t nflat,
+                                             const uint16_t *sel, uint32_t cnt, int64_t base, bool all_rows, int lane) {
+  const uint32_t qf = 32u / cnt, qj = 32u % cnt;
+  uint32_t f = (uint32_t)lane / cnt, j = (uint32_t)lane % cnt;
+  for (; f < nflat; f += qf, j += qj) {
+    if (j >= cnt) { j -= cnt; ++f; if (f >= nflat) break; }
+    const FlatCol &c = *reinterpret_cast<const FlatCol *>(plans + cols[f]);
+    const uint32_t row = all_rows ? j : (uint32_t)sel[j];
+    const uint32_t at = c.vbit + row * c.stride, width = c.width;
+    bool is_null = false;
+    uint64_t v;
+    if (c.kind == FLAT_BITS) {
+      v = (width <= 32u ? (uint64_t)sbits32(at, width) : sbits(at, width)) + c.add;
+    } else {
+      const uint32_t ref = sbits32(at, width), dbits = c.dbits;
+      is_null = ref >= c.dcount;
+      if (c.kind == FLAT_STR_DICT) {
+        uint32_t off = 0, end = 0;
+        if (!is_null) {
+          off = ref == 0 ? 0u : sbits32(c.dbit + (ref - 1u) * dbits, dbits);
+          end = ref == c.dcount - 1u ? c.last_end : sbits32(c.dbit + ref * dbits, dbits);
+        }
+        __stcs(&c.olen[j], is_null ? 0 : (int32_t)(end - off));
+        v = is_null ? 0ull : c.add + off;
+      } else if (is_null) {
+        v = 0;
+      } else {
+        const uint32_t e = c.dbit + ref * dbits;
+        v = (dbits <= 32u ? (uint64_t)sbits32(e, dbits) : sbits(e, dbits)) + c.add;
+        v = sign_fix(c.mask, v);
+      }
+    }
+    const uint32_t el = c.elem_len;
+    if (el == 8u) __stcs(reinterpret_cast<uint64_t *>(c.out) + j, v);
+    else if (el == 4u) __stcs(reinterpret_cast<uint32_t *>(c.out) + j, (uint32_t)v);
+    else __stcs(reinterpret_cast<uint8_t *>(c.out) + j, (uint8_t)v);
+    if (is_null) {
+      const int pc = c.pc;
+      const int64_t o = base + (int64_t)j;
+      atomicOr(&p.out_nulls[pc][o >> 5], 1u << (o & 31));
+      p.has_null[pc] = 1;
+    }
+  }
+}
 
 __global__ void __launch_bounds__(kThreads) obgpu_project_pipe_kernel(const __grid_constant__ ScanParams p) {
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -543,15 +678,20 @@ __global__ void __launch_bounds__(kThreads) obgpu_project_pipe_kernel(const __gr
   issue_meta(blk + nwarps_total, 1);
   cp_async_commit();
   int it = 0;
+  PIPE_CLOCK_START();
   for (; blk < p.n_blocks; blk += nwarps_total, ++it) {
     const int ms = it % 3, rsl = it & 1;
+    PIPE_CLOCK_AT(pclk_a);
     cp_async_wait_all();
     mbar_wait(bars + rsl, (uint32_t)(it >> 1) & 1u);
     __syncwarp();
+    PIPE_CLOCK_ADD(pclk_wait, pclk_a);
+    PIPE_CLOCK_AT(pclk_b);
     issue_regions(blk + nwarps_total, (it + 1) % 3, rsl ^ 1);
     cp_async_commit();
     issue_meta(blk + 2 * nwarps_total, (it + 2) % 3);
     cp_async_commit();
+    PIPE_CLOCK_ADD(pclk_issue, pclk_b);
 
     uint8_t *m = meta0 + (uint32_t)ms * p.pp_meta_bytes;
     uint8_t *rs = reg0 + (uint32_t)rsl * p.pp_region_bytes;
@@ -592,7 +732,18 @@ __global__ void __launch_bounds__(kThreads) obgpu_project_pipe_kernel(const __gr
     c.rle_slot_bytes = 0;
     c.rle_starts_bytes = p.words_cap * 4u;
     const uint64_t blk_addr = block_string_addr(p, blk, rec.off);
+    const bool flat = lane < np && plans[lane].ok && !((badmask >> lane) & 1u) && flat_kind(plans[lane]);
+    const uint32_t flatmask = __ballot_sync(0xffffffffu, flat);
+    if (flatmask != 0u) {
+      if (flat) {
+        flat_fill(p, plans[lane], lane, smem_u32(rs), hdr[2 * lane], hdr[2 * lane + 1], base, blk_addr, plans + lane);
+        m[__popc(flatmask & ((1u << lane) - 1u))] = (uint8_t)lane;
+      }
+      __syncwarp();
+      project_flat(p, plans, m, (uint32_t)__popc(flatmask), sel, cnt, base, all_rows, lane);
+    }
     for (int pc = 0; pc < np; ++pc) {
+      if ((flatmask >> pc) & 1u) continue;
       ColDesc *wdesc = plans + pc;
       if (!wdesc->ok || ((badmask >> pc) & 1u)) {
         if (lane == 0) atomicOr(p.status, ST_UNSUPPORTED);
@@ -617,5 +768,6 @@ __global__ void __launch_bounds__(kThreads) obgpu_project_pipe_kernel(const __gr
     }
     __syncwarp();
   }
+  PIPE_CLOCK_STOP(1);
   cp_async_wait_all();
 }
