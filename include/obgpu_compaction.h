@@ -195,6 +195,18 @@ int obgpu_encode_columns(obgpu_ctx *ctx, const obgpu_encode_col *cols, int32_t n
  * column (a column group of a column-oriented merge is one call with the group's columns: ObWriteHelper::project). */
 int obgpu_merge_result_encode(obgpu_merge_result *res, const int32_t *result_cols, const int32_t *obj_types, int32_t n_cols,
                               int32_t rowkey_col_cnt, int64_t rows_per_block, int32_t align, obgpu_encoded **out);
+/* The same with a codec per column: encodings[i] is OBGPU_ENC_RAW or OBGPU_ENC_AUTO (the codec of the column is chosen per
+ * micro-block among RAW / DICT / RLE / CONST / INTEGER_BASE_DIFF the way ObMicroBlockEncoder::choose_encoder does,
+ * ob_micro_block_encoder.cpp:1259-1366,1603-1823); encodings == NULL: every column RAW (the calls above). The blocks equal
+ * obgpu_writer_encode_table byte for byte for the same rows with the same per-column encoding: blocks, offsets and sizes, at
+ * every align. A block in which a column stored RAW would be var-stored is left to the host writer (size 0); with AUTO that
+ * happens only when AUTO picks RAW for that column. Any other OBGPU_ENC_* returns OBGPU_NOT_SUPPORTED before any launch, as
+ * does a rows_per_block / column count whose block does not fit one CTA's shared memory (AUTO columns need more of it). */
+int obgpu_encode_columns_ex(obgpu_ctx *ctx, const obgpu_encode_col *cols, const int32_t *encodings, int32_t n_cols,
+                            int32_t rowkey_col_cnt, int64_t total_rows, int64_t rows_per_block, int32_t align, obgpu_encoded **out);
+int obgpu_merge_result_encode_ex(obgpu_merge_result *res, const int32_t *result_cols, const int32_t *obj_types,
+                                 const int32_t *encodings, int32_t n_cols, int32_t rowkey_col_cnt, int64_t rows_per_block,
+                                 int32_t align, obgpu_encoded **out);
 typedef struct obgpu_encoded_info {
   int64_t image_size;    /* bytes of the image (aligned block slots)          */
   int64_t total_rows;

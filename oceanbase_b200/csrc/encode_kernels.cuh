@@ -1,4 +1,4 @@
-// Phase B of the compaction on the device: merged column arrays -> PAX micro-blocks (every column RAW), byte for byte the
+// Phase B of the compaction on the device: merged column arrays -> PAX micro-blocks (RAW columns; AUTO below), byte for byte the
 // blocks the host writer (sstable_writer.cpp: BlockBuilder::encode_raw / build / finish_header) produces for the same rows,
 // plus the column checksums of the rows (K16). One kernel, one CTA per micro-block, input read once, output written once:
 //
@@ -14,6 +14,14 @@
 //   offset  : decoupled look-back over the aligned block sizes (tickets in scheduling order, one 64-bit flag per block), resolved
 //             by thread 0 while the other warps pack
 //   store   : header + checksums, then ONE bulk copy (TMA, cp.async.bulk shared -> global) of the aligned slot
+//
+// Columns asking for OBGPU_ENC_AUTO run the AUTO instantiation, the device form of the writer's build_int_dict +
+// choose_auto_encoding (sstable_writer.cpp): per AUTO column a block-wide stable sort of (sort key, row) in shared memory
+// (bitonic over the next power of two; the sort key is the store image with the sign bit flipped for the signed class, the
+// writer's sorted order) gives the distinct values, their frequencies and first rows, the sorted ref of every row and the runs;
+// warp 0 then evaluates the writer's estimates in the writer's order and lays out the chosen codec, and the pack writes it as
+// BlockBuilder::encode_dict / encode_rle / encode_const / encode_base_diff do (re-sorting the columns that store a dictionary).
+// RAW-only calls keep the RAW instantiation.
 #pragma once
 #include <map>
 #include <mutex>
@@ -30,8 +38,9 @@ struct ColSpec {
   const int64_t *vals;
   const uint8_t *nulls;
   uint64_t store_mask;     // low type_store_size bytes (ColCtx::uval)
-  uint8_t obj_type, byte_only, datum_len, pad0;
-  uint32_t pad1;
+  uint8_t obj_type, byte_only, datum_len, is_auto;
+  uint8_t store_size, is_signed;   // type_store_size; store class 1 (signed)
+  uint16_t pad1;
 };
 
 struct Params {
@@ -39,7 +48,7 @@ struct Params {
   int32_t n_cols, rowkey_cnt, n_blocks, want_checksums;
   int64_t total_rows, rows_per_block;
   uint32_t align, slot_cap;          // slot_cap: bytes of the shared-memory block image (multiple of align)
-  uint32_t lw_max, pad;              // xpow32 holds (kThreads - 1) * lw_max + 1 entries
+  uint32_t lw_max, sort_cap;         // xpow32 holds (kThreads - 1) * lw_max + 1 entries; sort_cap: AUTO sort length (power of 2)
   uint8_t *image;
   int64_t *blk_off;                  // [n_blocks]
   uint32_t *blk_size;                // [n_blocks] exact bytes, 0: left to the host writer
@@ -90,7 +99,409 @@ struct ColLayout {
   uint8_t attr, size, bp, has_null;
 };
 
-template <bool CKSUM>
+// ---- OBGPU_ENC_AUTO ----------------------------------------------------------------------------------------------------------
+// What the analysis finds in one AUTO column of a block, and the layout the plan picks for it.
+struct AutoCol {
+  unsigned long long kmin, kmax;   // smallest / largest sort key of the non-NULL cells
+  uint32_t d;                      // distinct non-NULL values
+  uint32_t fmax;                   // largest frequency of a value
+  uint32_t runs, last_run;         // runs over the refs in row order (a NULL is ref d), first row of the last run
+  uint32_t row_e, row_w;           // last row off the constant, for the estimate's / encode_const's constant
+  uint32_t ref_w;                  // encode_const's constant: smallest sorted ref among the most frequent (d: NULL)
+  uint32_t exc, len;               // CONST exceptions; the column header's length_
+  uint8_t codec, size, bp, dsz, rib, refb, pad[2];   // chosen codec, its cell width (bits when bp), dict width, row-id / ref bytes
+};
+
+struct AutoScratch {
+  unsigned long long *sk;   // [sort_cap] sort keys, sorted
+  uint32_t *sr;             // [sort_cap] rows, sorted with the keys (0xffffffff: padding and NULL rows)
+  uint32_t *hs;             // [sort_cap] scan scratch
+  uint32_t *a;              // [rows] sorted ref of every row (NULL: d)
+  uint32_t *b;              // [rows] 1 on the first occurrence of a value (scanned: distinct values seen up to the row)
+  uint32_t *hp;             // [rows + 1] sorted position of each value's first entry; hp[d] = non-NULL rows
+  uint32_t *red;            // [kWarps] reduction scratch
+};
+
+__device__ __forceinline__ uint32_t bpis(unsigned long long v) {   // get_byte_packed_int_size
+  return v <= 0xffull ? 1u : v <= 0xffffull ? 2u : v <= 0xffffffffull ? 4u : 8u;
+}
+__device__ __forceinline__ uint32_t int_size_bytes(unsigned long long v) {   // get_int_size
+  const uint32_t bits = v == 0 ? 1u : 64u - (uint32_t)__clzll((long long)v);
+  return (bits + 7u) / 8u;
+}
+
+// OR the low w bits of x (w <= 64, x holds no higher bit) into the image at bit address b (the image is zeroed first)
+__device__ __forceinline__ void or_bits(uint32_t *img32, uint32_t b, uint32_t w, unsigned long long x) {
+  if (x == 0) return;
+  const uint32_t sh = b & 31u;
+  uint32_t *q = img32 + (b >> 5);
+  atomicOr(q, (uint32_t)(x << sh));
+  if (sh + w > 32u) atomicOr(q + 1, (uint32_t)(x >> (32u - sh)));
+  if (sh + w > 64u) atomicOr(q + 2, (uint32_t)(x >> (64u - sh)));
+}
+__device__ __forceinline__ void put_bytes(uint32_t *img32, uint32_t at, uint32_t n, unsigned long long x) {
+  or_bits(img32, at * 8u, 8u * n, n >= 8u ? x : (x & ((1ull << (8u * n)) - 1ull)));
+}
+
+__device__ __forceinline__ uint32_t blk_sum(uint32_t v, uint32_t *red) {
+  v = __reduce_add_sync(0xffffffffu, v);
+  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = v;
+  __syncthreads();
+  uint32_t r = 0;
+  for (int w = 0; w < kWarps; ++w) r += red[w];
+  __syncthreads();
+  return r;
+}
+__device__ __forceinline__ uint32_t blk_max(uint32_t v, uint32_t *red) {
+  v = __reduce_max_sync(0xffffffffu, v);
+  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = v;
+  __syncthreads();
+  uint32_t r = 0;
+  for (int w = 0; w < kWarps; ++w) r = max(r, red[w]);
+  __syncthreads();
+  return r;
+}
+__device__ __forceinline__ uint32_t blk_min(uint32_t v, uint32_t *red) {
+  v = __reduce_min_sync(0xffffffffu, v);
+  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = v;
+  __syncthreads();
+  uint32_t r = 0xffffffffu;
+  for (int w = 0; w < kWarps; ++w) r = min(r, red[w]);
+  __syncthreads();
+  return r;
+}
+
+// inclusive prefix sum of x[0, m) in place: one contiguous chunk per thread
+__device__ void blk_scan(uint32_t *x, uint32_t m, uint32_t *red) {
+  const uint32_t tid = threadIdx.x, lane = tid & 31u, per = (m + kThreads - 1u) / kThreads;
+  const uint32_t lo = min(tid * per, m), hi = min(lo + per, m);
+  uint32_t s = 0;
+  for (uint32_t i = lo; i < hi; ++i) s += x[i];
+  uint32_t incl = s;
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) {
+    const uint32_t u = __shfl_up_sync(0xffffffffu, incl, o);
+    if (lane >= (uint32_t)o) incl += u;
+  }
+  if (lane == 31u) red[tid >> 5] = incl;
+  __syncthreads();
+  uint32_t off = incl - s;
+  for (uint32_t w = 0; w < (tid >> 5); ++w) off += red[w];
+  for (uint32_t i = lo; i < hi; ++i) { off += x[i]; x[i] = off; }
+  __syncthreads();
+}
+
+// Stable sort of the block's non-NULL cells of one column by (sort key, row), then the sorted ref of every row (a), the
+// first occurrences (b) and the first sorted position of every value (hp). Returns the distinct count. Every thread calls it.
+__device__ uint32_t sort_column(const ColSpec &cs, const int64_t row0, const uint32_t n, const uint32_t nn, const uint32_t P,
+                                const AutoScratch &s) {
+  const uint32_t tid = threadIdx.x;
+  const unsigned long long flip = cs.is_signed ? 1ull << (8u * cs.store_size - 1u) : 0ull;
+  for (uint32_t i = tid; i < P; i += kThreads) {
+    unsigned long long k = ~0ull;
+    uint32_t r = 0xffffffffu;
+    if (i < n) {
+      if (!(cs.nulls && cs.nulls[row0 + i] != 0)) { k = ((unsigned long long)cs.vals[row0 + i] & cs.store_mask) ^ flip; r = i; }
+      s.a[i] = 0xffffffffu;
+      s.b[i] = 0u;
+    }
+    s.sk[i] = k;
+    s.sr[i] = r;
+  }
+  __syncthreads();
+  for (uint32_t k = 2; k <= P; k <<= 1) {   // bitonic, ascending; (key, row) pairs are unique, so the order is stable
+    for (uint32_t j = k >> 1; j > 0; j >>= 1) {
+      for (uint32_t i = tid; i < P / 2u; i += kThreads) {
+        const uint32_t lo = ((i & ~(j - 1u)) << 1) | (i & (j - 1u)), hi = lo + j;
+        const unsigned long long ka = s.sk[lo], kb = s.sk[hi];
+        const uint32_t ra = s.sr[lo], rb = s.sr[hi];
+        const bool gt = ka > kb || (ka == kb && ra > rb);
+        if (gt == ((lo & k) == 0)) { s.sk[lo] = kb; s.sk[hi] = ka; s.sr[lo] = rb; s.sr[hi] = ra; }
+      }
+      __syncthreads();
+    }
+  }
+  const uint32_t m = n - nn;
+  for (uint32_t i = tid; i < m; i += kThreads) s.hs[i] = (i == 0 || s.sk[i] != s.sk[i - 1]) ? 1u : 0u;
+  __syncthreads();
+  blk_scan(s.hs, m, s.red);
+  const uint32_t d = m ? s.hs[m - 1] : 0u;
+  for (uint32_t i = tid; i < m; i += kThreads) {
+    const uint32_t seg = s.hs[i] - 1u, r = s.sr[i];
+    s.a[r] = seg;
+    if (i == 0 || s.hs[i - 1] != s.hs[i]) { s.b[r] = 1u; s.hp[seg] = i; }
+  }
+  if (tid == 0) s.hp[d] = m;
+  __syncthreads();
+  for (uint32_t r = tid; r < n; r += kThreads)
+    if (s.a[r] == 0xffffffffu) s.a[r] = d;
+  __syncthreads();
+  return d;
+}
+
+// The analysis of one AUTO column (every thread calls it; thread 0 writes out).
+__device__ void analyze_column(const ColSpec &cs, const int64_t row0, const uint32_t n, const uint32_t nn, const uint32_t P,
+                               const AutoScratch &s, AutoCol &out) {
+  const uint32_t tid = threadIdx.x;
+  const uint32_t d = sort_column(cs, row0, n, nn, P, s);
+  uint32_t f = 0;
+  for (uint32_t v = tid; v < d; v += kThreads) f = max(f, s.hp[v + 1] - s.hp[v]);
+  const uint32_t fmax = blk_max(f, s.red);
+  // the estimate's constant: the most frequent value, ties to the earliest first occurrence; encode_const's: ties to the
+  // smallest sorted ref. NULL is the constant of both only when strictly more frequent.
+  uint32_t fr = 0xffffffffu, sw = 0xffffffffu;
+  for (uint32_t v = tid; v < d; v += kThreads)
+    if (s.hp[v + 1] - s.hp[v] == fmax) { fr = min(fr, s.sr[s.hp[v]]); sw = min(sw, v); }
+  fr = blk_min(fr, s.red);
+  sw = blk_min(sw, s.red);
+  const bool const_null = nn > fmax;
+  const uint32_t se = const_null ? d : s.a[fr], cw = const_null ? d : sw;
+  uint32_t chg = 0, last = 0, re = 0, rw = 0;
+  for (uint32_t r = tid; r < n; r += kThreads) {
+    const uint32_t x = s.a[r];
+    if (r > 0 && x != s.a[r - 1]) { ++chg; last = max(last, r); }
+    if (x != se) re = max(re, r);
+    if (x != cw) rw = max(rw, r);
+  }
+  chg = blk_sum(chg, s.red);
+  last = blk_max(last, s.red);
+  re = blk_max(re, s.red);
+  rw = blk_max(rw, s.red);
+  if (tid == 0) {
+    out.kmin = n > nn ? s.sk[0] : 0ull;
+    out.kmax = n > nn ? s.sk[n - nn - 1] : 0ull;
+    out.d = d;
+    out.fmax = fmax;
+    out.runs = 1u + chg;
+    out.last_run = last;
+    out.row_e = re;
+    out.row_w = rw;
+    out.ref_w = cw;
+  }
+  __syncthreads();
+}
+
+__device__ __forceinline__ long long sign_extend(unsigned long long v, uint32_t ts) {
+  const unsigned long long rev = ts >= 8u ? 0ull : ~((1ull << (8u * ts)) - 1ull);
+  if (rev != 0 && (v & (rev >> 1))) v |= rev;
+  return (long long)v;
+}
+
+// choose_auto_encoding (sstable_writer.cpp) for one integer column of the block, then the chosen codec's layout. Returns
+// the column store's bytes; the RAW layout already in l / var stays when RAW is chosen. Warp 0, one lane per column.
+__device__ uint32_t plan_auto(const ColSpec &cs, AutoCol &A, const uint32_t nrows, const uint32_t nnull,
+                              const unsigned long long mx, const uint32_t ext_bit, ColLayout &l, bool &var, uint32_t raw_bytes) {
+  const long long n = nrows, nn = nnull, ts = cs.store_size, distinct = A.d, eb = ext_bit;
+  const bool ebp = cs.byte_only == 0;
+  bool bp;
+  // ---- RAW (ObRawEncoder::traverse + calc_size)
+  long long raw_size;
+  {
+    long long bp_len = 0, fix_len = 0, raw_var = 0;
+    bool is_var = false;
+    const long long size = packing_size(mx, ebp, bp);
+    if (bp) {
+      if (size * nn > n * 2 * 8) { is_var = true; raw_var = (size / 8 + 1) * (n - nn); }
+      else bp_len = size;
+    } else {
+      fix_len = size;
+    }
+    if (fix_len > 0 && bp_len == 0 && fix_len * nn > n * 2) { is_var = true; fix_len = 0; }
+    raw_size = bp_len > 0 ? bp_len * n / 8 + 1 : (!is_var ? fix_len * n : raw_var + n * 2);
+    raw_size += nn > 0 ? (n * eb + 1) / 8 : 0;   // (n * ext_bit + 1) / 8, as the writer estimates it
+  }
+  // ---- DICT
+  const long long dsz = ebp ? int_size_bytes(mx) : bpis(mx);
+  const long long dict_meta = 9 + dsz * distinct;
+  const long long max_ref = nn > 0 ? distinct : distinct - 1;
+  const unsigned long long ref_v = (unsigned long long)(max_ref > 0 ? max_ref : 0);
+  long long dict_size;
+  bool ref_bp;
+  const long long ref_size = packing_size(ref_v, ebp, ref_bp);
+  dict_size = dict_meta + (ref_bp ? (n * ref_size + 7) / 8 : n * ref_size);
+  // ---- CONST
+  const long long max_cnt = nn > (long long)A.fmax ? nn : (long long)A.fmax, exc = n - max_cnt;
+  const bool const_ok = !(exc > 32 || exc > max(n * 10 / 100, 1ll));
+  long long const_size = 0;
+  if (exc == 0) const_size = (nn == 0 ? ts : 0) + 6;
+  else const_size = 6 + dict_meta + exc * (bpis(A.row_e) + 1);
+  int choose = 0 /*RAW*/;
+  if (distinct <= 1 && const_ok) {
+    choose = 3;
+  } else {
+    long long choose_size = raw_size;
+    const long long acceptable = raw_size / 4;
+    if (dict_size < choose_size) { choose = 1; choose_size = dict_size; }
+    if (distinct <= n / 2) {
+      const long long rle_size = 10 + dict_meta + (long long)A.runs * (bpis(A.last_run) + bpis(ref_v));
+      if (rle_size < choose_size) { choose = 2; choose_size = rle_size; }
+      if (const_ok && const_size < choose_size) { choose = 3; choose_size = const_size; }
+    }
+    if (choose_size > acceptable && distinct > 0) {   // ObIntegerBaseDiffEncoder (no ext-bit term in its estimate)
+      unsigned long long delta, max_unsigned;
+      if (cs.is_signed) {
+        const long long smin = sign_extend(A.kmin ^ (1ull << (8u * ts - 1u)), (uint32_t)ts);
+        const long long smax = sign_extend(A.kmax ^ (1ull << (8u * ts - 1u)), (uint32_t)ts);
+        delta = smin < smax ? (unsigned long long)smax - (unsigned long long)smin : 0ull;
+        max_unsigned = smin < 0 ? ~0ull : (unsigned long long)smax;
+      } else {
+        delta = A.kmin < A.kmax ? A.kmax - A.kmin : 0ull;
+        max_unsigned = A.kmax;
+      }
+      if (delta != 0) {
+        long long orig = packing_size(max_unsigned, true, bp);
+        if (!bp) orig *= 8;
+        long long dbits = packing_size(delta, true, bp);
+        if (!bp) dbits *= 8;
+        if ((orig - dbits) * n > (2 + ts) * 8) {
+          const long long bd_size = (bp ? (n * dbits + 7) / 8 : n * (dbits / 8)) + 2 + ts;
+          if (bd_size < choose_size) { choose = 4; choose_size = bd_size; }
+        }
+      }
+    }
+  }
+  A.codec = (uint8_t)choose;
+  if (choose == 0) return raw_bytes;
+  var = false;
+  l.has_null = nn != 0;
+  A.dsz = (uint8_t)dsz;
+  if (choose == 1) {   // encode_dict: [sorted dict meta][refs, NULL cells included, no ext bits]
+    A.size = (uint8_t)ref_size;
+    A.bp = ref_bp;
+    A.len = (uint32_t)dict_meta;
+    l.attr = (uint8_t)(0x1u | (ref_bp ? 0x4u : 0u));
+    return (uint32_t)dict_size;
+  }
+  if (choose == 2) {   // encode_rle: [header][run rows][run refs][dict meta, first-occurrence order]
+    A.rib = (uint8_t)bpis(A.last_run);
+    A.refb = (uint8_t)bpis(ref_v);
+    if ((long long)A.runs * A.rib > 32767) var = true;   // the writer refuses it (ObRLEDecoder's int16 bound): host block
+    A.len = (uint32_t)(10 + (long long)A.runs * (A.rib + A.refb) + dict_meta);
+    l.attr = 0;
+    return A.len;
+  }
+  if (choose == 3) {   // encode_const: header [+ exceptions + sorted dict meta] or [+ the value]
+    A.exc = (uint32_t)exc;
+    A.rib = (uint8_t)bpis(A.row_w);
+    A.len = exc == 0 ? (uint32_t)(6 + (distinct == 0 ? 0 : ts)) : (uint32_t)(6 + exc * (A.rib + 1) + dict_meta);
+    l.attr = 0;
+    return A.len;
+  }
+  // encode_base_diff: [header][base][ext bits][bit-packed deltas] or [..][byte-packed deltas]
+  unsigned long long delta;
+  if (cs.is_signed) {
+    const unsigned long long f = 1ull << (8u * ts - 1u);
+    delta = (unsigned long long)sign_extend(A.kmax ^ f, (uint32_t)ts) - (unsigned long long)sign_extend(A.kmin ^ f, (uint32_t)ts);
+  } else {
+    delta = A.kmax - A.kmin;
+  }
+  const uint32_t size = packing_size(delta, true, bp);
+  A.size = (uint8_t)size;
+  A.bp = bp;
+  A.len = (uint32_t)(2 + ts);
+  l.size = (uint8_t)size;
+  l.bp = bp;
+  l.attr = (uint8_t)(0x1u | (nn ? 0x2u : 0u) | (bp ? 0x4u : 0u));
+  const unsigned long long bits = (nn ? (unsigned long long)ext_bit * nrows : 0ull) + (bp ? (unsigned long long)size * nrows : 0ull);
+  l.bits_size = (uint32_t)((bits + 7ull) / 8ull);
+  return A.len + l.bits_size + (bp ? 0u : size * nrows);
+}
+
+// DictMetaHeader {version_, row_ref_size_, count_, data_size_, attr_} + the values, dsz bytes each, at byte `at`
+__device__ __forceinline__ void put_dict_header(uint32_t *img32, uint32_t at, uint32_t ref_size, uint32_t count, uint32_t dsz, uint32_t attr) {
+  put_bytes(img32, at + 1u, 1u, ref_size);
+  put_bytes(img32, at + 2u, 4u, count);
+  put_bytes(img32, at + 6u, 2u, dsz);
+  put_bytes(img32, at + 8u, 1u, attr);
+}
+
+// Pack one AUTO column whose codec is not RAW (every thread calls it).
+__device__ void pack_auto(const ColSpec &cs, const AutoCol &A, const ColLayout &l, const int64_t row0, const uint32_t n,
+                          const uint32_t nn, const uint32_t ext_bit, const uint32_t P, const AutoScratch &s, uint32_t *img32) {
+  const uint32_t tid = threadIdx.x, o = l.store_off, dsz = A.dsz;
+  const unsigned long long flip = cs.is_signed ? 1ull << (8u * cs.store_size - 1u) : 0ull;
+  if (A.codec == 4) {   // INTEGER_BASE_DIFF
+    const uint32_t ts = cs.store_size;
+    const unsigned long long base = cs.is_signed ? (unsigned long long)sign_extend(A.kmin ^ flip, ts) : A.kmin;
+    if (tid == 0) {
+      put_bytes(img32, o + 1u, 1u, A.size);
+      put_bytes(img32, o + 2u, ts, base);
+    }
+    const uint32_t bit0 = (o + 2u + ts) * 8u, val0 = bit0 + (nn ? ext_bit * n : 0u);
+    const uint8_t *nl = (cs.nulls && nn) ? cs.nulls + row0 : nullptr;
+    for (uint32_t r = tid; r < n; r += kThreads) {
+      if (nl && nl[r] != 0) { or_bits(img32, bit0 + r * ext_bit, ext_bit, 1ull); continue; }
+      const unsigned long long u = (unsigned long long)cs.vals[row0 + r] & cs.store_mask;
+      const unsigned long long x = (cs.is_signed ? (unsigned long long)sign_extend(u, ts) : u) - base;
+      if (A.bp) or_bits(img32, val0 + r * A.size, A.size, A.size >= 64u ? x : x & ((1ull << A.size) - 1ull));
+      else put_bytes(img32, o + 2u + ts + l.bits_size + r * A.size, min((uint32_t)A.size, 8u), x);
+    }
+    return;
+  }
+  if (A.codec == 3 && A.exc == 0) {   // CONST without exceptions: the value, or const_ref_ 1 when every row is NULL
+    if (tid == 0) {
+      if (A.d == 0) put_bytes(img32, o + 2u, 1u, 1u);
+      put_bytes(img32, o + 4u, 2u, 6u);
+      if (A.d != 0) put_bytes(img32, o + 6u, cs.store_size, A.kmin ^ flip);
+    }
+    return;
+  }
+  const uint32_t d = sort_column(cs, row0, n, nn, P, s);
+  if (A.codec == 1) {   // DICT: sorted dict, then the sorted ref of every row
+    if (tid == 0) put_dict_header(img32, o, A.size, d, dsz, 0x1u | 0x2u);
+    for (uint32_t v = tid; v < d; v += kThreads) put_bytes(img32, o + 9u + v * dsz, dsz, s.sk[s.hp[v]] ^ flip);
+    const uint32_t at = o + A.len;
+    for (uint32_t r = tid; r < n; r += kThreads) {
+      if (A.bp) or_bits(img32, at * 8u + r * A.size, A.size, s.a[r]);
+      else put_bytes(img32, at + r * A.size, A.size, s.a[r]);
+    }
+    return;
+  }
+  if (A.codec == 2) {   // RLE: refs and dict in first-occurrence order
+    blk_scan(s.b, n, s.red);   // b[r]: distinct values whose first occurrence is at or before row r
+    for (uint32_t r = tid; r < n; r += kThreads) s.hs[r] = (r == 0 || s.a[r] != s.a[r - 1]) ? 1u : 0u;
+    __syncthreads();
+    blk_scan(s.hs, n, s.red);
+    const uint32_t runs = A.runs, rib = A.rib, refb = A.refb, head = 10u + runs * (rib + refb);
+    if (tid == 0) {
+      put_bytes(img32, o + 1u, 1u, (rib & 7u) | ((refb & 7u) << 3));
+      put_bytes(img32, o + 2u, 4u, runs);
+      put_bytes(img32, o + 6u, 4u, head);
+      put_dict_header(img32, o + head, 0u, d, dsz, 0x1u);
+    }
+    for (uint32_t r = tid; r < n; r += kThreads) {
+      if (!(r == 0 || s.a[r] != s.a[r - 1])) continue;
+      const uint32_t k = s.hs[r] - 1u, x = s.a[r];
+      const uint32_t ref = x == d ? d : s.b[s.sr[s.hp[x]]] - 1u;
+      put_bytes(img32, o + 10u + k * rib, rib, r);
+      put_bytes(img32, o + 10u + runs * rib + k * refb, refb, ref);
+    }
+    for (uint32_t v = tid; v < d; v += kThreads)
+      put_bytes(img32, o + head + 9u + (s.b[s.sr[s.hp[v]]] - 1u) * dsz, dsz, s.sk[s.hp[v]] ^ flip);
+    return;
+  }
+  // CONST with exceptions: [header][exception refs, u8][exception rows][sorted dict meta]
+  const uint32_t cw = A.ref_w, exc = A.exc, rib = A.rib, head = 6u + exc * (rib + 1u);
+  for (uint32_t r = tid; r < n; r += kThreads) s.hs[r] = s.a[r] != cw ? 1u : 0u;
+  __syncthreads();
+  blk_scan(s.hs, n, s.red);
+  if (tid == 0) {
+    put_bytes(img32, o + 1u, 1u, exc);
+    put_bytes(img32, o + 2u, 1u, cw);
+    put_bytes(img32, o + 3u, 1u, rib & 7u);
+    put_bytes(img32, o + 4u, 2u, head);
+    put_dict_header(img32, o + head, 0u, d, dsz, 0x1u | 0x2u);
+  }
+  for (uint32_t r = tid; r < n; r += kThreads) {
+    if (s.a[r] == cw) continue;
+    const uint32_t k = s.hs[r] - 1u;
+    put_bytes(img32, o + 6u + k, 1u, s.a[r]);
+    put_bytes(img32, o + 6u + exc + k * rib, rib, r);
+  }
+  for (uint32_t v = tid; v < d; v += kThreads) put_bytes(img32, o + head + 9u + v * dsz, dsz, s.sk[s.hp[v]] ^ flip);
+}
+
+template <bool CKSUM, bool AUTO>
 __global__ void __launch_bounds__(kThreads) obgpu_encode_blocks_kernel(const __grid_constant__ Params p) {
   extern __shared__ __align__(128) uint8_t smem[];
   uint32_t *img32 = reinterpret_cast<uint32_t *>(smem);                 // block image, p.slot_cap bytes
@@ -99,6 +510,23 @@ __global__ void __launch_bounds__(kThreads) obgpu_encode_blocks_kernel(const __g
   unsigned long long *s_wmax = reinterpret_cast<unsigned long long *>(smem + p.slot_cap + 4096u);
   uint32_t *s_wnull = reinterpret_cast<uint32_t *>(s_wmax + kWarps * p.n_cols);
   ColLayout *s_lay = reinterpret_cast<ColLayout *>(s_wnull + kWarps * p.n_cols);
+  // AUTO: [n_cols] AutoCol, then the sort scratch (auto_smem_bytes on the host counts the same)
+  AutoCol *s_auto = nullptr;
+  AutoScratch scr{};
+  __shared__ uint32_t s_ared[AUTO ? kWarps : 1];
+  if constexpr (AUTO) {
+    uintptr_t q = (reinterpret_cast<uintptr_t>(s_lay + p.n_cols) + 15u) & ~(uintptr_t)15u;
+    s_auto = reinterpret_cast<AutoCol *>(q);
+    q = (q + (uintptr_t)p.n_cols * sizeof(AutoCol) + 15u) & ~(uintptr_t)15u;
+    const uint32_t P = p.sort_cap, R = (uint32_t)p.rows_per_block;
+    scr.sk = reinterpret_cast<unsigned long long *>(q);
+    scr.sr = reinterpret_cast<uint32_t *>(scr.sk + P);
+    scr.hs = scr.sr + P;
+    scr.a = scr.hs + P;
+    scr.b = scr.a + R;
+    scr.hp = scr.b + R;
+    scr.red = s_ared;
+  }
   __shared__ uint32_t s_red[kWarps];
   __shared__ int s_blk;
   __shared__ uint32_t s_size, s_original, s_ext_bit, s_host;
@@ -194,6 +622,15 @@ __global__ void __launch_bounds__(kThreads) obgpu_encode_blocks_kernel(const __g
   }
   __syncthreads();
 
+  if constexpr (AUTO) {   // ---- analysis of the AUTO columns, one after another, every thread --------------------------------
+    for (int c = 0; c < nc; ++c) {
+      if (!p.col[c].is_auto) continue;
+      uint32_t nn = 0;
+      for (int w = 0; w < kWarps; ++w) nn += s_wnull[w * nc + c];
+      analyze_column(p.col[c], row0, nrows, nn, p.sort_cap, scr, s_auto[c]);
+    }
+  }
+
   // ---- plan: warp 0, one lane per column (two rounds for more than 32 columns) -------------------------------------------
   if (warp == 0) {
     uint32_t at = kHeaderSize + 16u * (uint32_t)nc;
@@ -226,6 +663,9 @@ __global__ void __launch_bounds__(kThreads) obgpu_encode_blocks_kernel(const __g
         const unsigned long long bits = (nn ? (unsigned long long)ext_bit * nrows : 0ull) + (bp ? (unsigned long long)size * nrows : 0ull);
         l.bits_size = (uint32_t)((bits + 7ull) / 8ull);
         bytes = l.bits_size + (bp ? 0u : size * nrows);
+        if constexpr (AUTO) {
+          if (p.col[c].is_auto) bytes = plan_auto(p.col[c], s_auto[c], nrows, nn, mx, ext_bit, l, var, bytes);
+        }
       }
       uint32_t incl = bytes;   // column stores back to back: exclusive prefix over the columns
 #pragma unroll
@@ -242,6 +682,8 @@ __global__ void __launch_bounds__(kThreads) obgpu_encode_blocks_kernel(const __g
       const uint32_t cells = c < nc ? (nrows - nn) * p.col[c].datum_len : 0u;
       original += __reduce_add_sync(0xffffffffu, cells);
     }
+    // a layout above the shared-memory slot is left to the host writer, never written past the slot
+    if constexpr (AUTO) host = host || at > p.slot_cap;
     if (lane == 0) {
       s_size = host ? 0u : at;
       s_original = (uint32_t)min(original, 0x7fffffffull);
@@ -290,10 +732,25 @@ __global__ void __launch_bounds__(kThreads) obgpu_encode_blocks_kernel(const __g
       h[1] = 0u;
       h[2] = l.store_off - (kHeaderSize + 16u * (uint32_t)nc);
       h[3] = l.size;
+      if constexpr (AUTO) {
+        if (p.col[tid].is_auto && s_auto[tid].codec != 0) {   // type_ = the codec (COL_DICT 1 ... COL_INTEGER_BASE_DIFF 4)
+          h[0] |= (uint32_t)s_auto[tid].codec << 8;
+          h[3] = s_auto[tid].len;
+        }
+      }
     }
     for (int c = 0; c < nc; ++c) {
       const ColSpec &cs = p.col[c];
       const ColLayout l = s_lay[c];
+      if constexpr (AUTO) {
+        if (cs.is_auto && s_auto[c].codec != 0) {
+          uint32_t nn = 0;
+          for (int w = 0; w < kWarps; ++w) nn += s_wnull[w * nc + c];
+          pack_auto(cs, s_auto[c], l, row0, nrows, nn, ext_bit, p.sort_cap, scr, img32);
+          __syncthreads();
+          continue;
+        }
+      }
       const int64_t *v = cs.vals + row0;
       const uint8_t *nl = (cs.nulls && l.has_null) ? cs.nulls + row0 : nullptr;
       const uint32_t bit0 = l.store_off * 8u;                                    // block bit address of the bit area
@@ -476,6 +933,8 @@ static int enc_fill_cols(enc::Params &p, const obgpu_encode_col *cols, int32_t n
     s.obj_type = (uint8_t)cols[c].obj_type;
     s.byte_only = cols[c].byte_packing_only ? 1 : 0;
     s.datum_len = (uint8_t)obf::datum_len_of((uint8_t)cols[c].obj_type);
+    s.store_size = (uint8_t)obf::type_store_size((uint8_t)cols[c].obj_type);
+    s.is_signed = sc == 1 ? 1 : 0;
   }
   p.n_cols = n_cols;
   return OBGPU_SUCCESS;
@@ -483,21 +942,35 @@ static int enc_fill_cols(enc::Params &p, const obgpu_encode_col *cols, int32_t n
 
 extern "C" {
 
-int obgpu_encode_columns(obgpu_ctx *ctx, const obgpu_encode_col *cols, int32_t n_cols, int32_t rowkey_col_cnt, int64_t total_rows,
-                         int64_t rows_per_block, int32_t align, obgpu_encoded **out) {
+int obgpu_encode_columns_ex(obgpu_ctx *ctx, const obgpu_encode_col *cols, const int32_t *encodings, int32_t n_cols, int32_t rowkey_col_cnt,
+                            int64_t total_rows, int64_t rows_per_block, int32_t align, obgpu_encoded **out) {
   if (!ctx || !cols || !out || n_cols <= 0 || n_cols > enc::kMaxCols || rowkey_col_cnt < 0 || rowkey_col_cnt > n_cols || total_rows <= 0 ||
       rows_per_block <= 0 || rows_per_block > (1 << 22) || align < 16 || align > 4096 || (align & (align - 1)) != 0)
     return OBGPU_INVALID_ARGUMENT;
   const int64_t n_blocks64 = (total_rows + rows_per_block - 1) / rows_per_block;
   if (n_blocks64 > 0x7fffffff) return OBGPU_NOT_SUPPORTED;
+  int n_auto = 0;
+  for (int c = 0; encodings && c < n_cols; ++c) {
+    if (encodings[c] != OBGPU_ENC_RAW && encodings[c] != OBGPU_ENC_AUTO) return OBGPU_NOT_SUPPORTED;
+    n_auto += encodings[c] == OBGPU_ENC_AUTO;
+  }
   enc::Params p{};
   int rc = enc_fill_cols(p, cols, n_cols);
   if (rc != OBGPU_SUCCESS) return rc;
+  for (int c = 0; encodings && c < n_cols; ++c) p.col[c].is_auto = encodings[c] == OBGPU_ENC_AUTO ? 1 : 0;
   cudaSetDevice(ctx->device);
-  // the largest block: every column 8 bytes wide + one ext bit per cell
-  const int64_t bound = (int64_t)enc::kHeaderSize + 16 * n_cols + (int64_t)n_cols * (rows_per_block * 8 + (rows_per_block + 7) / 8 + 1);
+  // the largest block: every RAW column 8 bytes wide + one ext bit per cell; an AUTO column the largest store of any codec it
+  // can pick -- DICT / RLE at 12 bytes a row (8-byte values, 4-byte refs), BASE_DIFF at RAW's size + its 10-byte meta, CONST
+  // below 512 bytes (at most 32 exceptions)
+  const int64_t R = rows_per_block;
+  const int64_t bound = (int64_t)enc::kHeaderSize + 16 * n_cols + (int64_t)(n_cols - n_auto) * (R * 8 + (R + 7) / 8 + 1) +
+                        (int64_t)n_auto * (R * 12 + (R + 7) / 8 + 512);
   const int64_t slot_cap = (bound + align - 1) / align * align;
-  const size_t smem = (size_t)slot_cap + 4096 + (size_t)n_cols * (enc::kWarps * 12 + sizeof(enc::ColLayout)) + 16;
+  size_t smem = (size_t)slot_cap + 4096 + (size_t)n_cols * (enc::kWarps * 12 + sizeof(enc::ColLayout)) + 16;
+  uint32_t sort_cap = 1;
+  while ((int64_t)sort_cap < R) sort_cap <<= 1;
+  // AUTO: the AutoCol records and the sort scratch (keys, rows, scan: sort_cap each; refs, first occurrences: R each; R + 1 heads)
+  if (n_auto) smem += 32 + (size_t)n_cols * sizeof(enc::AutoCol) + (size_t)sort_cap * 16 + (size_t)R * 12 + 4;
   if ((int64_t)smem > (int64_t)ctx->max_smem_optin - 8192) return OBGPU_NOT_SUPPORTED;   // block image does not fit one CTA's shared memory
   const uint32_t lw_max = (uint32_t)(((slot_cap / 4 + enc::kThreads - 1) / enc::kThreads) | 1);
   const uint32_t *d_xpow = enc_xpow_table(ctx);
@@ -531,6 +1004,7 @@ int obgpu_encode_columns(obgpu_ctx *ctx, const obgpu_encode_col *cols, int32_t n
   p.align = (uint32_t)align;
   p.slot_cap = (uint32_t)slot_cap;
   p.lw_max = lw_max;
+  p.sort_cap = sort_cap;
   p.image = e->d_image;
   p.blk_off = e->d_off;
   p.blk_size = e->d_size;
@@ -539,9 +1013,11 @@ int obgpu_encode_columns(obgpu_ctx *ctx, const obgpu_encode_col *cols, int32_t n
   p.totals = e->d_totals;
   p.ticket = (int32_t *)(a + o_ctl + 128);
   p.xpow32 = d_xpow;
-  err = cudaFuncSetAttribute(enc::obgpu_encode_blocks_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+  // the AUTO instantiation only when some column asks for it: RAW-only calls keep the RAW kernel
+  auto kernel = n_auto ? enc::obgpu_encode_blocks_kernel<true, true> : enc::obgpu_encode_blocks_kernel<true, false>;
+  err = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   if (err != cudaSuccess) { ctx->err = cudaGetErrorString(err); obgpu_encoded_free(e); return OBGPU_ERR_SYS; }
-  enc::obgpu_encode_blocks_kernel<true><<<(unsigned)e->n_blocks, enc::kThreads, smem, ctx->stream>>>(p);
+  kernel<<<(unsigned)e->n_blocks, enc::kThreads, smem, ctx->stream>>>(p);
   ctx->launches++;
   err = cudaGetLastError();
   if (err != cudaSuccess) { ctx->err = cudaGetErrorString(err); obgpu_encoded_free(e); return OBGPU_ERR_SYS; }
@@ -634,9 +1110,16 @@ int obgpu_column_checksums(obgpu_ctx *ctx, const obgpu_encode_col *cols, int32_t
   return OBGPU_SUCCESS;
 }
 
-int obgpu_merge_result_encode(obgpu_merge_result *res, const int32_t *result_cols, const int32_t *obj_types, int32_t n_cols,
-                              int32_t rowkey_col_cnt, int64_t rows_per_block, int32_t align, obgpu_encoded **out) {
+int obgpu_encode_columns(obgpu_ctx *ctx, const obgpu_encode_col *cols, int32_t n_cols, int32_t rowkey_col_cnt, int64_t total_rows,
+                         int64_t rows_per_block, int32_t align, obgpu_encoded **out) {
+  return obgpu_encode_columns_ex(ctx, cols, nullptr, n_cols, rowkey_col_cnt, total_rows, rows_per_block, align, out);
+}
+
+int obgpu_merge_result_encode_ex(obgpu_merge_result *res, const int32_t *result_cols, const int32_t *obj_types, const int32_t *encodings,
+                                 int32_t n_cols, int32_t rowkey_col_cnt, int64_t rows_per_block, int32_t align, obgpu_encoded **out) {
   if (!res || !result_cols || !obj_types || n_cols <= 0 || n_cols > enc::kMaxCols || !out) return OBGPU_INVALID_ARGUMENT;
+  for (int c = 0; encodings && c < n_cols; ++c)
+    if (encodings[c] != OBGPU_ENC_RAW && encodings[c] != OBGPU_ENC_AUTO) return OBGPU_NOT_SUPPORTED;
   obgpu_merge_info info;
   int rc = obgpu_merge_result_info(res, &info);
   if (rc != OBGPU_SUCCESS) return rc;
@@ -660,7 +1143,12 @@ int obgpu_merge_result_encode(obgpu_merge_result *res, const int32_t *result_col
       c.dev_null = res->out_null[(size_t)k];
     }
   }
-  return obgpu_encode_columns(res->ctx, cols.data(), n_cols, rowkey_col_cnt, info.out_rows, rows_per_block, align, out);
+  return obgpu_encode_columns_ex(res->ctx, cols.data(), encodings, n_cols, rowkey_col_cnt, info.out_rows, rows_per_block, align, out);
+}
+
+int obgpu_merge_result_encode(obgpu_merge_result *res, const int32_t *result_cols, const int32_t *obj_types, int32_t n_cols,
+                              int32_t rowkey_col_cnt, int64_t rows_per_block, int32_t align, obgpu_encoded **out) {
+  return obgpu_merge_result_encode_ex(res, result_cols, obj_types, nullptr, n_cols, rowkey_col_cnt, rows_per_block, align, out);
 }
 
 }  // extern "C"

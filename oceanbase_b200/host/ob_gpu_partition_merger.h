@@ -56,6 +56,7 @@ struct ObGpuColumnGroup {
   std::vector<int32_t> cols_;
   std::vector<int32_t> obj_types_;   // OBGPU_OBJ_* of every column (integer classes)
   int32_t rowkey_col_cnt_ = 0;       // > 0 for the group that carries the rowkey (all-column / rowkey group)
+  std::vector<int32_t> encodings_;   // OBGPU_ENC_RAW / OBGPU_ENC_AUTO of every column; empty: every column RAW
 };
 
 // What the writer of one column group produced: the micro-blocks of its SSTable + the column checksums of its rows.
@@ -88,7 +89,8 @@ public:
   // ObWriteHelper::project / append, column_store/ob_column_oriented_merger.cpp:722-745, ob_co_merge_writer.cpp:67-117,345):
   // the merged stream -- produced once by merge_partition -- is replayed into the writer of every column group. Here a
   // writer is the device encoder (obgpu_merge_result_encode): the rows never leave the device as rows, each group comes back
-  // as reference-format micro-blocks (every column RAW) + its column checksums. rows_per_block cuts the blocks.
+  // as reference-format micro-blocks (each column RAW or AUTO, ObGpuColumnGroup::encodings_) + its column checksums.
+  // rows_per_block cuts the blocks.
   // compressor (ObCompressorType: OBGPU_COMPRESSOR_LZ4 / LZ4_1_9_1 / ZSTD_1_3_8): every group comes back in STORED form
   // (ObMicroBlockCompressor): the device's blocks compressed on the device (obgpu_compress_blocks) before the fetch, the
   // blocks left to the host writer compressed by obgpu_writer_compress_blocks; byte for byte obgpu_writer_compress_blocks
