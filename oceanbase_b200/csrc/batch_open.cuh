@@ -355,30 +355,37 @@ static int fill_batch(obgpu_ctx *ctx, obgpu_batch *b, const void *image, int64_t
   void *dp = nullptr;
   const size_t rows_bytes = ((size_t)n_blocks * 4 + 63) & ~(size_t)63;
   const size_t rec_bytes = (size_t)n_blocks * sizeof(BlockRec);
-  e = cudaMallocAsync(&dp, plan_bytes + rows_bytes + rec_bytes + (size_t)b->max_cols * 28 + 64, ctx->stream);
+  // stage records only where the small-block pipelined kernels can run
+  const bool pipe = pipe_wanted(b->max_rows);
+  const size_t stage_bytes = pipe ? (size_t)n_blocks * b->max_cols * sizeof(StageRec) : 0;
+  constexpr size_t kSpanRows = 8;
+  e = cudaMallocAsync(&dp, plan_bytes + stage_bytes + rows_bytes + rec_bytes + (size_t)b->max_cols * 4 * kSpanRows + 64, ctx->stream);
   if (e == cudaSuccess) {
     b->d_plans = (ColDesc *)dp;
-    b->d_rows = (uint32_t *)((uint8_t *)dp + plan_bytes);
-    b->d_recs = (BlockRec *)((uint8_t *)dp + plan_bytes + rows_bytes);
-    uint32_t *d_span = (uint32_t *)((uint8_t *)dp + plan_bytes + rows_bytes + rec_bytes);
+    b->d_stage = pipe ? (StageRec *)((uint8_t *)dp + plan_bytes) : nullptr;
+    b->d_rows = (uint32_t *)((uint8_t *)dp + plan_bytes + stage_bytes);
+    b->d_recs = (BlockRec *)((uint8_t *)dp + plan_bytes + stage_bytes + rows_bytes);
+    uint32_t *d_span = (uint32_t *)((uint8_t *)dp + plan_bytes + stage_bytes + rows_bytes + rec_bytes);
     // per-column reductions of the index kernel: [region span][dictionary size][type min][type max][RLE runs][projection span][materialised]
-    e = cudaMemsetAsync(d_span, 0, (size_t)b->max_cols * 28, ctx->stream);
+    // [stage record gaps: SR_NOT_FILTER | SR_NOT_FLAT]
+    e = cudaMemsetAsync(d_span, 0, (size_t)b->max_cols * 4 * kSpanRows, ctx->stream);
     if (e == cudaSuccess) e = cudaMemsetAsync(d_span + 2 * (size_t)b->max_cols, 0xff, (size_t)b->max_cols * 4, ctx->stream);
     const int64_t nthreads = (int64_t)n_blocks * b->max_cols;
     obgpu_index_kernel<<<(unsigned)((nthreads + 255) / 256), 256, 0, ctx->stream>>>(
         b->d_image, b->d_blk_off, b->d_blk_size, b->d_bm_word_off, n_blocks, (int)b->max_cols, b->d_plans,
-        b->d_rows, b->d_recs, d_span);
+        b->d_rows, b->d_recs, b->d_stage, d_span);
     if (e == cudaSuccess) e = cudaGetLastError();
     ctx->launches++;
-    b->col_span.assign((size_t)b->max_cols * 7, 0);
+    b->col_span.assign((size_t)b->max_cols * kSpanRows, 0);
     if (e == cudaSuccess)
-      e = cudaMemcpyAsync(b->col_span.data(), d_span, (size_t)b->max_cols * 28, cudaMemcpyDeviceToHost, ctx->stream);
+      e = cudaMemcpyAsync(b->col_span.data(), d_span, (size_t)b->max_cols * 4 * kSpanRows, cudaMemcpyDeviceToHost, ctx->stream);
   }
   // `stage` is pageable: the copy above is staged synchronously by the runtime before returning
   if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->stream);
   if (e != cudaSuccess) return cuda_failure(ctx, e);
   const size_t mc = b->max_cols;
   b->col_pspan.assign(b->col_span.begin() + 5 * mc, b->col_span.begin() + 6 * mc);
+  b->col_stage_gaps.assign(b->col_span.begin() + 7 * mc, b->col_span.begin() + 8 * mc);
   b->col_mat.assign(mc, 0);
   for (size_t c = 0; c < mc; ++c) b->col_mat[c] = b->col_span[6 * mc + c] ? 1 : 0;
   for (size_t c = 0; c < mc; ++c) {

@@ -148,6 +148,12 @@ struct ScanParams {
   uint32_t pp_meta, pp_region, pp_sel, pp_wscr, pp_bar, pp_bytes;    // project: per-warp layout
   uint32_t rle_slot_bytes;    // bytes per run-table slot: mask[words_cap] (u32) + pre[words_cap] (u16)
   uint32_t rows_cap, words_cap;
+  // stage records instead of plans in the meta slots (pc_rec: count, pp_rec: project), and what they need from the column type
+  // (about 256 bytes at the end of the block; every kernel taking ScanParams carries them, well inside the parameter space)
+  const StageRec *stage;      // [n_blocks][max_cols]
+  int32_t pc_rec, pp_rec;
+  uint8_t used_sc[kMaxUsedCols], used_elem_len[kMaxUsedCols];
+  uint64_t used_int_mask[kMaxUsedCols];
 };
 
 // =================================================================================================
@@ -1101,10 +1107,41 @@ __device__ __forceinline__ void project_column_global(const ScanParams &p, const
 // same kind of cached decoder state beside a block in its block cache (ObBlockCachedDecoderHeader,
 // blocksstable/ob_micro_block_cache.cpp:1345-1363).
 // =================================================================================================
+// Stage record of plan d (scan_device.cuh) and what it cannot stand in for: SR_NOT_FILTER unless the lean filter leaves of
+// obgpu_count_pipe_kernel can run on it (a K_DICT column whose filter region is the hull of its projection ranges), SR_NOT_FLAT
+// unless it is a flat projected column (flat_kind). A field that does not fit the record clears both.
+__device__ __forceinline__ uint32_t stage_rec_of(const ColDesc &d, const BlockView &b, StageRec &r) {
+  r = StageRec{};
+  uint32_t pr[4] = {0, 0, 0, 0}, flo = 0, fhi = 0;
+  const int nr = d.ok ? proj_ranges(d, b, pr) : 0;
+  const bool fr = d.ok && col_region(d, b, flo, fhi);
+  const bool str = d.kind == K_DICT && d.sc == 5;
+  const uint32_t last_end = d.dict_end - d.dict_var;
+  if (nr == 0 || !(d.kind == K_BITS || d.kind == K_DICT) || (str && d.dict_fixed) || pr[1] > 0xffff0u || pr[3] > 0xffff0u ||
+      d.dict_count > 0xffffu || d.stride > 0xffu || (str && last_end > 0xffffu))
+    return SR_NOT_FILTER | SR_NOT_FLAT;
+  r.add = str ? d.dict_var : d.base;
+  r.val_bit = d.val_bit;
+  r.dict_payload = d.dict_payload;
+  r.lo[0] = (uint16_t)(pr[0] >> 4);
+  r.hi[0] = (uint16_t)(pr[1] >> 4);
+  r.lo[1] = (uint16_t)(pr[2] >> 4);
+  r.hi[1] = (uint16_t)(pr[3] >> 4);
+  r.dict_count = (uint16_t)d.dict_count;
+  r.last_end = str ? (uint16_t)last_end : 0;
+  r.width = d.width;
+  r.stride = (uint8_t)d.stride;
+  r.dict_data_size = (uint8_t)d.dict_data_size;
+  r.flags = (d.kind == K_DICT ? SR_DICT : 0) | (d.dict_sorted ? SR_SORTED : 0) | (d.sign_fix ? SR_SIGN_FIX : 0);
+  uint32_t no = flat_kind(d) ? 0u : SR_NOT_FLAT;
+  if (!(d.kind == K_DICT && d.width <= 32u && fr && flo == pr[0] && fhi == max(pr[1], pr[3]))) no |= SR_NOT_FILTER;
+  return no;
+}
+
 __global__ void __launch_bounds__(256) obgpu_index_kernel(const uint8_t *image, const uint64_t *blk_off,
                                                           const uint32_t *blk_size, const int64_t *bm_word_off,
                                                           int n_blocks, int max_cols, ColDesc *plans, uint32_t *rows,
-                                                          BlockRec *recs, uint32_t *col_span) {
+                                                          BlockRec *recs, StageRec *stage, uint32_t *col_span) {
   const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= (int64_t)n_blocks * max_cols) return;
   const int block = (int)(i / max_cols), col = (int)(i % max_cols);
@@ -1114,6 +1151,15 @@ __global__ void __launch_bounds__(256) obgpu_index_kernel(const uint8_t *image, 
   d.rle_slot = -1;
   if (b.ok) build_col_desc(b, col, d);
   plans[i] = d;
+  if (stage != nullptr) {
+    // corrupt blocks are settled before the scan kernels read a record: they do not decide the column's path
+    StageRec sr;
+    const uint32_t no = stage_rec_of(d, b, sr);
+    stage[i] = sr;
+    // the bits are set by the first blocks that lack them: later blocks read them instead of queueing on one address
+    uint32_t *gaps = &col_span[7 * max_cols + col];
+    if (b.ok && (*(volatile uint32_t *)gaps & no) != no) atomicOr(gaps, no);
+  }
   if (col == 0) {
     rows[block] = b.ok ? b.row_count : 0u;
     BlockRec r{};
@@ -1771,8 +1817,10 @@ struct obgpu_batch {
   ColDesc *d_plans = nullptr;
   uint32_t *d_rows = nullptr;
   BlockRec *d_recs = nullptr;
+  StageRec *d_stage = nullptr;         // [n_blocks][max_cols] stage records (scan_small.cuh), in the plans' allocation; nullptr: none
   std::vector<uint32_t> col_span;      // per store index: max staged bytes of the value / ref array
   std::vector<uint32_t> col_pspan;     // per store index: max bytes a projection stages (proj_ranges)
+  std::vector<uint32_t> col_stage_gaps;  // per store index: SR_NOT_FILTER / SR_NOT_FLAT if some block's record cannot serve that path
   // skip index: serialized aggregate rows of the blocks (obgpu_batch_set_agg_rows), [d_agg_off[b], d_agg_off[b + 1])
   uint8_t *d_agg = nullptr;
   int64_t *d_agg_off = nullptr;
@@ -1780,6 +1828,14 @@ struct obgpu_batch {
   obcs::XformRec *d_xf = nullptr;
   std::vector<uint8_t> col_mat;        // per store index: 1 when some block rebuilt the column's strings at open (mat_codecs.cuh)
 };
+
+// Whether a scan of the batch may take the small-block pipelined kernels (scan_small.cuh): fill_batch builds stage records
+// for such batches, layout_pipe chooses the kernels
+static bool pipe_wanted(uint32_t max_rows) {
+  bool want = max_rows <= 512;
+  if (const char *e = getenv("OBGPU_PIPE")) want = atoi(e) != 0;   // testing knob: force the path on / off
+  return want;
+}
 
 struct ResultCol {
   void *data = nullptr;
@@ -1862,7 +1918,8 @@ int obgpu_ctx_create(int device, obgpu_ctx **out) {
   };
   const bool ok = opt_in((const void *)obgpu_count_kernel) && opt_in((const void *)obgpu_project_kernel<false>) && opt_in((const void *)obgpu_project_kernel<true>) &&
                   opt_in((const void *)obgpu_filter_block_kernel) && opt_in((const void *)obgpu_project_block_kernel) &&
-                  opt_in((const void *)obgpu_count_pipe_kernel) && opt_in((const void *)obgpu_project_pipe_kernel);
+                  opt_in((const void *)obgpu_count_pipe_kernel<false>) && opt_in((const void *)obgpu_count_pipe_kernel<true>) &&
+                  opt_in((const void *)obgpu_project_pipe_kernel<false>) && opt_in((const void *)obgpu_project_pipe_kernel<true>);
   cudaGetLastError();  // do not leave a stale (non-sticky) error for later launch checks
   if (!ok) {
     g_last_global_err = "cudaFuncSetAttribute(MaxDynamicSharedMemorySize) failed: not an sm_90a device?";
@@ -2233,10 +2290,20 @@ static void layout_smem_scan(const obgpu_batch *b, ScanParams &p, int max_smem) 
 // Small-block pipelined kernels (scan_small.cuh): which of them this scan can use, and their per-warp layouts.
 static void layout_pipe(const obgpu_batch *b, ScanParams &p, int max_smem) {
   p.pipe_count = p.pipe_project = 0;
-  bool want = b->max_rows <= 512;
-  if (const char *e = getenv("OBGPU_PIPE")) want = atoi(e) != 0;   // testing knob: force the path on / off
-  if (!want) return;
+  p.pc_rec = p.pp_rec = 0;
+  if (!pipe_wanted(b->max_rows)) return;
   auto r16 = [](uint32_t v) { return (v + 15u) & ~15u; };
+  // stage records serve used column i when every block's record can stand in for its plan on that path, and the blocks agree on
+  // the column's type (the record leaves the type facts to the scan)
+  auto rec_ok = [&](int i, uint32_t gap) {
+    const size_t col = (size_t)p.used_col[i];
+    if (b->d_stage == nullptr || col >= b->col_stage_gaps.size() || (b->col_stage_gaps[col] & gap) || b->col_types[col] == 0xff) return false;
+    const uint8_t t = b->col_types[col];
+    p.used_sc[i] = (uint8_t)obf::store_class_of(t);
+    p.used_elem_len[i] = (uint8_t)obf::datum_len_of(t);
+    p.used_int_mask[i] = obf::integer_mask_of(t);
+    return true;
+  };
   // ---- count: every filter column (= the first pf_n used columns) has a bounded region ----------------------
   if (p.n_nodes > 0 && p.simple_shape != 0) {
     int nf = 0;
@@ -2255,7 +2322,17 @@ static void layout_pipe(const obgpu_batch *b, ScanParams &p, int max_smem) {
     }
     if (ok) {
       p.pf_n = nf;
-      p.pc_meta_bytes = kMetaPlans + (uint32_t)nf * (uint32_t)sizeof(ColDesc);
+      // records: every block has at most 1024 rows (bitmap in registers) and every leaf takes a lean path (lean_leaf) on
+      // a column whose records all serve the filter
+      bool rec = b->max_rows <= 1024u;
+      const int n_leaves = p.n_nodes == 1 ? 1 : p.n_nodes - 1;
+      for (int i = 0; i < n_leaves && rec; ++i) {
+        const FilterNodeDev &nd = p.nodes[i];
+        rec = nd.op != OP_FALSE && nd.op != OP_TRUE && nd.slot >= 0 && nd.used_idx < nf && rec_ok(nd.used_idx, SR_NOT_FILTER);
+        if (rec) rec = p.used_sc[nd.used_idx] == 5 ? (nd.op == OP_EQ || nd.op == OP_NE || nd.op == OP_IN) : nd.range_ok != 0;
+      }
+      p.pc_rec = rec ? 1 : 0;
+      p.pc_meta_bytes = kMetaPlans + (uint32_t)nf * (rec ? kCountEnt<true> : kCountEnt<false>);
       p.pc_region_bytes = kCountHdrBytes + off;
       uint32_t w = 0;
       p.pc_meta = w;   w += 3u * p.pc_meta_bytes;
@@ -2280,7 +2357,10 @@ static void layout_pipe(const obgpu_batch *b, ScanParams &p, int max_smem) {
       off += r16(sp);
     }
     if (ok) {
-      p.pp_meta_bytes = kMetaPlans + (uint32_t)std::max(p.n_proj, 1) * (uint32_t)sizeof(ColDesc);
+      bool rec = true;
+      for (int i = 0; i < p.n_proj && rec; ++i) rec = rec_ok(p.proj_used[i], SR_NOT_FLAT);
+      p.pp_rec = rec ? 1 : 0;
+      p.pp_meta_bytes = kMetaPlans + (uint32_t)std::max(p.n_proj, 1) * (rec ? kProjEnt<true> : kProjEnt<false>);
       p.pp_hdr_bytes = r16((2u * (uint32_t)kMaxProj + 1u) * 4u);   // deltas + flags
       p.pp_bm_bytes = r16(p.words_cap * 4u);
       p.pp_region_bytes = p.pp_hdr_bytes + p.pp_bm_bytes + off;
@@ -2573,6 +2653,7 @@ static int scan_common(obgpu_batch *b, const obgpu_scan_spec *spec, const obgpu_
   p.plans = b->d_plans;
   p.rows = b->d_rows;
   p.recs = b->d_recs;
+  p.stage = b->d_stage;
   p.xf = reinterpret_cast<const XformRecFwd *>(b->d_xf);
   p.max_cols = (int32_t)b->max_cols;
   p.counts = (uint32_t *)(a + o_counts);
@@ -2621,9 +2702,10 @@ static int scan_common(obgpu_batch *b, const obgpu_scan_spec *spec, const obgpu_
     if (p.pipe_count) {
       const int smem = (int)(p.pc_bytes * (uint32_t)kWarps);
       int occ = 1;
-      cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, obgpu_count_pipe_kernel, kThreads, smem);
+      const auto kern = p.pc_rec ? obgpu_count_pipe_kernel<true> : obgpu_count_pipe_kernel<false>;
+      cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, kThreads, smem);
       const int grid = std::min((n + kWarps - 1) / kWarps, std::max(1, occ) * ctx->sm_count);
-      obgpu_count_pipe_kernel<<<grid, kThreads, smem, ctx->stream>>>(p);
+      kern<<<grid, kThreads, smem, ctx->stream>>>(p);
     } else {
       obgpu_count_kernel<<<(n + kWarps - 1) / kWarps, kThreads, cw_total, ctx->stream>>>(p);
     }
@@ -2641,9 +2723,10 @@ static int scan_common(obgpu_batch *b, const obgpu_scan_spec *spec, const obgpu_
     if (p.pipe_project) {
       const int smem = (int)(p.pp_bytes * (uint32_t)kWarps);
       int occ = 1;
-      cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, obgpu_project_pipe_kernel, kThreads, smem);
+      const auto kern = p.pp_rec ? obgpu_project_pipe_kernel<true> : obgpu_project_pipe_kernel<false>;
+      cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, kThreads, smem);
       const int grid = std::min((n + kWarps - 1) / kWarps, std::max(1, occ) * ctx->sm_count);
-      obgpu_project_pipe_kernel<<<grid, kThreads, smem, ctx->stream>>>(p);
+      kern<<<grid, kThreads, smem, ctx->stream>>>(p);
     } else if (p.sparse_split) obgpu_project_kernel<true><<<(n + p.proj_tiles - 1) / p.proj_tiles, kThreads, p.smem_total, ctx->stream>>>(p);
     else obgpu_project_kernel<false><<<n, kThreads, p.smem_total, ctx->stream>>>(p);
     ctx->launches++;

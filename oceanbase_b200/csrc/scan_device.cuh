@@ -199,6 +199,23 @@ struct alignas(16) BlockRec {
 };
 static_assert(sizeof(BlockRec) == 48, "BlockRec is loaded as three 16-byte pieces");
 
+// Per (block, column) stage record, written at batch open next to the plan by the index kernel for batches that can take
+// the small-block pipelined kernels (scan_small.cuh): the byte ranges a projection stages (proj_ranges) and the fields the
+// lean filter leaves and the flat projection read, so those kernels copy 32 bytes per column and block instead of the
+// 96-byte plan and never run col_region / proj_ranges. Offsets are block relative, as in the plan.
+enum : uint8_t { SR_DICT = 1, SR_SORTED = 2, SR_SIGN_FIX = 4 };
+enum : uint32_t { SR_NOT_FILTER = 1, SR_NOT_FLAT = 2 };   // per-column reduction over the blocks (index kernel)
+struct alignas(16) StageRec {
+  uint64_t add;           // K_BITS / integer dictionary: the plan's base; string dictionary: dict_var
+  uint32_t val_bit;       // bit offset of value / ref 0
+  uint32_t dict_payload;  // byte offset of dictionary entry 0 (string dictionary: END offset 0)
+  uint16_t lo[2], hi[2];  // projection ranges [16 lo, 16 hi); lo[1] == hi[1]: one range. A filter stages [16 lo[0], 16 max(hi))
+  uint16_t dict_count;
+  uint16_t last_end;      // string dictionary: dict_end - dict_var
+  uint8_t width, stride, dict_data_size, flags;   // flags: SR_DICT (else K_BITS), SR_SORTED, SR_SIGN_FIX
+};
+static_assert(sizeof(StageRec) == 32, "StageRec is loaded as two 16-byte pieces");
+
 __device__ __forceinline__ void view_from_rec(const BlockRec &r, const uint8_t *s, BlockView &b) {
   b.s = s;
   b.size = r.size;
@@ -931,6 +948,12 @@ __device__ __forceinline__ int proj_ranges(const ColDesc &d, const BlockView &bv
   r[1] = hi;
   return 1;
 }
+// "Flat" projected column (scan_small.cuh, project_flat): a row's output is one ref / value load plus at most two dictionary loads
+__device__ __forceinline__ bool flat_kind(const ColDesc &d) {
+  if (d.kind == K_BITS) return d.sc != 5 && d.ext_bit == 0 && !d.sign_fix && !d.var_is_last;
+  if (d.kind == K_DICT) return d.sc == 5 ? !d.dict_fixed : d.dict_data_size <= 8u;
+  return false;
+}
 __device__ __forceinline__ uint32_t proj_ranges_bytes(const ColDesc &d, const BlockView &bv) {
   uint32_t r[4];
   const int n = proj_ranges(d, bv, r);
@@ -1012,13 +1035,15 @@ __device__ __forceinline__ void dict_str(const uint8_t *s, const ColDesc &d, uin
 }
 
 // Shared-window twins of dict_int / dict_str: `sbit` is 8 * the shared-window address of the staged block (or of the
-// staged column region, shifted so block offsets resolve into it).
-__device__ __forceinline__ uint64_t dict_int_s(uint32_t sbit, const ColDesc &d, uint32_t ref) {
+// staged column region, shifted so block offsets resolve into it). D is a ColDesc or a descriptor with the same field names.
+template <class D>
+__device__ __forceinline__ uint64_t dict_int_s(uint32_t sbit, const D &d, uint32_t ref) {
   const uint32_t dbits = d.dict_data_size * 8u, at = sbit + d.dict_payload * 8u + ref * dbits;
   const uint64_t v = (dbits <= 32u ? (uint64_t)sbits32(at, dbits) : sbits(at, dbits)) + d.base;
   return d.sign_fix ? sign_fix(d.int_mask, v) : v;
 }
-__device__ __forceinline__ void dict_str_s(uint32_t sbit, const ColDesc &d, uint32_t ref, uint32_t &cell, uint32_t &len) {
+template <class D>
+__device__ __forceinline__ void dict_str_s(uint32_t sbit, const D &d, uint32_t ref, uint32_t &cell, uint32_t &len) {
   if (d.dict_fixed) {
     len = d.dict_data_size;
     cell = d.dict_payload + ref * len;
@@ -1067,7 +1092,8 @@ __device__ __forceinline__ uint64_t int_cell(const BlockView &b, const ColDesc &
 }
 
 // value used for comparisons: sign-extended from the datum length for signed classes
-__device__ __forceinline__ int64_t cmp_image(const ColDesc &d, uint64_t v) {
+template <class D>
+__device__ __forceinline__ int64_t cmp_image(const D &d, uint64_t v) {
   if (d.elem_len == 4) return d.sc == 1 ? (int64_t)(int32_t)(uint32_t)v : (int64_t)(uint32_t)v;
   if (d.elem_len == 1) return (int64_t)(uint8_t)v;
   return (int64_t)v;

@@ -62,7 +62,8 @@ static_assert(kMetaPlans % 16u == 0u, "decode plans are copied in 16-byte pieces
 
 // ---- lean leaf pieces for blocks of at most 1024 rows (bitmap in registers, lane g owns word g) ----------------------
 // Range leaf over the fixed-width integer dictionary of a K_DICT column -> predicate bitset (bit count = NULL: never set).
-__device__ __forceinline__ void lean_bitset_int_range(const ColDesc &d, const FilterNodeDev &nd, uint32_t sbit, uint32_t *bits, int lane) {
+template <class D>
+__device__ __forceinline__ void lean_bitset_int_range(const D &d, const FilterNodeDev &nd, uint32_t sbit, uint32_t *bits, int lane) {
   const uint32_t n = d.dict_count;
   const uint64_t lo = nd.lo, span = nd.span;
   const bool neg = nd.negate != 0;
@@ -78,8 +79,8 @@ __device__ __forceinline__ void lean_bitset_int_range(const ColDesc &d, const Fi
 // Rows of a K_DICT column against a predicate over refs -- a bitset in shared memory (BITSET) or a ref interval
 // [a, e), complemented inside [0, count) when neg (sorted dictionary). Lane g collects word g; returns the lane's
 // updated bitmap word.
-template <bool BITSET>
-__device__ __forceinline__ uint32_t lean_rows(const ColDesc &d, uint32_t sbit, const uint32_t *bits, uint32_t a, uint32_t e, bool neg,
+template <bool BITSET, class D>
+__device__ __forceinline__ uint32_t lean_rows(const D &d, uint32_t sbit, const uint32_t *bits, uint32_t a, uint32_t e, bool neg,
                                               uint32_t mybm, uint32_t myvalid, uint32_t nwords, bool and_mode, int lane) {
   const uint32_t step = 32u * d.stride, width = d.width, dcount = d.dict_count, cntp1 = dcount + 1u, span = e - a;
   uint32_t bit = sbit + d.val_bit + (uint32_t)lane * d.stride, acc = 0;
@@ -102,7 +103,8 @@ __device__ __forceinline__ uint32_t lean_rows(const ColDesc &d, uint32_t sbit, c
 
 // Sorted fixed-width integer dictionary and a range leaf: the matching refs are [a, e) = [#entries below the range,
 // #entries not above it) (the reference binary-searches the bounds, ob_dict_decoder.cpp:967-988,1085-1176).
-__device__ __forceinline__ void lean_interval_sorted_int(const ColDesc &d, const FilterNodeDev &nd, uint32_t sbit, int lane,
+template <class D>
+__device__ __forceinline__ void lean_interval_sorted_int(const D &d, const FilterNodeDev &nd, uint32_t sbit, int lane,
                                                          uint32_t &a, uint32_t &e) {
   const uint32_t n = d.dict_count;
   const uint64_t lo = nd.lo, hi = nd.lo + nd.span;
@@ -145,7 +147,8 @@ __device__ __forceinline__ uint64_t str_eq_screen(const FilterNodeDev &nd, uint3
 // EQ / NE / IN leaf over the string dictionary of a K_DICT column -> predicate bitset. Every entry is screened by
 // (length, first 8 bytes) against the constants; only the (few) entries that pass compare their tails, 8 bytes at a
 // time, out of shared memory.
-__device__ __forceinline__ void lean_bitset_str_eq(const ScanParams &p, const FilterNodeDev &nd, const ColDesc &d, uint32_t sbit,
+template <class D>
+__device__ __forceinline__ void lean_bitset_str_eq(const ScanParams &p, const FilterNodeDev &nd, const D &d, uint32_t sbit,
                                                    uint32_t *bits, int lane) {
   const uint32_t n = d.dict_count;
   const bool ne = nd.op == OP_NE;
@@ -178,7 +181,8 @@ __device__ __forceinline__ void lean_bitset_str_eq(const ScanParams &p, const Fi
 
 // AND leaf on a string K_DICT column when few rows are still alive: evaluate the leaf on the survivors' own
 // dictionary entries (one pass over <= alive rows) instead of on every dictionary entry.
-__device__ __forceinline__ uint32_t lean_survivor_str(const ScanParams &p, const FilterNodeDev &nd, const ColDesc &d, uint32_t sbit,
+template <class D>
+__device__ __forceinline__ uint32_t lean_survivor_str(const ScanParams &p, const FilterNodeDev &nd, const D &d, uint32_t sbit,
                                                       const uint8_t *rs_generic, uint32_t mybm, uint32_t nwords, uint32_t alive,
                                                       uint32_t *bm, int lane) {
   // survivor list (ascending rows) in the spilled-bitmap scratch: uint16 rows after the 32 bitmap words
@@ -218,11 +222,71 @@ __device__ __forceinline__ uint32_t lean_survivor_str(const ScanParams &p, const
   return (uint32_t)lane < nwords ? bm[lane] : 0u;
 }
 
+// A stage record (scan_device.cuh) in a meta slot read under the plan's field names, with the column's type facts of the
+// scan (store class, datum length, sign-fix mask: the same for every block of a column whose blocks agree on its type): the
+// lean leaves and flat_fill take either a plan or this.
+struct RecDesc {
+  uint64_t base, int_mask;
+  uint32_t val_bit, stride, width, dict_count, dict_payload, dict_data_size, dict_var, dict_end;
+  uint8_t kind, sc, elem_len, sign_fix, dict_sorted, dict_fixed;
+};
+__device__ __forceinline__ RecDesc rec_desc(const ScanParams &p, const StageRec &r, int used) {
+  RecDesc d;
+  d.sc = p.used_sc[used];
+  d.elem_len = p.used_elem_len[used];
+  d.kind = (r.flags & SR_DICT) ? K_DICT : K_BITS;
+  d.sign_fix = (r.flags & SR_SIGN_FIX) != 0;
+  d.int_mask = d.sign_fix ? p.used_int_mask[used] : 0ull;
+  const bool str = d.kind == K_DICT && d.sc == 5;
+  d.base = str ? 0ull : r.add;
+  d.dict_var = str ? (uint32_t)r.add : 0u;
+  d.dict_end = d.dict_var + r.last_end;
+  d.val_bit = r.val_bit;
+  d.stride = r.stride;
+  d.width = r.width;
+  d.dict_count = r.dict_count;
+  d.dict_payload = r.dict_payload;
+  d.dict_data_size = r.dict_data_size;
+  d.dict_sorted = (r.flags & SR_SORTED) != 0;
+  d.dict_fixed = 0;   // string dictionaries with records have variable-length entries (stage_rec_of)
+  return d;
+}
+// Meta-slot entry of a column: its plan, or its stage record (count) / its stage record with room for the FlatCol entry
+// flat_fill writes over it (projection).
+template <bool REC> constexpr uint32_t kCountEnt = REC ? (uint32_t)sizeof(StageRec) : (uint32_t)sizeof(ColDesc);
+template <bool REC> constexpr uint32_t kProjEnt = REC ? 64u : (uint32_t)sizeof(ColDesc);
+
+// One lean leaf on the K_DICT column of stage record d (width <= 32) staged at sbit (generic address rs_col): returns the lane's
+// bitmap word. The plan path of obgpu_count_pipe_kernel writes the same steps out with a fall-back to the generic dictionary
+// bitset (build_dict_bitset); layout_pipe gives a scan records only when no leaf needs that fall-back.
+__device__ __forceinline__ uint32_t lean_leaf(const ScanParams &p, const FilterNodeDev &nd, const RecDesc &d, uint32_t sbit, const uint8_t *rs_col,
+                                              uint32_t *bits, uint32_t *bm, uint32_t mybm, uint32_t myvalid, uint32_t nwords,
+                                              bool and_mode, int lane) {
+  const bool is_str = d.sc == 5;
+  if (is_str && and_mode) {
+    // few surviving rows and a larger dictionary: test the survivors' own entries instead of every entry
+    const uint32_t alive = warp_sum_u32(__popc(mybm));
+    if (alive * 4u <= d.dict_count) return lean_survivor_str(p, nd, d, sbit, rs_col, mybm, nwords, alive, bm, lane);
+  }
+  if (!is_str && nd.range_ok && d.dict_sorted) {
+    uint32_t a, e;
+    lean_interval_sorted_int(d, nd, sbit, lane, a, e);
+    return lean_rows<false>(d, sbit, nullptr, a, e, nd.negate != 0, mybm, myvalid, nwords, and_mode, lane);
+  }
+  if (!is_str && nd.range_ok) lean_bitset_int_range(d, nd, sbit, bits, lane);
+  else lean_bitset_str_eq(p, nd, d, sbit, bits, lane);
+  __syncwarp();
+  return lean_rows<true>(d, sbit, bits, 0u, 0u, false, mybm, myvalid, nwords, and_mode, lane);
+}
+
 // =================================================================================================
-// Count, pipelined. Per warp: meta ring (3 slots: block record + the filter columns' plans), region ring (2 slots:
-// header with the per-column deltas + the filter columns' regions), bitmap words, predicate bitsets.
+// Count, pipelined. Per warp: meta ring (3 slots: block record + the filter columns' plans, or their stage records when
+// REC), region ring (2 slots: header with the per-column deltas + the filter columns' regions), bitmap words, predicate bitsets.
 // =================================================================================================
+template <bool REC>
 __global__ void __launch_bounds__(kThreads) obgpu_count_pipe_kernel(const __grid_constant__ ScanParams p) {
+  constexpr uint32_t kEnt = kCountEnt<REC>;
+  constexpr int kEntPieces = (int)(kEnt / 16u);
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const int nwarps_total = (int)gridDim.x * kWarps;
   int blk = (int)blockIdx.x * kWarps + warp;
@@ -245,13 +309,13 @@ __global__ void __launch_bounds__(kThreads) obgpu_count_pipe_kernel(const __grid
     if (b >= p.n_blocks) return;
     const uint32_t sa = smem_u32(meta0 + (uint32_t)slot * p.pc_meta_bytes);
     const uint8_t *rec = reinterpret_cast<const uint8_t *>(p.recs + b);
-    const uint8_t *plans = reinterpret_cast<const uint8_t *>(p.plans + (int64_t)b * p.max_cols);
-    for (int q = lane; q < kRecPieces + nf * kPlanPieces; q += 32) {
+    const uint8_t *ents = REC ? reinterpret_cast<const uint8_t *>(p.stage + (int64_t)b * p.max_cols)
+                              : reinterpret_cast<const uint8_t *>(p.plans + (int64_t)b * p.max_cols);
+    for (int q = lane; q < kRecPieces + nf * kEntPieces; q += 32) {
       if (q < kRecPieces) cp_async16(sa + (uint32_t)q * 16u, rec + q * 16);
       else {
-        const int i = (q - kRecPieces) / kPlanPieces, piece = (q - kRecPieces) % kPlanPieces;
-        cp_async16(sa + kMetaPlans + (uint32_t)i * (uint32_t)sizeof(ColDesc) + (uint32_t)piece * 16u,
-                   plans + (size_t)p.used_col[i] * sizeof(ColDesc) + piece * 16);
+        const int i = (q - kRecPieces) / kEntPieces, piece = (q - kRecPieces) % kEntPieces;
+        cp_async16(sa + kMetaPlans + (uint32_t)i * kEnt + (uint32_t)piece * 16u, ents + (size_t)p.used_col[i] * kEnt + piece * 16);
       }
     }
   };
@@ -266,10 +330,17 @@ __global__ void __launch_bounds__(kThreads) obgpu_count_pipe_kernel(const __grid
     uint32_t lo = 0, hi = 0;
     bool bad = false;
     if (lane < nf && rec.rows != 0 && verdict == 0) {
-      BlockView bv;
-      view_from_rec(rec, nullptr, bv);
-      const ColDesc &d = descs[lane];
-      if (!d.ok || !col_region(d, bv, lo, hi) || hi - lo > p.pf_span[lane] || hi > ((rec.size + 15u) & ~15u) + 32u) { bad = true; lo = hi = 0; }
+      if constexpr (REC) {
+        const StageRec &r = reinterpret_cast<const StageRec *>(m + kMetaPlans)[lane];
+        lo = (uint32_t)r.lo[0] * 16u;
+        hi = (uint32_t)max(r.hi[0], r.hi[1]) * 16u;
+        if (hi - lo > p.pf_span[lane] || hi > ((rec.size + 15u) & ~15u) + 32u) { bad = true; lo = hi = 0; }
+      } else {
+        BlockView bv;
+        view_from_rec(rec, nullptr, bv);
+        const ColDesc &d = descs[lane];
+        if (!d.ok || !col_region(d, bv, lo, hi) || hi - lo > p.pf_span[lane] || hi > ((rec.size + 15u) & ~15u) + 32u) { bad = true; lo = hi = 0; }
+      }
       hdr[lane] = (int32_t)(kCountHdrBytes + p.pf_off[lane]) - (int32_t)lo;
     }
     const uint32_t badmask = __ballot_sync(0xffffffffu, bad);
@@ -318,7 +389,6 @@ __global__ void __launch_bounds__(kThreads) obgpu_count_pipe_kernel(const __grid
     const uint8_t *m = meta0 + (uint32_t)ms * p.pc_meta_bytes;
     uint8_t *rs = reg0 + (uint32_t)rsl * p.pc_region_bytes;
     const BlockRec rec = *reinterpret_cast<const BlockRec *>(m);
-    const ColDesc *descs = reinterpret_cast<const ColDesc *>(m + kMetaPlans);
     const int32_t *hdr = reinterpret_cast<const int32_t *>(rs);
     const uint32_t rows = rec.rows;
     uint32_t *gbm = p.bitmap_words + rec.bm_word_off;
@@ -330,113 +400,132 @@ __global__ void __launch_bounds__(kThreads) obgpu_count_pipe_kernel(const __grid
       __syncwarp();
       continue;
     }
-    BlockCtx c;
-    view_from_rec(rec, nullptr, c.b);
-    c.descs = descs;
-    c.bitsets = bitsets;
-    c.rle_base = nullptr;
-    c.rle_slot_bytes = c.rle_starts_bytes = 0;
-    const bool and_mode = p.simple_shape == 1;
-    const int n_leaves = p.n_nodes == 1 ? 1 : p.n_nodes - 1;
-    // every filter column is staged: block-relative offsets of a leaf's column resolve into its region
-    auto staged_at = [&](const FilterNodeDev &nd, const ColDesc &, BlockCtx &cs) {
-      if (nd.op != OP_FALSE && nd.op != OP_TRUE) {
-        cs.b.s = rs + hdr[nd.used_idx];
-        cs.sbit = (smem_u32(rs) + (uint32_t)hdr[nd.used_idx]) * 8u;
-      }
-      return true;
-    };
     uint32_t cnt = 0;
-    if (nwords <= 32u) {
-      // ---- lean path: the block's bitmap lives in registers (lane g owns word g); dictionary-coded leaves run
-      // through explicit shared-memory loads, everything else through the generic leaf code on a spilled bitmap
+    if constexpr (REC) {
+      // stage records: every block has at most 1024 rows (bitmap in registers) and every leaf is lean (layout_pipe)
+      const bool and_mode = p.simple_shape == 1;
+      const int n_leaves = p.n_nodes == 1 ? 1 : p.n_nodes - 1;
       const uint32_t myvalid = (uint32_t)lane < nwords ? valid_mask_of(rows, (uint32_t)lane) : 0u;
       uint32_t mybm = and_mode ? myvalid : 0u;
       for (int i = 0; i < n_leaves; ++i) {
         const FilterNodeDev &nd = p.nodes[i];
         if (p.leaf_const != nullptr && p.leaf_const[(int64_t)blk * p.n_nodes + i] != 0) continue;
-        const ColDesc &d = descs[nd.used_idx];
-        const uint32_t sbit = (smem_u32(rs) + (uint32_t)hdr[nd.used_idx]) * 8u;
-        if (d.kind == K_DICT && nd.slot >= 0 && nd.op != OP_FALSE && nd.op != OP_TRUE && d.width <= 32u) {
-          uint32_t *bits = bitsets + nd.slot * p.bitset_words;
-          const bool is_str = d.sc == 5;
-          if (is_str && and_mode) {
-            // few surviving rows and a larger dictionary: test the survivors' own entries instead of every entry
-            const uint32_t alive = warp_sum_u32(__popc(mybm));
-            if (alive * 4u <= d.dict_count) {
-              mybm = lean_survivor_str(p, nd, d, sbit, rs + hdr[nd.used_idx], mybm, nwords, alive, bm, lane);
-              continue;
-            }
-          }
-          if (!is_str && nd.range_ok && d.dict_sorted) {
-            uint32_t a, e;
-            lean_interval_sorted_int(d, nd, sbit, lane, a, e);
-            mybm = lean_rows<false>(d, sbit, nullptr, a, e, nd.negate != 0, mybm, myvalid, nwords, and_mode, lane);
-            goto leaf_done;
-          }
-          if (!is_str && nd.range_ok) lean_bitset_int_range(d, nd, sbit, bits, lane);
-          else if (is_str && (nd.op == OP_EQ || nd.op == OP_NE || nd.op == OP_IN)) lean_bitset_str_eq(p, nd, d, sbit, bits, lane);
-          else {
-            c.b.s = rs + hdr[nd.used_idx];
-            c.sbit = sbit;
-            build_dict_bitset(p, c.b, d, nd, bits, t);
-          }
-          __syncwarp();
-          mybm = lean_rows<true>(d, sbit, bits, 0u, 0u, false, mybm, myvalid, nwords, and_mode, lane);
-        } else {
-          bm[lane] = mybm;   // words_cap >= 32 words are reserved for the spilled bitmap
-          __syncwarp();
-          bool inited = true;
-          leaf_step(p, c, c, nd, false, inited, bm, rows, nwords, and_mode, t, staged_at);
-          mybm = (uint32_t)lane < nwords ? bm[lane] : 0u;
-        }
-      leaf_done:
+        const RecDesc d = rec_desc(p, reinterpret_cast<const StageRec *>(m + kMetaPlans)[nd.used_idx], nd.used_idx);
+        mybm = lean_leaf(p, nd, d, (smem_u32(rs) + (uint32_t)hdr[nd.used_idx]) * 8u, rs + hdr[nd.used_idx],
+                         bitsets + nd.slot * p.bitset_words, bm, mybm, myvalid, nwords, and_mode, lane);
         if (i + 1 < n_leaves && !__any_sync(0xffffffffu, and_mode ? mybm != 0u : mybm != myvalid)) break;   // early-out
       }
       if ((uint32_t)lane < nwords) gbm[lane] = mybm;
       cnt = __popc(mybm);
     } else {
-      // leaf_list_over_words written out: at 64 registers the shared loop costs this kernel 4 bytes of spills
-      bool inited = false;
-      for (int i = 0; i < n_leaves; ++i) {
-        const FilterNodeDev &nd = p.nodes[i];
-        if (p.leaf_const != nullptr && p.leaf_const[(int64_t)blk * p.n_nodes + i] != 0) continue;
+      const ColDesc *descs = reinterpret_cast<const ColDesc *>(m + kMetaPlans);
+      BlockCtx c;
+      view_from_rec(rec, nullptr, c.b);
+      c.descs = descs;
+      c.bitsets = bitsets;
+      c.rle_base = nullptr;
+      c.rle_slot_bytes = c.rle_starts_bytes = 0;
+      const bool and_mode = p.simple_shape == 1;
+      const int n_leaves = p.n_nodes == 1 ? 1 : p.n_nodes - 1;
+      // every filter column is staged: block-relative offsets of a leaf's column resolve into its region
+      auto staged_at = [&](const FilterNodeDev &nd, const ColDesc &, BlockCtx &cs) {
         if (nd.op != OP_FALSE && nd.op != OP_TRUE) {
-          c.b.s = rs + hdr[nd.used_idx];
-          c.sbit = (smem_u32(rs) + (uint32_t)hdr[nd.used_idx]) * 8u;
+          cs.b.s = rs + hdr[nd.used_idx];
+          cs.sbit = (smem_u32(rs) + (uint32_t)hdr[nd.used_idx]) * 8u;
         }
-        const ColDesc &d = descs[nd.used_idx];
-        if (nd.slot >= 0 && is_dict_kind(d)) {
-          build_dict_bitset(p, c.b, d, nd, bitsets + nd.slot * p.bitset_words, t);
-          __syncwarp();
+        return true;
+      };
+      if (nwords <= 32u) {
+        // ---- lean path: the block's bitmap lives in registers (lane g owns word g); dictionary-coded leaves run
+        // through explicit shared-memory loads, everything else through the generic leaf code on a spilled bitmap
+        const uint32_t myvalid = (uint32_t)lane < nwords ? valid_mask_of(rows, (uint32_t)lane) : 0u;
+        uint32_t mybm = and_mode ? myvalid : 0u;
+        for (int i = 0; i < n_leaves; ++i) {
+          const FilterNodeDev &nd = p.nodes[i];
+          if (p.leaf_const != nullptr && p.leaf_const[(int64_t)blk * p.n_nodes + i] != 0) continue;
+          const ColDesc &d = descs[nd.used_idx];
+          const uint32_t sbit = (smem_u32(rs) + (uint32_t)hdr[nd.used_idx]) * 8u;
+          if (d.kind == K_DICT && nd.slot >= 0 && nd.op != OP_FALSE && nd.op != OP_TRUE && d.width <= 32u) {
+            uint32_t *bits = bitsets + nd.slot * p.bitset_words;
+            const bool is_str = d.sc == 5;
+            if (is_str && and_mode) {
+              // few surviving rows and a larger dictionary: test the survivors' own entries instead of every entry
+              const uint32_t alive = warp_sum_u32(__popc(mybm));
+              if (alive * 4u <= d.dict_count) {
+                mybm = lean_survivor_str(p, nd, d, sbit, rs + hdr[nd.used_idx], mybm, nwords, alive, bm, lane);
+                continue;
+              }
+            }
+            if (!is_str && nd.range_ok && d.dict_sorted) {
+              uint32_t a, e;
+              lean_interval_sorted_int(d, nd, sbit, lane, a, e);
+              mybm = lean_rows<false>(d, sbit, nullptr, a, e, nd.negate != 0, mybm, myvalid, nwords, and_mode, lane);
+              goto leaf_done;
+            }
+            if (!is_str && nd.range_ok) lean_bitset_int_range(d, nd, sbit, bits, lane);
+            else if (is_str && (nd.op == OP_EQ || nd.op == OP_NE || nd.op == OP_IN)) lean_bitset_str_eq(p, nd, d, sbit, bits, lane);
+            else {
+              c.b.s = rs + hdr[nd.used_idx];
+              c.sbit = sbit;
+              build_dict_bitset(p, c.b, d, nd, bits, t);
+            }
+            __syncwarp();
+            mybm = lean_rows<true>(d, sbit, bits, 0u, 0u, false, mybm, myvalid, nwords, and_mode, lane);
+          } else {
+            bm[lane] = mybm;   // words_cap >= 32 words are reserved for the spilled bitmap
+            __syncwarp();
+            bool inited = true;
+            leaf_step(p, c, c, nd, false, inited, bm, rows, nwords, and_mode, t, staged_at);
+            mybm = (uint32_t)lane < nwords ? bm[lane] : 0u;
+          }
+        leaf_done:
+          if (i + 1 < n_leaves && !__any_sync(0xffffffffu, and_mode ? mybm != 0u : mybm != myvalid)) break;   // early-out
         }
-        if (i == 0 && leaf_first_fast<false>(p, c, nd, bm, rows, nwords, t)) {
-          inited = true;
+        if ((uint32_t)lane < nwords) gbm[lane] = mybm;
+        cnt = __popc(mybm);
+      } else {
+        // leaf_list_over_words written out: at 64 registers the shared loop costs this kernel 4 bytes of spills
+        bool inited = false;
+        for (int i = 0; i < n_leaves; ++i) {
+          const FilterNodeDev &nd = p.nodes[i];
+          if (p.leaf_const != nullptr && p.leaf_const[(int64_t)blk * p.n_nodes + i] != 0) continue;
+          if (nd.op != OP_FALSE && nd.op != OP_TRUE) {
+            c.b.s = rs + hdr[nd.used_idx];
+            c.sbit = (smem_u32(rs) + (uint32_t)hdr[nd.used_idx]) * 8u;
+          }
+          const ColDesc &d = descs[nd.used_idx];
+          if (nd.slot >= 0 && is_dict_kind(d)) {
+            build_dict_bitset(p, c.b, d, nd, bitsets + nd.slot * p.bitset_words, t);
+            __syncwarp();
+          }
+          if (i == 0 && leaf_first_fast<false>(p, c, nd, bm, rows, nwords, t)) {
+            inited = true;
+            __syncwarp();
+            continue;
+          }
+          if (!inited) {
+            for (uint32_t g = (uint32_t)lane; g < nwords; g += 32u) bm[g] = and_mode ? valid_mask_of(rows, g) : 0u;
+            inited = true;
+            __syncwarp();
+          }
+          leaf_over_words<false>(p, c, nd, bm, rows, nwords, and_mode, t);
           __syncwarp();
-          continue;
+          if (i + 1 < n_leaves) {
+            bool undecided = false;
+            for (uint32_t g = (uint32_t)lane; g < nwords; g += 32u)
+              undecided = undecided || (and_mode ? bm[g] != 0u : bm[g] != valid_mask_of(rows, g));
+            if (!__any_sync(0xffffffffu, undecided)) break;
+          }
         }
         if (!inited) {
           for (uint32_t g = (uint32_t)lane; g < nwords; g += 32u) bm[g] = and_mode ? valid_mask_of(rows, g) : 0u;
-          inited = true;
           __syncwarp();
         }
-        leaf_over_words<false>(p, c, nd, bm, rows, nwords, and_mode, t);
-        __syncwarp();
-        if (i + 1 < n_leaves) {
-          bool undecided = false;
-          for (uint32_t g = (uint32_t)lane; g < nwords; g += 32u)
-            undecided = undecided || (and_mode ? bm[g] != 0u : bm[g] != valid_mask_of(rows, g));
-          if (!__any_sync(0xffffffffu, undecided)) break;
+        for (uint32_t g = (uint32_t)lane; g < nwords; g += 32u) {
+          const uint32_t w = bm[g];
+          gbm[g] = w;
+          cnt += __popc(w);
         }
-      }
-      if (!inited) {
-        for (uint32_t g = (uint32_t)lane; g < nwords; g += 32u) bm[g] = and_mode ? valid_mask_of(rows, g) : 0u;
-        __syncwarp();
-      }
-      for (uint32_t g = (uint32_t)lane; g < nwords; g += 32u) {
-        const uint32_t w = bm[g];
-        gbm[g] = w;
-        cnt += __popc(w);
       }
     }
     cnt = warp_sum_u32(cnt);
@@ -494,21 +583,20 @@ struct FlatCol {
   uint32_t last_end;   // string dictionary: END of the last entry, relative to the var data
   uint8_t kind, elem_len, pc, pad_;
 };
-static_assert(sizeof(FlatCol) <= sizeof(ColDesc), "a flat entry replaces its column's plan");
+static_assert(sizeof(FlatCol) <= sizeof(ColDesc) && sizeof(FlatCol) <= kProjEnt<true>, "a flat entry replaces its column's plan or record");
 static_assert(kMetaPlans >= kMaxProj, "the flat column list (one byte per column) fits before the plans");
 
-__device__ __forceinline__ bool flat_kind(const ColDesc &d) {
-  if (d.kind == K_BITS) return d.sc != 5 && d.ext_bit == 0 && !d.sign_fix && !d.var_is_last;
-  if (d.kind == K_DICT) return d.sc == 5 ? !d.dict_fixed : d.dict_data_size <= 8u;
-  return false;
-}
+__device__ __forceinline__ const ColDesc &flat_desc(const ScanParams &, const ColDesc &d, int) { return d; }
+__device__ __forceinline__ RecDesc flat_desc(const ScanParams &p, const StageRec &r, int pc) { return rec_desc(p, r, p.proj_used[pc]); }
 
-// Entry of projected column pc (flat_kind) from its plan and its staged byte ranges (slot deltas d0, d1). Not inlined: once
-// per block, and inlined into obgpu_project_pipe_kernel it costs the kernel spills at 64 registers.
-// dst overlays the plan d: the entry is built in registers and stored with memcpy, whose byte stores may alias any type, so
-// no load of the plan can move past them.
-__device__ __noinline__ void flat_fill(const ScanParams &p, const ColDesc &d, int pc, uint32_t rs_addr, int32_t d0, int32_t d1,
+// Entry of projected column pc (flat_kind) from its plan or stage record and its staged byte ranges (slot deltas d0, d1). Not
+// inlined: once per block, and inlined into obgpu_project_pipe_kernel it costs the kernel spills at 64 registers.
+// dst overlays src: the entry is built in registers and stored with memcpy, whose byte stores may alias any type, so
+// no load of src can move past them.
+template <class S>
+__device__ __noinline__ void flat_fill(const ScanParams &p, const S &src, int pc, uint32_t rs_addr, int32_t d0, int32_t d1,
                                        int64_t base, uint64_t blk_addr, void *dst) {
+  const auto &d = flat_desc(p, src, pc);
   FlatCol f;
   const uint32_t s0 = (rs_addr + (uint32_t)d0) * 8u;
   uint32_t rbit = s0, ibit = s0;
@@ -537,14 +625,15 @@ __device__ __noinline__ void flat_fill(const ScanParams &p, const ColDesc &d, in
 }
 
 // Item k = f * cnt + j (flat column f, selected row j); lane l starts at item l and steps by 32.
-// Flat column f is the entry over plan cols[f] of `plans`.
-__device__ __forceinline__ void project_flat(const ScanParams &p, const ColDesc *plans, const uint8_t *cols, uint32_t nflat,
+// Flat column f is the entry over meta-slot entry cols[f] of `ents` (kEnt bytes each).
+template <uint32_t kEnt>
+__device__ __forceinline__ void project_flat(const ScanParams &p, const uint8_t *ents, const uint8_t *cols, uint32_t nflat,
                                              const uint16_t *sel, uint32_t cnt, int64_t base, bool all_rows, int lane) {
   const uint32_t qf = 32u / cnt, qj = 32u % cnt;
   uint32_t f = (uint32_t)lane / cnt, j = (uint32_t)lane % cnt;
   for (; f < nflat; f += qf, j += qj) {
     if (j >= cnt) { j -= cnt; ++f; if (f >= nflat) break; }
-    const FlatCol &c = *reinterpret_cast<const FlatCol *>(plans + cols[f]);
+    const FlatCol &c = *reinterpret_cast<const FlatCol *>(ents + (uint32_t)cols[f] * kEnt);
     const uint32_t row = all_rows ? j : (uint32_t)sel[j];
     const uint32_t at = c.vbit + row * c.stride, width = c.width;
     bool is_null = false;
@@ -583,7 +672,10 @@ __device__ __forceinline__ void project_flat(const ScanParams &p, const ColDesc 
   }
 }
 
+template <bool REC>
 __global__ void __launch_bounds__(kThreads) obgpu_project_pipe_kernel(const __grid_constant__ ScanParams p) {
+  constexpr uint32_t kEnt = kProjEnt<REC>, kSrc = REC ? (uint32_t)sizeof(StageRec) : (uint32_t)sizeof(ColDesc);
+  constexpr int kSrcPieces = (int)(kSrc / 16u);
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const int nwarps_total = (int)gridDim.x * kWarps;
   int blk = (int)blockIdx.x * kWarps + warp;
@@ -607,15 +699,16 @@ __global__ void __launch_bounds__(kThreads) obgpu_project_pipe_kernel(const __gr
     if (b >= p.n_blocks) return;
     const uint32_t sa = smem_u32(meta0 + (uint32_t)slot * p.pp_meta_bytes);
     const uint8_t *rec = reinterpret_cast<const uint8_t *>(p.recs + b);
-    const uint8_t *plans = reinterpret_cast<const uint8_t *>(p.plans + (int64_t)b * p.max_cols);
+    const uint8_t *ents = REC ? reinterpret_cast<const uint8_t *>(p.stage + (int64_t)b * p.max_cols)
+                              : reinterpret_cast<const uint8_t *>(p.plans + (int64_t)b * p.max_cols);
     constexpr int kHead = kRecPieces + 2;   // the record, then the two sel_offset entries
-    for (int q = lane; q < kHead + np * kPlanPieces; q += 32) {
+    for (int q = lane; q < kHead + np * kSrcPieces; q += 32) {
       if (q < kRecPieces) cp_async16(sa + (uint32_t)q * 16u, rec + q * 16);
       else if (q < kHead) cp_async8(sa + kMetaSel + (uint32_t)(q - kRecPieces) * 8u, p.sel_offset + b + (q - kRecPieces));
       else {
-        const int i = (q - kHead) / kPlanPieces, piece = (q - kHead) % kPlanPieces;
-        cp_async16(sa + kMetaPlans + (uint32_t)i * (uint32_t)sizeof(ColDesc) + (uint32_t)piece * 16u,
-                   plans + (size_t)p.used_col[p.proj_used[i]] * sizeof(ColDesc) + piece * 16);
+        const int i = (q - kHead) / kSrcPieces, piece = (q - kHead) % kSrcPieces;
+        cp_async16(sa + kMetaPlans + (uint32_t)i * kEnt + (uint32_t)piece * 16u,
+                   ents + (size_t)p.used_col[p.proj_used[i]] * kSrc + piece * 16);
       }
     }
   };
@@ -637,15 +730,23 @@ __global__ void __launch_bounds__(kThreads) obgpu_project_pipe_kernel(const __gr
       const uint32_t *gbm = p.bitmap_words + rec.bm_word_off;
       for (uint32_t g = (uint32_t)lane; g < nwords; g += 32u) cp_async4(smem_u32(rs) + hdr_bytes + g * 4u, gbm + g);
     }
-    const ColDesc *plans = reinterpret_cast<const ColDesc *>(m + kMetaPlans);
     int32_t *hdr = reinterpret_cast<int32_t *>(rs);
     uint32_t r[4] = {0, 0, 0, 0};
     int nr = 0;
     if (lane < np) {
-      BlockView bv;
-      view_from_rec(rec, nullptr, bv);
-      const ColDesc &d = plans[lane];
-      nr = d.ok ? proj_ranges(d, bv, r) : 0;
+      if constexpr (REC) {
+        const StageRec &sr = *reinterpret_cast<const StageRec *>(m + kMetaPlans + (uint32_t)lane * kEnt);
+        r[0] = (uint32_t)sr.lo[0] * 16u;
+        r[1] = (uint32_t)sr.hi[0] * 16u;
+        r[2] = (uint32_t)sr.lo[1] * 16u;
+        r[3] = (uint32_t)sr.hi[1] * 16u;
+        nr = r[3] != r[2] ? 2 : 1;
+      } else {
+        BlockView bv;
+        view_from_rec(rec, nullptr, bv);
+        const ColDesc &d = reinterpret_cast<const ColDesc *>(m + kMetaPlans)[lane];
+        nr = d.ok ? proj_ranges(d, bv, r) : 0;
+      }
       const uint32_t lim = ((rec.size + 15u) & ~15u) + 32u;
       if (nr > 0 && ((r[1] - r[0]) + (nr == 2 ? r[3] - r[2] : 0u) > p.pp_span[lane] || r[1] > lim || (nr == 2 && r[3] > lim))) nr = 0;
       if (nr == 0) r[0] = r[1] = r[2] = r[3] = 0;
@@ -705,7 +806,8 @@ __global__ void __launch_bounds__(kThreads) obgpu_project_pipe_kernel(const __gr
       __syncwarp();
       continue;
     }
-    ColDesc *plans = reinterpret_cast<ColDesc *>(m + kMetaPlans);
+    uint8_t *ents = m + kMetaPlans;
+    ColDesc *plans = reinterpret_cast<ColDesc *>(ents);
     const int32_t *hdr = reinterpret_cast<const int32_t *>(rs);
     const uint32_t badmask = (uint32_t)hdr[2 * kMaxProj];
     const bool all_rows = cnt == rows;
@@ -732,20 +834,23 @@ __global__ void __launch_bounds__(kThreads) obgpu_project_pipe_kernel(const __gr
     c.rle_slot_bytes = 0;
     c.rle_starts_bytes = p.words_cap * 4u;
     const uint64_t blk_addr = block_string_addr(p, blk, rec.off);
-    const bool flat = lane < np && plans[lane].ok && !((badmask >> lane) & 1u) && flat_kind(plans[lane]);
+    // with records every projected column is flat in every block (layout_pipe)
+    const bool flat = lane < np && !((badmask >> lane) & 1u) && (REC || (plans[lane].ok && flat_kind(plans[lane])));
     const uint32_t flatmask = __ballot_sync(0xffffffffu, flat);
     if (flatmask != 0u) {
       if (flat) {
-        flat_fill(p, plans[lane], lane, smem_u32(rs), hdr[2 * lane], hdr[2 * lane + 1], base, blk_addr, plans + lane);
+        uint8_t *ent = ents + (uint32_t)lane * kEnt;
+        if constexpr (REC) flat_fill(p, *reinterpret_cast<const StageRec *>(ent), lane, smem_u32(rs), hdr[2 * lane], hdr[2 * lane + 1], base, blk_addr, ent);
+        else flat_fill(p, *reinterpret_cast<const ColDesc *>(ent), lane, smem_u32(rs), hdr[2 * lane], hdr[2 * lane + 1], base, blk_addr, ent);
         m[__popc(flatmask & ((1u << lane) - 1u))] = (uint8_t)lane;
       }
       __syncwarp();
-      project_flat(p, plans, m, (uint32_t)__popc(flatmask), sel, cnt, base, all_rows, lane);
+      project_flat<kEnt>(p, ents, m, (uint32_t)__popc(flatmask), sel, cnt, base, all_rows, lane);
     }
     for (int pc = 0; pc < np; ++pc) {
       if ((flatmask >> pc) & 1u) continue;
       ColDesc *wdesc = plans + pc;
-      if (!wdesc->ok || ((badmask >> pc) & 1u)) {
+      if (REC || !wdesc->ok || ((badmask >> pc) & 1u)) {
         if (lane == 0) atomicOr(p.status, ST_UNSUPPORTED);
         continue;
       }
