@@ -2293,6 +2293,20 @@ static void layout_pipe(const obgpu_batch *b, ScanParams &p, int max_smem) {
   p.pc_rec = p.pp_rec = 0;
   if (!pipe_wanted(b->max_rows)) return;
   auto r16 = [](uint32_t v) { return (v + 15u) & ~15u; };
+  // n column areas back to back in a region slot: column i (block column col(i)) at off[i], with its widest span in the batch rounded
+  // to 16 bytes as its budget span[i]. Returns the bytes of all n, or 0xffffffff for a column with no bounded span or one over cap.
+  auto pack_spans = [&](int n, auto col, const std::vector<uint32_t> &spans, uint32_t cap, uint32_t *off, uint32_t *span) {
+    uint32_t at = 0;
+    for (int i = 0; i < n; ++i) {
+      const size_t c = (size_t)col(i);
+      const uint32_t sp = c < spans.size() ? spans[c] : 0xffffffffu;
+      if (sp == 0xffffffffu || sp > cap) return 0xffffffffu;
+      off[i] = at;
+      span[i] = r16(sp);
+      at += r16(sp);
+    }
+    return at;
+  };
   // stage records serve used column i when every block's record can stand in for its plan on that path, and the blocks agree on
   // the column's type (the record leaves the type facts to the scan)
   auto rec_ok = [&](int i, uint32_t gap) {
@@ -2311,16 +2325,8 @@ static void layout_pipe(const obgpu_batch *b, ScanParams &p, int max_smem) {
     while (nf < p.n_used && p.used_in_filter[nf]) ++nf;
     for (int i = nf; i < p.n_used; ++i) ok = ok && !p.used_in_filter[i];
     ok = ok && nf > 0 && nf <= 8;
-    uint32_t off = 0;
-    for (int i = 0; i < nf && ok; ++i) {
-      const size_t col = (size_t)p.used_col[i];
-      const uint32_t sp = col < b->col_span.size() ? b->col_span[col] : 0xffffffffu;
-      if (sp == 0xffffffffu || sp > 12288u) { ok = false; break; }
-      p.pf_off[i] = off;
-      p.pf_span[i] = r16(sp);
-      off += r16(sp);
-    }
-    if (ok) {
+    const uint32_t off = ok ? pack_spans(nf, [&](int i) { return p.used_col[i]; }, b->col_span, 12288u, p.pf_off, p.pf_span) : 0xffffffffu;
+    if (off != 0xffffffffu) {
       p.pf_n = nf;
       // records: every block has at most 1024 rows (bitmap in registers) and every leaf takes a lean path (lean_leaf) on
       // a column whose records all serve the filter
@@ -2346,17 +2352,10 @@ static void layout_pipe(const obgpu_batch *b, ScanParams &p, int max_smem) {
   }
   // ---- project ------------------------------------------------------------------------------------------------------
   if (p.n_proj + p.want_row_ids > 0) {
-    bool ok = p.n_proj <= 32;   // one lane per projected column computes and issues its byte ranges
-    uint32_t off = 0;
-    for (int i = 0; i < p.n_proj && ok; ++i) {
-      const size_t col = (size_t)p.used_col[p.proj_used[i]];
-      const uint32_t sp = col < b->col_pspan.size() ? b->col_pspan[col] : 0xffffffffu;
-      if (sp == 0xffffffffu || sp > 16384u) { ok = false; break; }
-      p.pp_off[i] = off;
-      p.pp_span[i] = r16(sp);
-      off += r16(sp);
-    }
-    if (ok) {
+    // one lane per projected column computes and issues its byte ranges
+    const uint32_t off = p.n_proj <= 32 ? pack_spans(p.n_proj, [&](int i) { return p.used_col[p.proj_used[i]]; }, b->col_pspan, 16384u,
+                                                     p.pp_off, p.pp_span) : 0xffffffffu;
+    if (off != 0xffffffffu) {
       bool rec = true;
       for (int i = 0; i < p.n_proj && rec; ++i) rec = rec_ok(p.proj_used[i], SR_NOT_FLAT);
       p.pp_rec = rec ? 1 : 0;

@@ -3,13 +3,16 @@
 // global round trips (record -> plans -> column bytes), not by bandwidth. These two kernels keep ONE WARP per block
 // but run it as a software pipeline over the blocks it owns (persistent grid, blocks strided over the warps):
 //
-//     iteration b:   wait   regions(b), meta(b + 1)          (cp.async groups, issued one / two iterations ago)
+//     iteration b:   wait   regions(b), meta(b + 1)          (issued one / two iterations ago)
 //                    issue  regions(b + 1)   <- needs meta(b + 1): block offset, decode plans -> column byte ranges
 //                    issue  meta(b + 2)      <- block record, decode plans (and the two prefix entries)
 //                    work   on block b from shared memory
 //
-// so a block's three round trips overlap the work on the two blocks before it. All copies are 16-byte cp.async
-// (LDGSTS: no registers, no mbarrier), completion is cp.async.wait_group + __syncwarp.
+// so a block's three round trips overlap the work on the two blocks before it. Meta copies are cp.async (LDGSTS: no
+// registers), completed by cp.async.wait_group + __syncwarp; region copies are TMA bulk copies completing on one mbarrier per
+// region slot. warp_pipeline owns that loop, its rings and its waits; each kernel gives it three steps -- issue a block's meta,
+// issue its regions, work on it -- and reads each column's meta entry (a plan, or a stage record) through one set of helpers:
+// issue_meta, staged_ranges, lean_leaf / flat_fill.
 //   obgpu_count_pipe_kernel   : stages every filter column's region of the block at once, then the same leaf loops
 //                               as obgpu_count_kernel (K4 / K6 / K9 / K14)
 //   obgpu_project_pipe_kernel : stages the block's bitmap words and the projected columns' byte ranges; a projected
@@ -18,6 +21,8 @@
 //                               "Flat" columns (project_flat) are decoded in one pass over (column, selected row)
 //                               items, the others column after column
 #pragma once
+
+#include <type_traits>
 
 __device__ __forceinline__ void cp_async16(uint32_t saddr, const void *g) {
   asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(saddr), "l"(g) : "memory");
@@ -56,7 +61,7 @@ constexpr int kPipeMaxFilterCols = 8;
 constexpr uint32_t kCountHdrBytes = 64u;   // count region slot: deltas + flags | regions
 // meta slot: [block record | project: sel_offset[b], sel_offset[b + 1] | decode plans], copied in 16-byte pieces
 // (the two sel_offset entries in 8-byte ones)
-constexpr int kRecPieces = (int)(sizeof(BlockRec) / 16), kPlanPieces = (int)(sizeof(ColDesc) / 16);
+constexpr int kRecPieces = (int)(sizeof(BlockRec) / 16);
 constexpr uint32_t kMetaSel = (uint32_t)sizeof(BlockRec), kMetaPlans = kMetaSel + 2u * (uint32_t)sizeof(int64_t);
 static_assert(kMetaPlans % 16u == 0u, "decode plans are copied in 16-byte pieces");
 
@@ -224,13 +229,14 @@ __device__ __forceinline__ uint32_t lean_survivor_str(const ScanParams &p, const
 
 // A stage record (scan_device.cuh) in a meta slot read under the plan's field names, with the column's type facts of the
 // scan (store class, datum length, sign-fix mask: the same for every block of a column whose blocks agree on its type): the
-// lean leaves and flat_fill take either a plan or this.
+// lean leaves and flat_fill take either a plan or this. desc_of gives used column `used`'s descriptor from its meta-slot entry.
 struct RecDesc {
   uint64_t base, int_mask;
   uint32_t val_bit, stride, width, dict_count, dict_payload, dict_data_size, dict_var, dict_end;
   uint8_t kind, sc, elem_len, sign_fix, dict_sorted, dict_fixed;
 };
-__device__ __forceinline__ RecDesc rec_desc(const ScanParams &p, const StageRec &r, int used) {
+__device__ __forceinline__ const ColDesc &desc_of(const ScanParams &, const ColDesc &d, int) { return d; }
+__device__ __forceinline__ RecDesc desc_of(const ScanParams &p, const StageRec &r, int used) {
   RecDesc d;
   d.sc = p.used_sc[used];
   d.elem_len = p.used_elem_len[used];
@@ -253,15 +259,18 @@ __device__ __forceinline__ RecDesc rec_desc(const ScanParams &p, const StageRec 
 }
 // Meta-slot entry of a column: its plan, or its stage record (count) / its stage record with room for the FlatCol entry
 // flat_fill writes over it (projection).
-template <bool REC> constexpr uint32_t kCountEnt = REC ? (uint32_t)sizeof(StageRec) : (uint32_t)sizeof(ColDesc);
+template <bool REC> using MetaEnt = typename std::conditional<REC, StageRec, ColDesc>::type;
+template <bool REC> constexpr uint32_t kCountEnt = (uint32_t)sizeof(MetaEnt<REC>);
 template <bool REC> constexpr uint32_t kProjEnt = REC ? 64u : (uint32_t)sizeof(ColDesc);
 
-// One lean leaf on the K_DICT column of stage record d (width <= 32) staged at sbit (generic address rs_col): returns the lane's
-// bitmap word. The plan path of obgpu_count_pipe_kernel writes the same steps out with a fall-back to the generic dictionary
-// bitset (build_dict_bitset); layout_pipe gives a scan records only when no leaf needs that fall-back.
-__device__ __forceinline__ uint32_t lean_leaf(const ScanParams &p, const FilterNodeDev &nd, const RecDesc &d, uint32_t sbit, const uint8_t *rs_col,
+// One lean leaf on the K_DICT column of descriptor d (width <= 32) staged at sbit (generic address rs_col): returns the lane's
+// bitmap word. A plan's leaf that is neither an integer range nor a string EQ / NE / IN falls back to the generic dictionary bitset
+// (build_dict_bitset, over bv pointed at the staged column); layout_pipe gives a scan records only when no leaf needs it.
+template <class D>
+__device__ __forceinline__ uint32_t lean_leaf(const ScanParams &p, const FilterNodeDev &nd, const D &d, uint32_t sbit, const uint8_t *rs_col,
                                               uint32_t *bits, uint32_t *bm, uint32_t mybm, uint32_t myvalid, uint32_t nwords,
-                                              bool and_mode, int lane) {
+                                              bool and_mode, BlockView &bv, const Team &t, int lane) {
+  constexpr bool kPlan = std::is_same<D, ColDesc>::value;
   const bool is_str = d.sc == 5;
   if (is_str && and_mode) {
     // few surviving rows and a larger dictionary: test the survivors' own entries instead of every entry
@@ -273,10 +282,123 @@ __device__ __forceinline__ uint32_t lean_leaf(const ScanParams &p, const FilterN
     lean_interval_sorted_int(d, nd, sbit, lane, a, e);
     return lean_rows<false>(d, sbit, nullptr, a, e, nd.negate != 0, mybm, myvalid, nwords, and_mode, lane);
   }
-  if (!is_str && nd.range_ok) lean_bitset_int_range(d, nd, sbit, bits, lane);
-  else lean_bitset_str_eq(p, nd, d, sbit, bits, lane);
+  if (!is_str && nd.range_ok) {
+    lean_bitset_int_range(d, nd, sbit, bits, lane);
+  } else if (!kPlan || (is_str && (nd.op == OP_EQ || nd.op == OP_NE || nd.op == OP_IN))) {
+    lean_bitset_str_eq(p, nd, d, sbit, bits, lane);
+  } else if constexpr (kPlan) {
+    bv.s = rs_col;
+    build_dict_bitset(p, bv, d, nd, bits, t);
+  }
   __syncwarp();
   return lean_rows<true>(d, sbit, bits, 0u, 0u, false, mybm, myvalid, nwords, and_mode, lane);
+}
+
+// Issues block b's meta slot at shared address sa: the block record, for the projection (SEL) the two sel_offset entries, then n
+// entries from the block's plans or (REC) stage records, entry i taken from column col(i) into kEnt bytes at kMetaPlans + i kEnt.
+template <bool REC, bool SEL, uint32_t kEnt, class Col>
+__device__ __forceinline__ void issue_meta(const ScanParams &p, int b, uint32_t sa, int n, Col col, int lane) {
+  constexpr uint32_t kSrc = (uint32_t)sizeof(MetaEnt<REC>);
+  constexpr int kSrcPieces = (int)(kSrc / 16u), kHead = kRecPieces + (SEL ? 2 : 0);
+  const uint8_t *rec = reinterpret_cast<const uint8_t *>(p.recs + b);
+  const uint8_t *src = REC ? reinterpret_cast<const uint8_t *>(p.stage + (int64_t)b * p.max_cols)
+                           : reinterpret_cast<const uint8_t *>(p.plans + (int64_t)b * p.max_cols);
+  for (int q = lane; q < kHead + n * kSrcPieces; q += 32) {
+    if (q < kRecPieces) cp_async16(sa + (uint32_t)q * 16u, rec + q * 16);
+    else if (q < kHead) cp_async8(sa + kMetaSel + (uint32_t)(q - kRecPieces) * 8u, p.sel_offset + b + (q - kRecPieces));
+    else {
+      const int i = (q - kHead) / kSrcPieces, piece = (q - kHead) % kSrcPieces;
+      cp_async16(sa + kMetaPlans + (uint32_t)i * kEnt + (uint32_t)piece * 16u, src + (size_t)col(i) * kSrc + piece * 16);
+    }
+  }
+}
+
+// Byte ranges r = {lo0, hi0, lo1, hi1} of block rec that a kernel stages for the column of meta-slot entry ent: its filter
+// region (FILTER: [16 lo[0], 16 max(hi)) of a record, col_region of a plan) or its projection ranges (the record's, or
+// proj_ranges). Returns how many (1, or 2 for a string dictionary's refs and END offsets), or 0 -- r all zero -- when the column has
+// no bounded range, or its ranges exceed the column's budget or run past the block's padded end.
+template <bool REC, bool FILTER>
+__device__ __forceinline__ int staged_ranges(const BlockRec &rec, const uint8_t *ent, uint32_t budget, uint32_t r[4]) {
+  int nr;
+  if constexpr (REC) {
+    const StageRec &sr = *reinterpret_cast<const StageRec *>(ent);
+    r[0] = (uint32_t)sr.lo[0] * 16u;
+    r[1] = (uint32_t)(FILTER ? max(sr.hi[0], sr.hi[1]) : sr.hi[0]) * 16u;
+    r[2] = FILTER ? 0u : (uint32_t)sr.lo[1] * 16u;
+    r[3] = FILTER ? 0u : (uint32_t)sr.hi[1] * 16u;
+    nr = r[3] != r[2] ? 2 : 1;
+  } else {
+    BlockView bv;
+    view_from_rec(rec, nullptr, bv);
+    const ColDesc &d = *reinterpret_cast<const ColDesc *>(ent);
+    if (FILTER) nr = d.ok && col_region(d, bv, r[0], r[1]) ? 1 : 0;
+    else nr = d.ok ? proj_ranges(d, bv, r) : 0;
+  }
+  const uint32_t lim = ((rec.size + 15u) & ~15u) + 32u;
+  if (nr > 0 && ((r[1] - r[0]) + (nr == 2 ? r[3] - r[2] : 0u) > budget || r[1] > lim || (nr == 2 && r[3] > lim))) nr = 0;
+  if (nr == 0) r[0] = r[1] = r[2] = r[3] = 0;
+  return nr;
+}
+
+// Staged bit addresses of a string dictionary's refs (rbit) and END offsets (ibit) from the slot deltas d0, d1 of its projection
+// ranges: with two ranges they are ordered by block offset (proj_ranges); with one (d0 == d1) both are in it.
+template <class D>
+__device__ __forceinline__ void str_dict_bits(const D &d, uint32_t rs_addr, int32_t d0, int32_t d1, uint32_t &rbit, uint32_t &ibit) {
+  const uint32_t s0 = (rs_addr + (uint32_t)d0) * 8u, s1 = (rs_addr + (uint32_t)d1) * 8u;
+  const bool refs_first = (d.val_bit >> 3) < d.dict_payload;
+  rbit = refs_first ? s0 : s1;
+  ibit = refs_first ? s1 : s0;
+}
+
+// The warp pipeline of both kernels. Warp w of the persistent grid takes blocks w, w + W, w + 2W, ... (W: every warp of the grid)
+// through a meta ring of 3 slots and a region ring of 2 slots, with one mbarrier per region slot at bars. The kernel owns the slots'
+// layout and gives three steps, each called with the ring slots it is to use:
+//   meta(b, ms)              issue the cp.async copies of block b's meta into meta slot ms
+//   regions(b, ms, rsl)      from block b's landed meta slot ms, issue its region slot rsl (one mbar_expect_tx on bars[rsl], even
+//                            with nothing to copy, so the slot's phase completes)
+//   work(b, ms, rsl)         block b, with both of its slots landed
+// meta and regions are also called one and two blocks past the warp's last block and then return at once (the test sits in them:
+// in this loop it costs the plan kernels spills). K names the kernel's PIPE_CLOCK counters.
+template <int K, class Meta, class Regions, class Work>
+__device__ __forceinline__ void warp_pipeline(int n_blocks, uint64_t *bars, int lane, Meta meta, Regions regions, Work work) {
+  const int stride = (int)gridDim.x * kWarps;
+  int blk = (int)blockIdx.x * kWarps + (int)(threadIdx.x >> 5);
+  if (blk >= n_blocks) return;
+  if (lane == 0) {
+    mbar_init(bars, 1);
+    mbar_init(bars + 1, 1);
+    fence_barrier_init();
+  }
+  __syncwarp();
+  // prologue: meta(b0), then regions(b0) + meta(b1)
+  meta(blk, 0);
+  cp_async_commit();
+  cp_async_wait_all();
+  __syncwarp();
+  regions(blk, 0, 0);
+  cp_async_commit();
+  meta(blk + stride, 1);
+  cp_async_commit();
+  int it = 0;
+  PIPE_CLOCK_START();
+  for (; blk < n_blocks; blk += stride, ++it) {
+    const int rsl = it & 1;
+    PIPE_CLOCK_AT(pclk_a);
+    cp_async_wait_all();
+    mbar_wait(bars + rsl, (uint32_t)(it >> 1) & 1u);
+    __syncwarp();
+    PIPE_CLOCK_ADD(pclk_wait, pclk_a);
+    PIPE_CLOCK_AT(pclk_b);
+    regions(blk + stride, (it + 1) % 3, rsl ^ 1);
+    cp_async_commit();
+    meta(blk + 2 * stride, (it + 2) % 3);
+    cp_async_commit();
+    PIPE_CLOCK_ADD(pclk_issue, pclk_b);
+    work(blk, it % 3, rsl);
+    __syncwarp();   // every lane is done with this iteration's slots before the next iteration refills them
+  }
+  PIPE_CLOCK_STOP(K);
+  cp_async_wait_all();
 }
 
 // =================================================================================================
@@ -286,106 +408,51 @@ __device__ __forceinline__ uint32_t lean_leaf(const ScanParams &p, const FilterN
 template <bool REC>
 __global__ void __launch_bounds__(kThreads) obgpu_count_pipe_kernel(const __grid_constant__ ScanParams p) {
   constexpr uint32_t kEnt = kCountEnt<REC>;
-  constexpr int kEntPieces = (int)(kEnt / 16u);
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  const int nwarps_total = (int)gridDim.x * kWarps;
-  int blk = (int)blockIdx.x * kWarps + warp;
-  if (blk >= p.n_blocks) return;
   uint8_t *wr = g_smem + (uint32_t)warp * p.pc_bytes;
-  uint8_t *meta0 = wr + p.pc_meta, *reg0 = wr + p.pc_region;
   uint32_t *bm = reinterpret_cast<uint32_t *>(wr + p.pc_bm);
   uint32_t *bitsets = reinterpret_cast<uint32_t *>(wr + p.pc_bitset);
-  uint64_t *bars = reinterpret_cast<uint64_t *>(wr + p.pc_bar);   // one mbarrier per region slot
   const int nf = p.pf_n;
   const Team t = warp_team(lane);
-  if (lane == 0) {
-    mbar_init(bars, 1);
-    mbar_init(bars + 1, 1);
-    fence_barrier_init();
-  }
-  __syncwarp();
+  // skip-index verdict of the block whose meta was issued last: fetched two blocks ahead of the block's work, it decides whether
+  // regions() stages the block and travels to work() in the region slot's header
+  uint32_t verdict = 0;
 
-  auto issue_meta = [&](int b, int slot) {
+  uint8_t *meta0 = wr + p.pc_meta, *reg0 = wr + p.pc_region;
+  uint64_t *bars = reinterpret_cast<uint64_t *>(wr + p.pc_bar);
+  auto meta = [&](int b, int ms) {
     if (b >= p.n_blocks) return;
-    const uint32_t sa = smem_u32(meta0 + (uint32_t)slot * p.pc_meta_bytes);
-    const uint8_t *rec = reinterpret_cast<const uint8_t *>(p.recs + b);
-    const uint8_t *ents = REC ? reinterpret_cast<const uint8_t *>(p.stage + (int64_t)b * p.max_cols)
-                              : reinterpret_cast<const uint8_t *>(p.plans + (int64_t)b * p.max_cols);
-    for (int q = lane; q < kRecPieces + nf * kEntPieces; q += 32) {
-      if (q < kRecPieces) cp_async16(sa + (uint32_t)q * 16u, rec + q * 16);
-      else {
-        const int i = (q - kRecPieces) / kEntPieces, piece = (q - kRecPieces) % kEntPieces;
-        cp_async16(sa + kMetaPlans + (uint32_t)i * kEnt + (uint32_t)piece * 16u, ents + (size_t)p.used_col[i] * kEnt + piece * 16);
-      }
-    }
+    uint8_t *m = meta0 + (uint32_t)ms * p.pc_meta_bytes;
+    if (p.blk_const != nullptr) verdict = p.blk_const[b];
+    issue_meta<REC, false, kEnt>(p, b, smem_u32(m), nf, [&](int i) { return p.used_col[i]; }, lane);
   };
-  // region slot: [int32 delta[kPipeMaxFilterCols] | uint32 flags] (64 bytes) then the regions at p.pf_off[i]
-  auto issue_regions = [&](int b, int mslot, int rslot, uint32_t verdict) {
+  // region slot: [int32 delta[kPipeMaxFilterCols] | declined mask | verdict] (64 bytes) then the regions at p.pf_off[i]
+  auto regions = [&](int b, int ms, int rsl) {
     if (b >= p.n_blocks) return;
-    const uint8_t *m = meta0 + (uint32_t)mslot * p.pc_meta_bytes;
-    uint8_t *rs = reg0 + (uint32_t)rslot * p.pc_region_bytes;
+    const uint8_t *m = meta0 + (uint32_t)ms * p.pc_meta_bytes;
+    uint8_t *rs = reg0 + (uint32_t)rsl * p.pc_region_bytes;
+    uint64_t *bar = bars + rsl;
     const BlockRec &rec = *reinterpret_cast<const BlockRec *>(m);
-    const ColDesc *descs = reinterpret_cast<const ColDesc *>(m + kMetaPlans);
     int32_t *hdr = reinterpret_cast<int32_t *>(rs);
-    uint32_t lo = 0, hi = 0;
+    uint32_t r[4] = {0, 0, 0, 0};
     bool bad = false;
     if (lane < nf && rec.rows != 0 && verdict == 0) {
-      if constexpr (REC) {
-        const StageRec &r = reinterpret_cast<const StageRec *>(m + kMetaPlans)[lane];
-        lo = (uint32_t)r.lo[0] * 16u;
-        hi = (uint32_t)max(r.hi[0], r.hi[1]) * 16u;
-        if (hi - lo > p.pf_span[lane] || hi > ((rec.size + 15u) & ~15u) + 32u) { bad = true; lo = hi = 0; }
-      } else {
-        BlockView bv;
-        view_from_rec(rec, nullptr, bv);
-        const ColDesc &d = descs[lane];
-        if (!d.ok || !col_region(d, bv, lo, hi) || hi - lo > p.pf_span[lane] || hi > ((rec.size + 15u) & ~15u) + 32u) { bad = true; lo = hi = 0; }
-      }
-      hdr[lane] = (int32_t)(kCountHdrBytes + p.pf_off[lane]) - (int32_t)lo;
+      bad = staged_ranges<REC, true>(rec, m + kMetaPlans + (uint32_t)lane * kEnt, p.pf_span[lane], r) == 0;
+      hdr[lane] = (int32_t)(kCountHdrBytes + p.pf_off[lane]) - (int32_t)r[0];
     }
     const uint32_t badmask = __ballot_sync(0xffffffffu, bad);
-    if (lane == 0) hdr[kPipeMaxFilterCols] = (int32_t)badmask;
+    if (lane == 0) {
+      hdr[kPipeMaxFilterCols] = (int32_t)badmask;
+      hdr[kPipeMaxFilterCols + 1] = (int32_t)verdict;
+    }
     // one bulk copy (TMA) per filter column, all completing on the slot's mbarrier
-    const uint32_t total = warp_sum_u32(hi - lo);
-    uint64_t *bar = bars + rslot;
+    const uint32_t total = warp_sum_u32(r[1] - r[0]);
     if (lane == 0) mbar_expect_tx(bar, total);
     __syncwarp();
-    if (hi > lo) tma_bulk_g2s(rs + kCountHdrBytes + p.pf_off[lane], p.image + rec.off + lo, hi - lo, bar);
+    if (r[1] > r[0]) tma_bulk_g2s(rs + kCountHdrBytes + p.pf_off[lane], p.image + rec.off + r[0], r[1] - r[0], bar);
   };
 
-  // prologue: meta(b0), then regions(b0) + meta(b1)
-  uint32_t v_cur = 0, v_next = 0, v_next2 = 0;   // skip-index verdicts, fetched two blocks ahead
-  if (p.blk_const != nullptr) {
-    v_cur = p.blk_const[blk];
-    if (blk + nwarps_total < p.n_blocks) v_next = p.blk_const[blk + nwarps_total];
-  }
-  issue_meta(blk, 0);
-  cp_async_commit();
-  cp_async_wait_all();
-  __syncwarp();
-  issue_regions(blk, 0, 0, v_cur);
-  cp_async_commit();
-  issue_meta(blk + nwarps_total, 1);
-  cp_async_commit();
-  int it = 0;
-  PIPE_CLOCK_START();
-  for (; blk < p.n_blocks; blk += nwarps_total, ++it) {
-    const int ms = it % 3, rsl = it & 1;
-    PIPE_CLOCK_AT(pclk_a);
-    cp_async_wait_all();
-    mbar_wait(bars + rsl, (uint32_t)(it >> 1) & 1u);
-    __syncwarp();
-    PIPE_CLOCK_ADD(pclk_wait, pclk_a);
-    PIPE_CLOCK_AT(pclk_b);
-    const int b2 = blk + 2 * nwarps_total;
-    if (p.blk_const != nullptr && b2 < p.n_blocks) v_next2 = p.blk_const[b2];
-    issue_regions(blk + nwarps_total, (it + 1) % 3, rsl ^ 1, v_next);
-    cp_async_commit();
-    issue_meta(b2, (it + 2) % 3);
-    cp_async_commit();
-    PIPE_CLOCK_ADD(pclk_issue, pclk_b);
-
-    // ---- block `blk` from shared memory -------------------------------------------------------------------------
+  auto work = [&](int blk, int ms, int rsl) {
     const uint8_t *m = meta0 + (uint32_t)ms * p.pc_meta_bytes;
     uint8_t *rs = reg0 + (uint32_t)rsl * p.pc_region_bytes;
     const BlockRec rec = *reinterpret_cast<const BlockRec *>(m);
@@ -393,147 +460,99 @@ __global__ void __launch_bounds__(kThreads) obgpu_count_pipe_kernel(const __grid
     const uint32_t rows = rec.rows;
     uint32_t *gbm = p.bitmap_words + rec.bm_word_off;
     const uint32_t nwords = (rows + 31u) >> 5;
-    const uint32_t verdict = v_cur;
-    v_cur = v_next;
-    v_next = v_next2;
-    if (count_block_settled(p, blk, rows, gbm, verdict, hdr[kPipeMaxFilterCols] != 0, lane)) {
-      __syncwarp();
-      continue;
-    }
+    if (count_block_settled(p, blk, rows, gbm, (uint32_t)hdr[kPipeMaxFilterCols + 1], hdr[kPipeMaxFilterCols] != 0, lane)) return;
+    const MetaEnt<REC> *ents = reinterpret_cast<const MetaEnt<REC> *>(m + kMetaPlans);
+    BlockCtx c;
+    view_from_rec(rec, nullptr, c.b);
+    c.descs = reinterpret_cast<const ColDesc *>(ents);
+    c.bitsets = bitsets;
+    c.rle_base = nullptr;
+    c.rle_slot_bytes = c.rle_starts_bytes = 0;
+    const bool and_mode = p.simple_shape == 1;
+    const int n_leaves = p.n_nodes == 1 ? 1 : p.n_nodes - 1;
+    // every filter column is staged: block-relative offsets of a leaf's column resolve into its region
+    auto staged_at = [&](const FilterNodeDev &nd, const ColDesc &, BlockCtx &cs) {
+      if (nd.op != OP_FALSE && nd.op != OP_TRUE) {
+        cs.b.s = rs + hdr[nd.used_idx];
+        cs.sbit = (smem_u32(rs) + (uint32_t)hdr[nd.used_idx]) * 8u;
+      }
+      return true;
+    };
     uint32_t cnt = 0;
-    if constexpr (REC) {
-      // stage records: every block has at most 1024 rows (bitmap in registers) and every leaf is lean (layout_pipe)
-      const bool and_mode = p.simple_shape == 1;
-      const int n_leaves = p.n_nodes == 1 ? 1 : p.n_nodes - 1;
+    if (REC || nwords <= 32u) {
+      // ---- lean path (with records every block has at most 1024 rows: layout_pipe): the block's bitmap lives in registers
+      // (lane g owns word g); dictionary-coded leaves run through explicit shared-memory loads, everything else (plans only)
+      // through the generic leaf code on a spilled bitmap
       const uint32_t myvalid = (uint32_t)lane < nwords ? valid_mask_of(rows, (uint32_t)lane) : 0u;
       uint32_t mybm = and_mode ? myvalid : 0u;
       for (int i = 0; i < n_leaves; ++i) {
         const FilterNodeDev &nd = p.nodes[i];
         if (p.leaf_const != nullptr && p.leaf_const[(int64_t)blk * p.n_nodes + i] != 0) continue;
-        const RecDesc d = rec_desc(p, reinterpret_cast<const StageRec *>(m + kMetaPlans)[nd.used_idx], nd.used_idx);
-        mybm = lean_leaf(p, nd, d, (smem_u32(rs) + (uint32_t)hdr[nd.used_idx]) * 8u, rs + hdr[nd.used_idx],
-                         bitsets + nd.slot * p.bitset_words, bm, mybm, myvalid, nwords, and_mode, lane);
+        const auto &d = desc_of(p, ents[nd.used_idx], nd.used_idx);
+        // with records every leaf is lean (layout_pipe)
+        if (REC || (d.kind == K_DICT && nd.slot >= 0 && nd.op != OP_FALSE && nd.op != OP_TRUE && d.width <= 32u)) {
+          mybm = lean_leaf(p, nd, d, (smem_u32(rs) + (uint32_t)hdr[nd.used_idx]) * 8u, rs + hdr[nd.used_idx],
+                           bitsets + nd.slot * p.bitset_words, bm, mybm, myvalid, nwords, and_mode, c.b, t, lane);
+        } else {
+          bm[lane] = mybm;   // words_cap >= 32 words are reserved for the spilled bitmap
+          __syncwarp();
+          bool inited = true;
+          leaf_step(p, c, c, nd, false, inited, bm, rows, nwords, and_mode, t, staged_at);
+          mybm = (uint32_t)lane < nwords ? bm[lane] : 0u;
+        }
         if (i + 1 < n_leaves && !__any_sync(0xffffffffu, and_mode ? mybm != 0u : mybm != myvalid)) break;   // early-out
       }
       if ((uint32_t)lane < nwords) gbm[lane] = mybm;
       cnt = __popc(mybm);
     } else {
-      const ColDesc *descs = reinterpret_cast<const ColDesc *>(m + kMetaPlans);
-      BlockCtx c;
-      view_from_rec(rec, nullptr, c.b);
-      c.descs = descs;
-      c.bitsets = bitsets;
-      c.rle_base = nullptr;
-      c.rle_slot_bytes = c.rle_starts_bytes = 0;
-      const bool and_mode = p.simple_shape == 1;
-      const int n_leaves = p.n_nodes == 1 ? 1 : p.n_nodes - 1;
-      // every filter column is staged: block-relative offsets of a leaf's column resolve into its region
-      auto staged_at = [&](const FilterNodeDev &nd, const ColDesc &, BlockCtx &cs) {
+      // leaf_list_over_words written out: at 64 registers the shared loop costs this kernel 4 bytes of spills
+      bool inited = false;
+      for (int i = 0; i < n_leaves; ++i) {
+        const FilterNodeDev &nd = p.nodes[i];
+        if (p.leaf_const != nullptr && p.leaf_const[(int64_t)blk * p.n_nodes + i] != 0) continue;
         if (nd.op != OP_FALSE && nd.op != OP_TRUE) {
-          cs.b.s = rs + hdr[nd.used_idx];
-          cs.sbit = (smem_u32(rs) + (uint32_t)hdr[nd.used_idx]) * 8u;
+          c.b.s = rs + hdr[nd.used_idx];
+          c.sbit = (smem_u32(rs) + (uint32_t)hdr[nd.used_idx]) * 8u;
         }
-        return true;
-      };
-      if (nwords <= 32u) {
-        // ---- lean path: the block's bitmap lives in registers (lane g owns word g); dictionary-coded leaves run
-        // through explicit shared-memory loads, everything else through the generic leaf code on a spilled bitmap
-        const uint32_t myvalid = (uint32_t)lane < nwords ? valid_mask_of(rows, (uint32_t)lane) : 0u;
-        uint32_t mybm = and_mode ? myvalid : 0u;
-        for (int i = 0; i < n_leaves; ++i) {
-          const FilterNodeDev &nd = p.nodes[i];
-          if (p.leaf_const != nullptr && p.leaf_const[(int64_t)blk * p.n_nodes + i] != 0) continue;
-          const ColDesc &d = descs[nd.used_idx];
-          const uint32_t sbit = (smem_u32(rs) + (uint32_t)hdr[nd.used_idx]) * 8u;
-          if (d.kind == K_DICT && nd.slot >= 0 && nd.op != OP_FALSE && nd.op != OP_TRUE && d.width <= 32u) {
-            uint32_t *bits = bitsets + nd.slot * p.bitset_words;
-            const bool is_str = d.sc == 5;
-            if (is_str && and_mode) {
-              // few surviving rows and a larger dictionary: test the survivors' own entries instead of every entry
-              const uint32_t alive = warp_sum_u32(__popc(mybm));
-              if (alive * 4u <= d.dict_count) {
-                mybm = lean_survivor_str(p, nd, d, sbit, rs + hdr[nd.used_idx], mybm, nwords, alive, bm, lane);
-                continue;
-              }
-            }
-            if (!is_str && nd.range_ok && d.dict_sorted) {
-              uint32_t a, e;
-              lean_interval_sorted_int(d, nd, sbit, lane, a, e);
-              mybm = lean_rows<false>(d, sbit, nullptr, a, e, nd.negate != 0, mybm, myvalid, nwords, and_mode, lane);
-              goto leaf_done;
-            }
-            if (!is_str && nd.range_ok) lean_bitset_int_range(d, nd, sbit, bits, lane);
-            else if (is_str && (nd.op == OP_EQ || nd.op == OP_NE || nd.op == OP_IN)) lean_bitset_str_eq(p, nd, d, sbit, bits, lane);
-            else {
-              c.b.s = rs + hdr[nd.used_idx];
-              c.sbit = sbit;
-              build_dict_bitset(p, c.b, d, nd, bits, t);
-            }
-            __syncwarp();
-            mybm = lean_rows<true>(d, sbit, bits, 0u, 0u, false, mybm, myvalid, nwords, and_mode, lane);
-          } else {
-            bm[lane] = mybm;   // words_cap >= 32 words are reserved for the spilled bitmap
-            __syncwarp();
-            bool inited = true;
-            leaf_step(p, c, c, nd, false, inited, bm, rows, nwords, and_mode, t, staged_at);
-            mybm = (uint32_t)lane < nwords ? bm[lane] : 0u;
-          }
-        leaf_done:
-          if (i + 1 < n_leaves && !__any_sync(0xffffffffu, and_mode ? mybm != 0u : mybm != myvalid)) break;   // early-out
-        }
-        if ((uint32_t)lane < nwords) gbm[lane] = mybm;
-        cnt = __popc(mybm);
-      } else {
-        // leaf_list_over_words written out: at 64 registers the shared loop costs this kernel 4 bytes of spills
-        bool inited = false;
-        for (int i = 0; i < n_leaves; ++i) {
-          const FilterNodeDev &nd = p.nodes[i];
-          if (p.leaf_const != nullptr && p.leaf_const[(int64_t)blk * p.n_nodes + i] != 0) continue;
-          if (nd.op != OP_FALSE && nd.op != OP_TRUE) {
-            c.b.s = rs + hdr[nd.used_idx];
-            c.sbit = (smem_u32(rs) + (uint32_t)hdr[nd.used_idx]) * 8u;
-          }
-          const ColDesc &d = descs[nd.used_idx];
-          if (nd.slot >= 0 && is_dict_kind(d)) {
-            build_dict_bitset(p, c.b, d, nd, bitsets + nd.slot * p.bitset_words, t);
-            __syncwarp();
-          }
-          if (i == 0 && leaf_first_fast<false>(p, c, nd, bm, rows, nwords, t)) {
-            inited = true;
-            __syncwarp();
-            continue;
-          }
-          if (!inited) {
-            for (uint32_t g = (uint32_t)lane; g < nwords; g += 32u) bm[g] = and_mode ? valid_mask_of(rows, g) : 0u;
-            inited = true;
-            __syncwarp();
-          }
-          leaf_over_words<false>(p, c, nd, bm, rows, nwords, and_mode, t);
+        const ColDesc &d = c.descs[nd.used_idx];
+        if (nd.slot >= 0 && is_dict_kind(d)) {
+          build_dict_bitset(p, c.b, d, nd, bitsets + nd.slot * p.bitset_words, t);
           __syncwarp();
-          if (i + 1 < n_leaves) {
-            bool undecided = false;
-            for (uint32_t g = (uint32_t)lane; g < nwords; g += 32u)
-              undecided = undecided || (and_mode ? bm[g] != 0u : bm[g] != valid_mask_of(rows, g));
-            if (!__any_sync(0xffffffffu, undecided)) break;
-          }
+        }
+        if (i == 0 && leaf_first_fast<false>(p, c, nd, bm, rows, nwords, t)) {
+          inited = true;
+          __syncwarp();
+          continue;
         }
         if (!inited) {
           for (uint32_t g = (uint32_t)lane; g < nwords; g += 32u) bm[g] = and_mode ? valid_mask_of(rows, g) : 0u;
+          inited = true;
           __syncwarp();
         }
-        for (uint32_t g = (uint32_t)lane; g < nwords; g += 32u) {
-          const uint32_t w = bm[g];
-          gbm[g] = w;
-          cnt += __popc(w);
+        leaf_over_words<false>(p, c, nd, bm, rows, nwords, and_mode, t);
+        __syncwarp();
+        if (i + 1 < n_leaves) {
+          bool undecided = false;
+          for (uint32_t g = (uint32_t)lane; g < nwords; g += 32u)
+            undecided = undecided || (and_mode ? bm[g] != 0u : bm[g] != valid_mask_of(rows, g));
+          if (!__any_sync(0xffffffffu, undecided)) break;
         }
+      }
+      if (!inited) {
+        for (uint32_t g = (uint32_t)lane; g < nwords; g += 32u) bm[g] = and_mode ? valid_mask_of(rows, g) : 0u;
+        __syncwarp();
+      }
+      for (uint32_t g = (uint32_t)lane; g < nwords; g += 32u) {
+        const uint32_t w = bm[g];
+        gbm[g] = w;
+        cnt += __popc(w);
       }
     }
     cnt = warp_sum_u32(cnt);
     if (lane == 0) p.counts[blk] = cnt;
-    __syncwarp();   // every lane is done with this iteration's slots before the next iteration refills them
-  }
-  PIPE_CLOCK_STOP(0);
-  cp_async_wait_all();
+  };
+
+  warp_pipeline<0>(p.n_blocks, bars, lane, meta, regions, work);
 }
 
 // =================================================================================================
@@ -586,9 +605,6 @@ struct FlatCol {
 static_assert(sizeof(FlatCol) <= sizeof(ColDesc) && sizeof(FlatCol) <= kProjEnt<true>, "a flat entry replaces its column's plan or record");
 static_assert(kMetaPlans >= kMaxProj, "the flat column list (one byte per column) fits before the plans");
 
-__device__ __forceinline__ const ColDesc &flat_desc(const ScanParams &, const ColDesc &d, int) { return d; }
-__device__ __forceinline__ RecDesc flat_desc(const ScanParams &p, const StageRec &r, int pc) { return rec_desc(p, r, p.proj_used[pc]); }
-
 // Entry of projected column pc (flat_kind) from its plan or stage record and its staged byte ranges (slot deltas d0, d1). Not
 // inlined: once per block, and inlined into obgpu_project_pipe_kernel it costs the kernel spills at 64 registers.
 // dst overlays src: the entry is built in registers and stored with memcpy, whose byte stores may alias any type, so
@@ -596,17 +612,11 @@ __device__ __forceinline__ RecDesc flat_desc(const ScanParams &p, const StageRec
 template <class S>
 __device__ __noinline__ void flat_fill(const ScanParams &p, const S &src, int pc, uint32_t rs_addr, int32_t d0, int32_t d1,
                                        int64_t base, uint64_t blk_addr, void *dst) {
-  const auto &d = flat_desc(p, src, pc);
+  const auto &d = desc_of(p, src, p.proj_used[pc]);
   FlatCol f;
-  const uint32_t s0 = (rs_addr + (uint32_t)d0) * 8u;
-  uint32_t rbit = s0, ibit = s0;
+  uint32_t rbit = (rs_addr + (uint32_t)d0) * 8u, ibit = rbit;
   f.kind = d.kind == K_BITS ? FLAT_BITS : d.sc == 5 ? FLAT_STR_DICT : FLAT_INT_DICT;
-  if (f.kind == FLAT_STR_DICT && d0 != d1) {
-    // which delta belongs to the refs: with two ranges they are ordered by block offset (proj_ranges)
-    const uint32_t s1 = (rs_addr + (uint32_t)d1) * 8u;
-    if ((d.val_bit >> 3) < d.dict_payload) ibit = s1;
-    else rbit = s1;
-  }
+  if (f.kind == FLAT_STR_DICT) str_dict_bits(d, rs_addr, d0, d1, rbit, ibit);
   f.elem_len = f.kind == FLAT_STR_DICT ? 8u : d.elem_len;
   f.pc = (uint8_t)pc;
   f.pad_ = 0;
@@ -674,55 +684,34 @@ __device__ __forceinline__ void project_flat(const ScanParams &p, const uint8_t 
 
 template <bool REC>
 __global__ void __launch_bounds__(kThreads) obgpu_project_pipe_kernel(const __grid_constant__ ScanParams p) {
-  constexpr uint32_t kEnt = kProjEnt<REC>, kSrc = REC ? (uint32_t)sizeof(StageRec) : (uint32_t)sizeof(ColDesc);
-  constexpr int kSrcPieces = (int)(kSrc / 16u);
+  constexpr uint32_t kEnt = kProjEnt<REC>;
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  const int nwarps_total = (int)gridDim.x * kWarps;
-  int blk = (int)blockIdx.x * kWarps + warp;
-  if (blk >= p.n_blocks) return;
   uint8_t *wr = g_smem + (uint32_t)warp * p.pp_bytes;
-  uint8_t *meta0 = wr + p.pp_meta, *reg0 = wr + p.pp_region;
   uint16_t *sel = reinterpret_cast<uint16_t *>(wr + p.pp_sel);
   uint8_t *wscr = wr + p.pp_wscr;
-  uint64_t *bars = reinterpret_cast<uint64_t *>(wr + p.pp_bar);   // one mbarrier per region slot
-  if (lane == 0) {
-    mbar_init(bars, 1);
-    mbar_init(bars + 1, 1);
-    fence_barrier_init();
-  }
-  __syncwarp();
   const int np = p.n_proj;
   const uint32_t hdr_bytes = p.pp_hdr_bytes, bm_bytes = p.pp_bm_bytes;
   const Team t = warp_team(lane);
 
-  auto issue_meta = [&](int b, int slot) {
+  uint8_t *meta0 = wr + p.pp_meta, *reg0 = wr + p.pp_region;
+  uint64_t *bars = reinterpret_cast<uint64_t *>(wr + p.pp_bar);
+  auto meta = [&](int b, int ms) {
     if (b >= p.n_blocks) return;
-    const uint32_t sa = smem_u32(meta0 + (uint32_t)slot * p.pp_meta_bytes);
-    const uint8_t *rec = reinterpret_cast<const uint8_t *>(p.recs + b);
-    const uint8_t *ents = REC ? reinterpret_cast<const uint8_t *>(p.stage + (int64_t)b * p.max_cols)
-                              : reinterpret_cast<const uint8_t *>(p.plans + (int64_t)b * p.max_cols);
-    constexpr int kHead = kRecPieces + 2;   // the record, then the two sel_offset entries
-    for (int q = lane; q < kHead + np * kSrcPieces; q += 32) {
-      if (q < kRecPieces) cp_async16(sa + (uint32_t)q * 16u, rec + q * 16);
-      else if (q < kHead) cp_async8(sa + kMetaSel + (uint32_t)(q - kRecPieces) * 8u, p.sel_offset + b + (q - kRecPieces));
-      else {
-        const int i = (q - kHead) / kSrcPieces, piece = (q - kHead) % kSrcPieces;
-        cp_async16(sa + kMetaPlans + (uint32_t)i * kEnt + (uint32_t)piece * 16u,
-                   ents + (size_t)p.used_col[p.proj_used[i]] * kSrc + piece * 16);
-      }
-    }
+    uint8_t *m = meta0 + (uint32_t)ms * p.pp_meta_bytes;
+    issue_meta<REC, true, kEnt>(p, b, smem_u32(m), np, [&](int i) { return p.used_col[p.proj_used[i]]; }, lane);
   };
   // what a block needs beyond its meta: nothing (no selected row / overflow / corrupt), or bitmap words + column ranges
-  auto issue_regions = [&](int b, int mslot, int rslot) {
+  auto regions = [&](int b, int ms, int rsl) {
     if (b >= p.n_blocks) return;
-    const uint8_t *m = meta0 + (uint32_t)mslot * p.pp_meta_bytes;
-    uint8_t *rs = reg0 + (uint32_t)rslot * p.pp_region_bytes;
+    const uint8_t *m = meta0 + (uint32_t)ms * p.pp_meta_bytes;
+    uint8_t *rs = reg0 + (uint32_t)rsl * p.pp_region_bytes;
+    uint64_t *bar = bars + rsl;
     const BlockRec &rec = *reinterpret_cast<const BlockRec *>(m);
     const int64_t base = *reinterpret_cast<const int64_t *>(m + kMetaSel);
     const uint32_t cnt = (uint32_t)(*reinterpret_cast<const int64_t *>(m + kMetaSel + 8u) - base);
     const uint32_t rows = rec.rows;
     if (rows == 0 || cnt == 0 || base + (int64_t)cnt > p.out_cap) {
-      if (lane == 0) mbar_expect_tx(bars + rslot, 0u);   // nothing to stage: the slot's phase still completes
+      if (lane == 0) mbar_expect_tx(bar, 0u);   // nothing to stage: the slot's phase still completes
       return;
     }
     if (cnt != rows) {
@@ -734,22 +723,7 @@ __global__ void __launch_bounds__(kThreads) obgpu_project_pipe_kernel(const __gr
     uint32_t r[4] = {0, 0, 0, 0};
     int nr = 0;
     if (lane < np) {
-      if constexpr (REC) {
-        const StageRec &sr = *reinterpret_cast<const StageRec *>(m + kMetaPlans + (uint32_t)lane * kEnt);
-        r[0] = (uint32_t)sr.lo[0] * 16u;
-        r[1] = (uint32_t)sr.hi[0] * 16u;
-        r[2] = (uint32_t)sr.lo[1] * 16u;
-        r[3] = (uint32_t)sr.hi[1] * 16u;
-        nr = r[3] != r[2] ? 2 : 1;
-      } else {
-        BlockView bv;
-        view_from_rec(rec, nullptr, bv);
-        const ColDesc &d = reinterpret_cast<const ColDesc *>(m + kMetaPlans)[lane];
-        nr = d.ok ? proj_ranges(d, bv, r) : 0;
-      }
-      const uint32_t lim = ((rec.size + 15u) & ~15u) + 32u;
-      if (nr > 0 && ((r[1] - r[0]) + (nr == 2 ? r[3] - r[2] : 0u) > p.pp_span[lane] || r[1] > lim || (nr == 2 && r[3] > lim))) nr = 0;
-      if (nr == 0) r[0] = r[1] = r[2] = r[3] = 0;
+      nr = staged_ranges<REC, false>(rec, m + kMetaPlans + (uint32_t)lane * kEnt, p.pp_span[lane], r);
       const uint32_t o0 = hdr_bytes + bm_bytes + p.pp_off[lane], o1 = o0 + (r[1] - r[0]);
       hdr[2 * lane] = (int32_t)o0 - (int32_t)r[0];
       hdr[2 * lane + 1] = nr == 2 ? (int32_t)o1 - (int32_t)r[2] : (int32_t)o0 - (int32_t)r[0];
@@ -759,7 +733,6 @@ __global__ void __launch_bounds__(kThreads) obgpu_project_pipe_kernel(const __gr
     // one bulk copy (TMA) per byte range, all completing on the slot's mbarrier
     const uint32_t len0 = r[1] - r[0], len1 = nr == 2 ? r[3] - r[2] : 0u;
     const uint32_t total = warp_sum_u32(len0 + len1);
-    uint64_t *bar = bars + rslot;
     if (lane == 0) mbar_expect_tx(bar, total);
     __syncwarp();
     if (lane < np && nr >= 1) {
@@ -770,30 +743,7 @@ __global__ void __launch_bounds__(kThreads) obgpu_project_pipe_kernel(const __gr
     }
   };
 
-  issue_meta(blk, 0);
-  cp_async_commit();
-  cp_async_wait_all();
-  __syncwarp();
-  issue_regions(blk, 0, 0);
-  cp_async_commit();
-  issue_meta(blk + nwarps_total, 1);
-  cp_async_commit();
-  int it = 0;
-  PIPE_CLOCK_START();
-  for (; blk < p.n_blocks; blk += nwarps_total, ++it) {
-    const int ms = it % 3, rsl = it & 1;
-    PIPE_CLOCK_AT(pclk_a);
-    cp_async_wait_all();
-    mbar_wait(bars + rsl, (uint32_t)(it >> 1) & 1u);
-    __syncwarp();
-    PIPE_CLOCK_ADD(pclk_wait, pclk_a);
-    PIPE_CLOCK_AT(pclk_b);
-    issue_regions(blk + nwarps_total, (it + 1) % 3, rsl ^ 1);
-    cp_async_commit();
-    issue_meta(blk + 2 * nwarps_total, (it + 2) % 3);
-    cp_async_commit();
-    PIPE_CLOCK_ADD(pclk_issue, pclk_b);
-
+  auto work = [&](int blk, int ms, int rsl) {
     uint8_t *m = meta0 + (uint32_t)ms * p.pp_meta_bytes;
     uint8_t *rs = reg0 + (uint32_t)rsl * p.pp_region_bytes;
     const BlockRec rec = *reinterpret_cast<const BlockRec *>(m);
@@ -803,8 +753,7 @@ __global__ void __launch_bounds__(kThreads) obgpu_project_pipe_kernel(const __gr
     if (rows == 0 || cnt == 0 || base + (int64_t)cnt > p.out_cap) {
       if (lane == 0 && rows == 0) atomicOr(p.status, ST_CORRUPT);
       if (lane == 0 && rows != 0 && cnt != 0) atomicOr(p.status, ST_OVERFLOW);
-      __syncwarp();
-      continue;
+      return;
     }
     uint8_t *ents = m + kMetaPlans;
     ColDesc *plans = reinterpret_cast<ColDesc *>(ents);
@@ -840,8 +789,7 @@ __global__ void __launch_bounds__(kThreads) obgpu_project_pipe_kernel(const __gr
     if (flatmask != 0u) {
       if (flat) {
         uint8_t *ent = ents + (uint32_t)lane * kEnt;
-        if constexpr (REC) flat_fill(p, *reinterpret_cast<const StageRec *>(ent), lane, smem_u32(rs), hdr[2 * lane], hdr[2 * lane + 1], base, blk_addr, ent);
-        else flat_fill(p, *reinterpret_cast<const ColDesc *>(ent), lane, smem_u32(rs), hdr[2 * lane], hdr[2 * lane + 1], base, blk_addr, ent);
+        flat_fill(p, *reinterpret_cast<const MetaEnt<REC> *>(ent), lane, smem_u32(rs), hdr[2 * lane], hdr[2 * lane + 1], base, blk_addr, ent);
         m[__popc(flatmask & ((1u << lane) - 1u))] = (uint8_t)lane;
       }
       __syncwarp();
@@ -856,11 +804,8 @@ __global__ void __launch_bounds__(kThreads) obgpu_project_pipe_kernel(const __gr
       }
       const int32_t d0 = hdr[2 * pc], d1 = hdr[2 * pc + 1];
       if (wdesc->kind == K_DICT && wdesc->sc == 5) {
-        const uint32_t idx_sbit = (smem_u32(rs) + (uint32_t)d0) * 8u, ref_sbit = (smem_u32(rs) + (uint32_t)d1) * 8u;
-        // which delta belongs to the refs: with two ranges they are ordered by block offset (proj_ranges)
-        uint32_t rbit = ref_sbit, ibit = idx_sbit;
-        if (d0 == d1) rbit = ibit = idx_sbit;
-        else if ((wdesc->val_bit >> 3) < wdesc->dict_payload) { rbit = idx_sbit; ibit = ref_sbit; }
+        uint32_t rbit, ibit;
+        str_dict_bits(*wdesc, smem_u32(rs), d0, d1, rbit, ibit);
         if (all_rows) project_str_dict_shallow<true>(p, *wdesc, pc, sel, cnt, base, blk_addr, rbit, ibit, lane);
         else project_str_dict_shallow<false>(p, *wdesc, pc, sel, cnt, base, blk_addr, rbit, ibit, lane);
         __syncwarp();
@@ -871,8 +816,7 @@ __global__ void __launch_bounds__(kThreads) obgpu_project_pipe_kernel(const __gr
       project_column_staged(p, c, wdesc, pc, sel, cnt, base, blk_addr, all_rows, rows, wscr, t);
       __syncwarp();
     }
-    __syncwarp();
-  }
-  PIPE_CLOCK_STOP(1);
-  cp_async_wait_all();
+  };
+
+  warp_pipeline<1>(p.n_blocks, bars, lane, meta, regions, work);
 }
