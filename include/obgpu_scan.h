@@ -85,11 +85,13 @@ enum {
 
 /* ---- common::ObCompressorType values the path accepts (lib/compress/ob_compress_util.h) ------
  * LZ4 ("lz4_1.0") and LZ4_1_9_1 ("lz4_1.9.1") both store the plain LZ4 block format per micro-block payload;
+ * ZLIB ("zlib_1.0", OceanBase's high-ratio option) stores one zlib stream (RFC 1950 around RFC 1951 DEFLATE) per payload;
  * ZSTD_1_3_8 ("zstd_1.3.8", the default table compression of OceanBase 4.x) stores one plain zstd frame (RFC 8878) per
  * payload. ZSTD ("zstd_1.0", 5) is not accepted. */
 enum {
   OBGPU_COMPRESSOR_NONE = 1,
   OBGPU_COMPRESSOR_LZ4 = 2,
+  OBGPU_COMPRESSOR_ZLIB = 4,
   OBGPU_COMPRESSOR_ZSTD_1_3_8 = 6,
   OBGPU_COMPRESSOR_LZ4_1_9_1 = 7
 };
@@ -167,10 +169,10 @@ int obgpu_batch_total_rows(const obgpu_batch *batch, int64_t *total_rows);
  * their micro-blocks re-laid into an aligned image that the returned page batch owns -- what ObMacroBlockReader /
  * ObMicroBlockBareIterator (blocksstable/ob_micro_block_bare_iterator.cpp) do block by block on the CPU. The macro image may be
  * host memory (copied once) or device memory. Macro blocks whose compressor_type_ is OBGPU_COMPRESSOR_LZ4 / LZ4_1_9_1 /
- * ZSTD_1_3_8 are decoded on the device as obgpu_batch_open_compressed does (raw and compressed micro-blocks may be mixed; the
+ * ZLIB / ZSTD_1_3_8 are decoded on the device as obgpu_batch_open_compressed does (raw and compressed micro-blocks may be mixed; the
  * macro blocks of one call that are not NONE must share one compressor, as one SSTable has one, else OBGPU_NOT_SUPPORTED);
  * other compressors and encrypted macro blocks: OBGPU_NOT_SUPPORTED; broken headers, chains, checksums of compressed
- * micro-blocks, LZ4 streams or zstd frames: OBGPU_INVALID_DATA. The macro payload checksum is not re-computed here (the IO layer's job in the reference).
+ * micro-blocks, LZ4 streams, zlib streams or zstd frames: OBGPU_INVALID_DATA. The macro payload checksum is not re-computed here (the IO layer's job in the reference).
  * The batch owns its re-laid image: string pointers of a scan are string_base + offset inside THAT image
  * (obgpu_batch_device_image). */
 int obgpu_batch_open_macro_blocks(obgpu_ctx *ctx, const void *macro_image, int64_t image_size, int64_t macro_block_size,
@@ -179,13 +181,14 @@ int obgpu_batch_open_macro_blocks(obgpu_ctx *ctx, const void *macro_image, int64
  * on the device. Block i is [offsets[i], offsets[i] + sizes[i]) of `image` in STORED form (plain ObMicroBlockHeader, payload
  * of data_zlength_ bytes; any byte offset); compressor_type is the SSTable's (the reference takes it from the SSTable meta).
  * A block with data_zlength_ == data_length_ is stored raw and copied; the others are decoded (OBGPU_COMPRESSOR_LZ4 and
- * LZ4_1_9_1: the plain LZ4 block format; ZSTD_1_3_8: one zstd frame, obgpu_zstd_decompress) after their header checksum and
+ * LZ4_1_9_1: the plain LZ4 block format; ZLIB: one zlib stream, obgpu_zlib_decompress; ZSTD_1_3_8: one zstd frame,
+ * obgpu_zstd_decompress) after their header checksum and
  * payload checksum (crc32c of the stored bytes == data_checksum_) are checked. Every decoded block goes to a 128-byte aligned slot of a new device image that the
  * batch owns; the decoded copy keeps the stored header unchanged. image_on_device: as obgpu_batch_open (a device image must be
  * 16-byte aligned; a host image is copied once).
  *   OBGPU_COMPRESSOR_NONE : every block must have data_zlength_ == data_length_, else OBGPU_INVALID_DATA
  *   other compressors     : OBGPU_NOT_SUPPORTED
- *   a bad header, checksum, LZ4 stream or zstd frame: OBGPU_INVALID_DATA; the ctx stays usable.
+ *   a bad header, checksum, LZ4 stream, zlib stream or zstd frame: OBGPU_INVALID_DATA; the ctx stays usable.
  * String pointers of a scan are string_base + offset inside the batch's image (obgpu_batch_device_image). */
 int obgpu_batch_open_compressed(obgpu_ctx *ctx, const void *image, int64_t image_size, const int64_t *offsets,
                                 const int64_t *sizes, int32_t n_blocks, int32_t image_on_device, int32_t compressor_type,
@@ -207,6 +210,13 @@ int obgpu_lz4_decompress(obgpu_ctx *ctx, const void *d_in, const int64_t *in_off
  * frames, bytes after the first frame, reserved bits and block types (DESIGN 3.14 lists where this is stricter than
  * libzstd). */
 int obgpu_zstd_decompress(obgpu_ctx *ctx, const void *d_in, const int64_t *in_off, const int64_t *in_len, void *d_out,
+                          const int64_t *out_off, const int64_t *out_len, int32_t n, int32_t *status);
+/* ObZlibCompressor::decompress (zlib's uncompress into a buffer of the expected size) for n independent zlib streams
+ * (RFC 1950 / RFC 1951) in device memory, with the contract of obgpu_lz4_decompress: status[i] == 0 when
+ * d_in[in_off[i], + in_len[i]) is exactly one zlib stream, its Adler-32 included, that decodes to exactly out_len[i] bytes.
+ * Refused besides what zlib's inflate refuses: a preset dictionary (FDICT), bytes after the Adler-32, which uncompress
+ * ignores, and a stream or output longer than 0x7fff0000 bytes (DESIGN 3.16). */
+int obgpu_zlib_decompress(obgpu_ctx *ctx, const void *d_in, const int64_t *in_off, const int64_t *in_len, void *d_out,
                           const int64_t *out_off, const int64_t *out_len, int32_t n, int32_t *status);
 
 /* =============================================================================================

@@ -125,7 +125,7 @@ int obgpu_writer_build_macro_blocks(const void *micro_image, const int64_t *offs
                                     int32_t *n_macro, int32_t *first_micro, int32_t first_micro_cap);
 /* The same with the FixedHeader's compressor_type_ (OBGPU_COMPRESSOR_*). The micro-blocks are taken as they are, in stored
  * form (obgpu_writer_compress_blocks): a macro block records the compressor, it does not apply it. With NONE every block must
- * have data_zlength_ == data_length_ (OBGPU_INVALID_ARGUMENT otherwise); LZ4 / LZ4_1_9_1 / ZSTD_1_3_8 record that compressor;
+ * have data_zlength_ == data_length_ (OBGPU_INVALID_ARGUMENT otherwise); LZ4 / LZ4_1_9_1 / ZLIB / ZSTD_1_3_8 record that compressor;
  * other compressors: OBGPU_NOT_SUPPORTED. obgpu_writer_build_macro_blocks is this call with OBGPU_COMPRESSOR_NONE. */
 int obgpu_writer_build_macro_blocks_ex(const void *micro_image, const int64_t *offsets, const int64_t *sizes, int32_t n_blocks,
                                        const obgpu_macro_spec *spec, void *out, int64_t out_cap, int64_t *out_size,
@@ -144,8 +144,14 @@ int obgpu_writer_lz4_compress(const void *src, int64_t src_len, void *out, int64
  * literals; sequences in Predefined mode (FSE from the RFC's default distributions); a block that does not shrink is a Raw
  * block. out == NULL: only *out_len (never more than src_len + 3 * (src_len / 128 KiB + 1) + 13). */
 int obgpu_writer_zstd_compress(const void *src, int64_t src_len, void *out, int64_t out_cap, int64_t *out_len);
+/* One zlib stream (RFC 1950 / RFC 1951; what uncompress and ObZlibCompressor::decompress read): header 78 01, the payload in
+ * segments of >= 32 KiB of input (whole symbols), each one fixed-Huffman block from the LZ4 compressor's greedy matcher
+ * (matches farther than 32 KiB stay literals, longer ones than 258 bytes are split) or, where that does not shrink it, one
+ * stored block; the Adler-32 trailer. out == NULL: only *out_len (never more than src_len + 5 * (src_len / 32 KiB + 1) + 7). */
+int obgpu_writer_zlib_compress(const void *src, int64_t src_len, void *out, int64_t out_cap, int64_t *out_len);
 /* Re-frames n plain micro-blocks (data_zlength_ == data_length_) into stored form with `compressor` (OBGPU_COMPRESSOR_LZ4 /
- * LZ4_1_9_1: an LZ4 block; ZSTD_1_3_8: a zstd frame, obgpu_writer_zstd_compress; NONE copies): the payload is compressed and kept raw when that is not smaller; a compressed block gets
+ * LZ4_1_9_1: an LZ4 block; ZLIB: a zlib stream, obgpu_writer_zlib_compress; ZSTD_1_3_8: a zstd frame,
+ * obgpu_writer_zstd_compress; NONE copies): the payload is compressed and kept raw when that is not smaller; a compressed block gets
  * data_zlength_, data_checksum_ (crc32c of the stored bytes) and a recomputed header checksum. Block i goes to
  * out[out_offsets[i], out_offsets[i] + out_sizes[i]), offsets multiples of align (a power of two; 1: back to back).
  * out_cap >= sum over i of (sizes[i] rounded up to align) always suffices; *out_size = bytes used. */

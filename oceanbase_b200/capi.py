@@ -24,7 +24,7 @@ OBJ_TINYINT, OBJ_SMALLINT, OBJ_MEDIUMINT, OBJ_INT32, OBJ_INT = 1, 2, 3, 4, 5
 OBJ_UTINYINT, OBJ_USMALLINT, OBJ_UMEDIUMINT, OBJ_UINT32, OBJ_UINT64 = 6, 7, 8, 9, 10
 OBJ_DATETIME, OBJ_TIMESTAMP, OBJ_DATE, OBJ_TIME, OBJ_YEAR, OBJ_VARCHAR, OBJ_CHAR = 17, 18, 19, 20, 21, 22, 23
 NODE_WHITE, NODE_AND, NODE_OR = 0, 1, 2
-COMPRESSOR_NONE, COMPRESSOR_LZ4, COMPRESSOR_ZSTD_1_3_8, COMPRESSOR_LZ4_1_9_1 = 1, 2, 6, 7  # common::ObCompressorType
+COMPRESSOR_NONE, COMPRESSOR_LZ4, COMPRESSOR_ZLIB, COMPRESSOR_ZSTD_1_3_8, COMPRESSOR_LZ4_1_9_1 = 1, 2, 4, 6, 7  # common::ObCompressorType
 
 
 def datum_len_of(obj_type: int) -> int:
@@ -156,6 +156,7 @@ def writer_signatures():
         "obgpu_writer_build_macro_blocks_ex": (C.c_int, [vp, vp, vp, i32, P(MacroSpec), vp, i64, P(i64), P(i32), vp, i32, i32]),
         "obgpu_writer_lz4_compress": (C.c_int, [vp, i64, vp, i64, P(i64)]),
         "obgpu_writer_zstd_compress": (C.c_int, [vp, i64, vp, i64, P(i64)]),
+        "obgpu_writer_zlib_compress": (C.c_int, [vp, i64, vp, i64, P(i64)]),
         "obgpu_writer_compress_blocks": (C.c_int, [vp, vp, vp, i32, i32, i64, vp, i64, vp, vp, P(i64)]),
     }
 
@@ -241,6 +242,7 @@ def declared_signatures():
         "obgpu_batch_device_image": (C.c_int, [vp, P(vp), P(i64)]),
         "obgpu_lz4_decompress": (C.c_int, [vp, vp, vp, vp, vp, vp, vp, i32, vp]),
         "obgpu_zstd_decompress": (C.c_int, [vp, vp, vp, vp, vp, vp, vp, i32, vp]),
+        "obgpu_zlib_decompress": (C.c_int, [vp, vp, vp, vp, vp, vp, vp, i32, vp]),
         "obgpu_encode_columns": (C.c_int, [vp, P(EncodeCol), i32, i32, i64, i64, i32, P(vp)]),
         "obgpu_merge_result_encode": (C.c_int, [vp, vp, vp, i32, i32, i64, i32, P(vp)]),
         "obgpu_encode_columns_ex": (C.c_int, [vp, P(EncodeCol), vp, i32, i32, i64, i64, i32, P(vp)]),

@@ -7,7 +7,7 @@
 //             micro_block_data_offset_; the walk must end at micro_block_data_offset_ + micro_block_data_size_ with row_count_ rows
 //   open    : the walk's (offset, stored size) pairs go to open_stored_blocks (stored_blocks.cuh), which copies every raw
 //             micro-block to a 128-byte aligned slot of a new image (obgpu_macro_realign_kernel) and decodes the compressed ones
-//             (compressor_type_ LZ4 / LZ4_1_9_1 / ZSTD_1_3_8) into theirs -- once per cache fill
+//             (compressor_type_ LZ4 / LZ4_1_9_1 / ZLIB / ZSTD_1_3_8) into theirs -- once per cache fill
 // The survey reports each macro block's compressor, and the ones of one open must agree. 16 bytes per micro-block (offset,
 // size) and 4 per macro block come back to the host for obgpu_batch_open's tables; the block bytes never touch the CPU. Other
 // compressors and encrypted blocks are refused.

@@ -139,9 +139,15 @@ enum IntStreamAttr : uint8_t { IS_USE_BASE = 0x1, IS_REPLACE_NULL_VALUE = 0x2, I
 enum IntStreamType : uint8_t { IS_RAW = 1 };   // the other codecs need the CPU transformer (not handled)
 constexpr uint8_t INTEGER_STREAM_META_V2 = 1;
 
-// ObCompressorType values whose micro-blocks the library writes and opens in stored form: NONE, and the payload codecs the
-// device decodes (stored_blocks.cuh)
+// ObCompressorType values whose micro-blocks the library writes (host writer) and opens in stored form: NONE, and the payload
+// codecs the device decodes (stored_blocks.cuh)
 OBF_HD bool stored_compressor(int32_t c) {
+  return c == OBGPU_COMPRESSOR_NONE || c == OBGPU_COMPRESSOR_LZ4 || c == OBGPU_COMPRESSOR_ZLIB || c == OBGPU_COMPRESSOR_ZSTD_1_3_8 ||
+         c == OBGPU_COMPRESSOR_LZ4_1_9_1;
+}
+
+// The subset the device also compresses (obgpu_compress_blocks, stored_compress.cuh): zlib is decoded but not encoded there
+OBF_HD bool device_compressor(int32_t c) {
   return c == OBGPU_COMPRESSOR_NONE || c == OBGPU_COMPRESSOR_LZ4 || c == OBGPU_COMPRESSOR_LZ4_1_9_1 || c == OBGPU_COMPRESSOR_ZSTD_1_3_8;
 }
 

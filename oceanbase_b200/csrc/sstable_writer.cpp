@@ -2608,6 +2608,146 @@ void zstd_compress_frame(const uint8_t *src, int64_t n, std::vector<uint8_t> &o)
   } while (at < n);
 }
 
+// ---- zlib stream (RFC 1950 / RFC 1951): what ObZlibCompressor::compress's output decodes like per micro-block payload --------
+// Header 78 01, then the payload in segments of whole symbols covering >= 32 KiB of input each (the last one shorter), each
+// segment one fixed-Huffman block or, where fixed coding does not shrink it, one stored block; an Adler-32 trailer. Symbols
+// come from greedy_matches: a match farther than 32768 bytes becomes literals, a longer one than 258 bytes pieces of 3..258.
+struct Deflater {
+  std::vector<uint8_t> &o;
+  uint64_t acc = 0;
+  int nb = 0;
+  void put(uint32_t v, int k) {   // k <= 32 bits, LSB first
+    acc |= (uint64_t)v << nb;
+    nb += k;
+    for (; nb >= 8; nb -= 8, acc >>= 8) o.push_back((uint8_t)acc);
+  }
+  void align() {
+    if (nb > 0) o.push_back((uint8_t)acc);
+    acc = 0;
+    nb = 0;
+  }
+  void code(uint32_t c, int len) {   // a Huffman code goes most significant bit first
+    uint32_t r = 0;
+    for (int k = 0; k < len; ++k) r |= ((c >> k) & 1u) << (len - 1 - k);
+    put(r, len);
+  }
+};
+
+struct DeflateTok {   // len 0: literal `v`; else a match of len 3..258 at distance v 1..32768
+  uint16_t len;
+  uint16_t v;
+};
+
+inline int fixed_lit_bits(int s) { return s < 144 ? 8 : s < 256 ? 9 : s < 280 ? 7 : 8; }
+inline void fixed_lit(Deflater &d, int s) {
+  if (s < 144) d.code(0x30u + s, 8);
+  else if (s < 256) d.code(0x190u + (s - 144), 9);
+  else if (s < 280) d.code((uint32_t)(s - 256), 7);
+  else d.code(0xc0u + (s - 280), 8);
+}
+// length 3..258 -> symbol 257..285 and extra bits; distance 1..32768 -> symbol 0..29 and extra bits
+inline void len_code(uint32_t len, int &sym, int &ebits, uint32_t &extra) {
+  if (len == 258) { sym = 285; ebits = 0; extra = 0; return; }
+  if (len < 11) { sym = 257 + (int)len - 3; ebits = 0; extra = 0; return; }
+  int c = 27;
+  while ((((4u + (c & 3)) << ((c >> 2) - 1)) + 3u) > len) --c;
+  sym = 257 + c;
+  ebits = (c >> 2) - 1;
+  extra = len - ((((4u + (c & 3)) << ebits)) + 3u);
+}
+inline void dist_code(uint32_t dist, int &sym, int &ebits, uint32_t &extra) {
+  if (dist < 5) { sym = (int)dist - 1; ebits = 0; extra = 0; return; }
+  int c = 29;
+  while ((((2u + (c & 1)) << ((c >> 1) - 1)) + 1u) > dist) --c;
+  sym = c;
+  ebits = (c >> 1) - 1;
+  extra = dist - (((2u + (c & 1)) << ebits) + 1u);
+}
+
+uint32_t adler32_bytes(const uint8_t *p, int64_t n) {
+  uint32_t a = 1, b = 0;
+  for (int64_t i = 0; i < n; ++i) {
+    a = (a + p[i]) % 65521u;
+    b = (b + a) % 65521u;
+  }
+  return (b << 16) | a;
+}
+
+void zlib_compress_stream(const uint8_t *src, int64_t n, std::vector<uint8_t> &o) {
+  o.clear();
+  o.reserve((size_t)(n + 5 * (n / 32768 + 1) + 8));
+  std::vector<DeflateTok> toks;
+  int64_t anchor = 0;
+  greedy_matches(src, n, [&](int64_t at, int64_t offset, int64_t len) {
+    for (; anchor < at; ++anchor) toks.push_back({0, src[anchor]});
+    if (offset > 32768) return;   // its bytes stay literals: the next match or the tail emits them
+    for (int64_t left = len; left > 0;) {   // pieces of 3..258 bytes
+      const int64_t piece = left <= 258 ? left : (left - 258 < 3 ? left - 3 : 258);
+      toks.push_back({(uint16_t)piece, (uint16_t)offset});
+      left -= piece;
+    }
+    anchor = at + len;
+  });
+  for (; anchor < n; ++anchor) toks.push_back({0, src[anchor]});
+  Deflater d{o};
+  d.put(0x78, 8);
+  d.put(0x01, 8);
+  size_t t = 0;
+  int64_t in_at = 0;
+  do {
+    const size_t t0 = t;
+    const int64_t in0 = in_at;
+    int64_t bits = 3 + 7;   // block header, end of block
+    while (t < toks.size() && in_at - in0 < 32768) {
+      const DeflateTok &k = toks[t++];
+      if (k.len == 0) {
+        bits += fixed_lit_bits(k.v);
+        ++in_at;
+      } else {
+        int s, e, ds, de;
+        uint32_t x;
+        len_code(k.len, s, e, x);
+        dist_code(k.v, ds, de, x);
+        bits += fixed_lit_bits(s) + e + 5 + de;
+        in_at += k.len;
+      }
+    }
+    const bool last = t == toks.size();
+    const int64_t seg = in_at - in0;
+    const int64_t stored_bits = 3 + ((8 - (d.nb + 3) % 8) % 8) + 32 + 8 * seg;
+    if (seg > 0 && stored_bits <= bits) {
+      d.put(last ? 1u : 0u, 1);
+      d.put(0, 2);
+      d.align();
+      d.put((uint32_t)seg, 16);
+      d.put((uint32_t)~seg & 0xffffu, 16);
+      o.insert(o.end(), src + in0, src + in_at);
+    } else {
+      d.put(last ? 1u : 0u, 1);
+      d.put(1, 2);
+      for (size_t j = t0; j < t; ++j) {
+        const DeflateTok &k = toks[j];
+        if (k.len == 0) {
+          fixed_lit(d, k.v);
+          continue;
+        }
+        int s, e, ds, de;
+        uint32_t x, dx;
+        len_code(k.len, s, e, x);
+        dist_code(k.v, ds, de, dx);
+        fixed_lit(d, s);
+        if (e) d.put(x, e);
+        d.code((uint32_t)ds, 5);
+        if (de) d.put(dx, de);
+      }
+      fixed_lit(d, 256);
+    }
+  } while (t < toks.size());
+  d.align();
+  const uint32_t ad = adler32_bytes(src, n);
+  for (int k = 3; k >= 0; --k) o.push_back((uint8_t)(ad >> (8 * k)));
+}
+
 }  // namespace
 
 extern "C" {
@@ -2627,6 +2767,17 @@ int obgpu_writer_zstd_compress(const void *src, int64_t src_len, void *out, int6
   if ((!src && src_len > 0) || src_len < 0 || src_len > 0x7e000000ll || !out_len) return OBGPU_INVALID_ARGUMENT;
   std::vector<uint8_t> o;
   zstd_compress_frame((const uint8_t *)src, src_len, o);
+  *out_len = (int64_t)o.size();
+  if (!out) return OBGPU_SUCCESS;
+  if ((int64_t)o.size() > out_cap) return OBGPU_BUF_NOT_ENOUGH;
+  memcpy(out, o.data(), o.size());
+  return OBGPU_SUCCESS;
+}
+
+int obgpu_writer_zlib_compress(const void *src, int64_t src_len, void *out, int64_t out_cap, int64_t *out_len) {
+  if ((!src && src_len > 0) || src_len < 0 || src_len > 0x7e000000ll || !out_len) return OBGPU_INVALID_ARGUMENT;
+  std::vector<uint8_t> o;
+  zlib_compress_stream((const uint8_t *)src, src_len, o);
   *out_len = (int64_t)o.size();
   if (!out) return OBGPU_SUCCESS;
   if ((int64_t)o.size() > out_cap) return OBGPU_BUF_NOT_ENOUGH;
@@ -2658,6 +2809,7 @@ int obgpu_writer_compress_blocks(const void *image, const int64_t *offsets, cons
     bool keep_raw = compressor == OBGPU_COMPRESSOR_NONE;
     if (!keep_raw) {
       if (compressor == OBGPU_COMPRESSOR_ZSTD_1_3_8) zstd_compress_frame(blk + hs, len, z);
+      else if (compressor == OBGPU_COMPRESSOR_ZLIB) zlib_compress_stream(blk + hs, len, z);
       else lz4_compress_block(blk + hs, len, z);
       keep_raw = (int64_t)z.size() >= len;   // a block that does not shrink is stored raw (data_zlength_ == data_length_)
     }

@@ -10,8 +10,9 @@
 //             header checksum (lane 0) and payload crc32c over the stored bytes (every lane the raw CRC of a contiguous chunk,
 //             shifted into place by a carry-less multiplication with x^(8 * bytes after it), XOR-reduced -- enc::gf2_mulmod /
 //             enc::crc_byte of the device encoder), then the codec's decoder straight into the block's slot in global memory:
-//             lz4d::warp_lz4_decode (lz4_decode.cuh; compressors 2 and 7) or zstdd::decode_frame (zstd_decode.cuh, compressor 6,
-//             one plain zstd frame per payload, with the warp's tables in shared memory). The slot's tail up to 128 bytes is zeroed.
+//             lz4d::warp_lz4_decode (lz4_decode.cuh; compressors 2 and 7), zstdd::decode_frame (zstd_decode.cuh, compressor 6,
+//             one plain zstd frame per payload) or zlibd::decode_stream (zlib_decode.cuh, compressor 4, one zlib stream per
+//             payload), with the warp's tables in shared memory. The slot's tail up to 128 bytes is zeroed.
 //   open    : obgpu_batch_open(image_on_device = 1, header_view = NULL) over the decoded image, which the batch then owns
 // The decoders are the boundary for bytes from outside the program: every read is checked against the stored extent, every
 // write against data_length_. A failed block sets its status; the open returns OBGPU_INVALID_DATA and the ctx stays usable.
@@ -19,6 +20,7 @@
 #include <type_traits>
 
 #include "lz4_decode.cuh"
+#include "zlib_decode.cuh"
 #include "zstd_decode.cuh"
 
 namespace sb {
@@ -132,9 +134,16 @@ struct Zstd {
     return zstdd::decode_frame(in, n_in, out, n_out, *w, lane, 32) == zstdd::kOk ? kStOk : kStBadStream;
   }
 };
+struct Zlib {
+  using Scratch = zlibd::Work;
+  static __device__ __forceinline__ int32_t decode(const uint8_t *in, int64_t n_in, uint8_t *out, int64_t n_out, Scratch *w, int lane) {
+    return zlibd::decode_stream(in, n_in, out, n_out, *w, lane, 32) == zlibd::kOk ? kStOk : kStBadStream;
+  }
+};
 
 // BLOCKS = true : micro-blocks (checksums checked, header copied, payload decoded, slot tail zeroed), tables indexed by block
-// BLOCKS = false: bare payloads in[in_off, + in_len) -> out[out_off, + out_len) (obgpu_lz4_decompress, obgpu_zstd_decompress)
+// BLOCKS = false: bare payloads in[in_off, + in_len) -> out[out_off, + out_len) (obgpu_lz4_decompress, obgpu_zstd_decompress,
+//                 obgpu_zlib_decompress)
 template <class Codec, bool BLOCKS>
 __global__ void __launch_bounds__(kWarps * 32) obgpu_stored_decode_kernel(const uint8_t *in_base, const int64_t *in_off, const int64_t *in_len,
                                                                           uint8_t *out_base, const int64_t *out_off, const int64_t *out_len,
@@ -198,6 +207,10 @@ static const char *launch_decode(obgpu_ctx *ctx, int32_t compressor, bool blocks
     case OBGPU_COMPRESSOR_ZSTD_1_3_8:
       kernel = blocks ? sb::obgpu_stored_decode_kernel<sb::Zstd, true> : sb::obgpu_stored_decode_kernel<sb::Zstd, false>;
       malformed = blocks ? "zstd payload of a micro-block is malformed" : "a zstd frame is malformed";
+      break;
+    case OBGPU_COMPRESSOR_ZLIB:
+      kernel = blocks ? sb::obgpu_stored_decode_kernel<sb::Zlib, true> : sb::obgpu_stored_decode_kernel<sb::Zlib, false>;
+      malformed = blocks ? "zlib payload of a micro-block is malformed" : "a zlib stream is malformed";
       break;
     default:
       return nullptr;
@@ -320,7 +333,7 @@ static int open_stored_blocks(obgpu_ctx *ctx, const uint8_t *d_image, int64_t im
   return ret;
 }
 
-// n independent payloads of one codec in device memory (obgpu_lz4_decompress, obgpu_zstd_decompress)
+// n independent payloads of one codec in device memory (obgpu_lz4_decompress, obgpu_zstd_decompress, obgpu_zlib_decompress)
 static int decompress_streams(obgpu_ctx *ctx, const void *d_in, const int64_t *in_off, const int64_t *in_len, void *d_out, const int64_t *out_off,
                               const int64_t *out_len, int32_t n, int32_t *status, int32_t compressor) {
   if (!ctx || !d_in || !in_off || !in_len || !d_out || !out_off || !out_len || n <= 0 || !status) return OBGPU_INVALID_ARGUMENT;
@@ -405,6 +418,11 @@ int obgpu_lz4_decompress(obgpu_ctx *ctx, const void *d_in, const int64_t *in_off
 int obgpu_zstd_decompress(obgpu_ctx *ctx, const void *d_in, const int64_t *in_off, const int64_t *in_len, void *d_out, const int64_t *out_off,
                           const int64_t *out_len, int32_t n, int32_t *status) {
   return decompress_streams(ctx, d_in, in_off, in_len, d_out, out_off, out_len, n, status, OBGPU_COMPRESSOR_ZSTD_1_3_8);
+}
+
+int obgpu_zlib_decompress(obgpu_ctx *ctx, const void *d_in, const int64_t *in_off, const int64_t *in_len, void *d_out, const int64_t *out_off,
+                          const int64_t *out_len, int32_t n, int32_t *status) {
+  return decompress_streams(ctx, d_in, in_off, in_len, d_out, out_off, out_len, n, status, OBGPU_COMPRESSOR_ZLIB);
 }
 
 }  // extern "C"

@@ -391,7 +391,7 @@ extern "C" int obgpu_compress_blocks(obgpu_ctx *ctx, const void *d_image, const 
   if (!ctx || !d_image || !d_offsets || !d_sizes || n_blocks <= 0 || !out_size || align < 1 || align > 4096 || (align & (align - 1)) != 0 ||
       (d_out && (!d_out_offsets || !d_out_sizes)))
     return OBGPU_INVALID_ARGUMENT;
-  if (!obf::stored_compressor(compressor)) {
+  if (!obf::device_compressor(compressor)) {
     ctx->err = "compressor not handled by the device path";
     return OBGPU_NOT_SUPPORTED;
   }

@@ -155,7 +155,8 @@ class PageBatch:
         """host_view=False: a device-resident image is opened without a host copy of it (table.image may then be
         None; the headers are surveyed on the device).
         compressor (capi.COMPRESSOR_*): the blocks of `table` are in stored form (sstable.compress_table) and are decoded on
-        the device by obgpu_batch_open_compressed into an image the batch owns (device_image()); None: plain blocks."""
+        the device by obgpu_batch_open_compressed into an image the batch owns (device_image()): LZ4 / LZ4_1_9_1 (LZ4
+        blocks), ZLIB (zlib streams) or ZSTD_1_3_8 (zstd frames); None: plain blocks."""
         self.ctx = ctx
         self.table = table
         self._h = C.c_void_p()

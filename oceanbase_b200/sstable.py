@@ -192,6 +192,16 @@ def zstd_compress(data) -> np.ndarray:
     return out[:n.value]
 
 
+def zlib_compress(data) -> np.ndarray:
+    """One zlib stream (RFC 1950: header 78 01, fixed-Huffman or stored blocks, Adler-32) of `data` by the writer's compressor."""
+    src = np.ascontiguousarray(np.frombuffer(bytes(data), dtype=np.uint8) if not isinstance(data, np.ndarray) else data, dtype=np.uint8)
+    n = C.c_int64(0)
+    check(lib.obgpu_writer_zlib_compress(src.ctypes.data, src.size, None, 0, C.byref(n)), "obgpu_writer_zlib_compress(size)")
+    out = np.zeros(max(n.value, 1), dtype=np.uint8)
+    check(lib.obgpu_writer_zlib_compress(src.ctypes.data, src.size, out.ctypes.data, out.size, C.byref(n)), "obgpu_writer_zlib_compress")
+    return out[:n.value]
+
+
 def compress_table(table: TableImage, compressor: int, align: int = 1) -> TableImage:
     """The blocks of `table` in stored form: each payload compressed with `compressor` (capi.COMPRESSOR_*) and kept raw when
     that is not smaller (data_zlength_, data_checksum_ and the header checksum follow). align=1: blocks back to back, at any

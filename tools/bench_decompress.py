@@ -1,4 +1,4 @@
-"""Cost of opening LZ4-compressed (default) or zstd-compressed (--compressor zstd) micro-blocks on the device vs opening the
+"""Cost of opening LZ4-compressed (default), zstd-compressed (--compressor zstd) or zlib-compressed (--compressor zlib) micro-blocks on the device vs opening the
 plain image of the same table.
 
 Table: seeded RAW int64 key + RAW small ints + RAW 9-byte strings, ~1 GB plain (the writer's LZ4 stores it ~1.5x smaller).
@@ -13,7 +13,11 @@ and from libzstd at levels 1 and 3 (libzstd.so.1 through ctypes), obgpu_zstd_dec
 CPU baseline: libzstd's ZSTD_decompressDCtx over the same payloads on --cpu-threads threads (one call per micro-block, what
 the reference does), timed with a host clock.
 
-  python tools/bench_decompress.py [--compressor lz4|zstd] [--rows N] [--reps R] [--cpu-threads T] [--out FILE]
+--compressor zlib (compressor 4, zlib_1.0; default --rows 8M): the same for blocks from the writer's zlib compressor (fixed
+Huffman) and from the system zlib at levels 1 and 6 (Python's zlib module), obgpu_zlib_decompress alone on each, and a CPU
+baseline: libz.so.1's uncompress over the same payloads on --cpu-threads threads, timed with a host clock.
+
+  python tools/bench_decompress.py [--compressor lz4|zstd|zlib] [--rows N] [--reps R] [--cpu-threads T] [--out FILE]
 """
 import argparse
 import ctypes as C
@@ -92,21 +96,17 @@ def reframe_libzstd(table, level):
     return _reframe_with(table, lambda p: zs.compress(p, level))
 
 
-def zstd_main(a):
+def stored_opens(a, compressor, variants, entry, key, cpu_decode, cpu_key):
+    """For the plain table a.table: the plain opens, then per stored variant (name -> TableImage, or None when its library is missing): the host and device
+    opens with `compressor`, the device entry point `entry` (obgpu_*_decompress) over the compressed payloads alone (results
+    under `key`_decompress_ms / `key`_decoded_gbps), and the CPU baseline: cpu_decode() -> fn(dst, dst_len, src, src_len)
+    returning the decoded length, one call per payload on --cpu-threads threads (results under `cpu_key`_ms / _decoded_gbps;
+    cpu_decode None: not measured)."""
     import concurrent.futures as cf
     import torch
     import oceanbase_b200 as ob
-    from oceanbase_b200 import capi
     from oceanbase_b200.capi import lib
-    from oceanbase_b200.sstable import compress_table
-    sys.path.insert(0, os.path.join(ROOT, "tests", "golden"))
-    import make_zstd_golden as golden
-    rows = a.rows or 8_000_000
-    t0 = time.time()
-    table = make_table(rows, a.rpb)
-    variants = {"writer": compress_table(table, capi.COMPRESSOR_ZSTD_1_3_8), "libzstd1": reframe_libzstd(table, 1),
-                "libzstd3": reframe_libzstd(table, 3)}
-    build_s = time.time() - t0
+    table = a.table
     ctx = ob.ScanContext(0, stream=torch.cuda.current_stream().cuda_stream)
     pinned_plain = torch.from_numpy(table.image).pin_memory()
     plain_h = type(table)(pinned_plain.numpy(), table.offsets, table.sizes, table.total_rows, table.n_cols)
@@ -115,18 +115,17 @@ def zstd_main(a):
     res = {"open_host_plain_ms": timed(lambda: ob.PageBatch(ctx, plain_h), a.reps),
            "open_device_plain_ms": timed(lambda: ob.PageBatch(ctx, table, device_image_ptr=dev_plain.data_ptr(), host_view=False,
                                                               image_size=table.image.size), a.reps)}
-    z = golden.libzstd()
     for name, stored in variants.items():
         if stored is None:
-            res[name] = "not measured (libzstd.so.1 not present)"
+            res[name] = "not measured (library not present)"
             continue
         pinned = torch.from_numpy(stored.image).pin_memory()
         st_h = type(stored)(pinned.numpy(), stored.offsets, stored.sizes, stored.total_rows, stored.n_cols)
         dev = pinned.cuda()
         torch.cuda.synchronize()
-        r = {"open_host_ms": timed(lambda: ob.PageBatch(ctx, st_h, compressor=capi.COMPRESSOR_ZSTD_1_3_8), a.reps),
+        r = {"open_host_ms": timed(lambda: ob.PageBatch(ctx, st_h, compressor=compressor), a.reps),
              "open_device_ms": timed(lambda: ob.PageBatch(ctx, stored, device_image_ptr=dev.data_ptr(), image_size=stored.image.size,
-                                                          compressor=capi.COMPRESSOR_ZSTD_1_3_8), a.reps)}
+                                                          compressor=compressor), a.reps)}
         zlen, dlen = stored_sizes(stored)
         comp = zlen < dlen
         idx = np.nonzero(comp)[0]
@@ -140,31 +139,31 @@ def zstd_main(a):
         for rep in range(a.reps + 1):
             e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
             e0.record()
-            code = lib.obgpu_zstd_decompress(ctx._h, C.c_void_p(dev.data_ptr()), in_off.ctypes.data, in_len.ctypes.data,
-                                             C.c_void_p(d_out.data_ptr()), out_off.ctypes.data, out_len.ctypes.data, len(idx), stv.ctypes.data)
+            code = getattr(lib, entry)(ctx._h, C.c_void_p(dev.data_ptr()), in_off.ctypes.data, in_len.ctypes.data,
+                                       C.c_void_p(d_out.data_ptr()), out_off.ctypes.data, out_len.ctypes.data, len(idx), stv.ctypes.data)
             e1.record()
             e1.synchronize()
             assert code == 0 and (stv == 0).all()
             if rep:
                 ks.append(e0.elapsed_time(e1))
-        r["zstd_decompress_ms"] = float(np.median(ks))
-        r["zstd_decoded_gbps"] = float(out_len.sum()) / (r["zstd_decompress_ms"] * 1e-3) / 1e9
+        r[key + "_decompress_ms"] = float(np.median(ks))
+        r[key + "_decoded_gbps"] = float(out_len.sum()) / (r[key + "_decompress_ms"] * 1e-3) / 1e9
         r.update({"compressed_blocks": int(comp.sum()), "stored_bytes": int(stored.image.size),
                   "ratio": float(table.image.size) / float(stored.image.size),
                   "payload_ratio": float(out_len.sum()) / float(max(in_len.sum(), 1))})
-        if z is None:
-            r["cpu_libzstd"] = "not measured (libzstd.so.1 not present)"
-        else:   # CPU baseline: one ZSTD_decompressDCtx per compressed payload, --cpu-threads threads (ctypes drops the GIL)
+        if cpu_decode is None:
+            r[cpu_key] = "not measured (library not present)"
+        else:   # one call per compressed payload, --cpu-threads threads (ctypes drops the GIL)
             img = stored.image
             chunks = np.array_split(np.arange(len(idx)), a.cpu_threads)
             outbuf = np.empty(int(out_len.sum()), dtype=np.uint8)
 
             def work(ks_):
-                d = z.ZSTD_createDCtx()
+                fn = cpu_decode()
                 base = img.ctypes.data
                 for k in ks_:
-                    n = z.ZSTD_decompressDCtx(d, C.c_void_p(outbuf.ctypes.data + int(out_off[k])), int(out_len[k]),
-                                              C.cast(C.c_void_p(base + int(in_off[k])), C.c_char_p), int(in_len[k]))
+                    n = fn(C.c_void_p(outbuf.ctypes.data + int(out_off[k])), int(out_len[k]),
+                           C.cast(C.c_void_p(base + int(in_off[k])), C.c_char_p), int(in_len[k]))
                     assert n == out_len[k]
                 return len(ks_)
             with cf.ThreadPoolExecutor(a.cpu_threads) as ex:
@@ -174,30 +173,78 @@ def zstd_main(a):
                     t1 = time.perf_counter()
                     list(ex.map(work, chunks))
                     cpu.append((time.perf_counter() - t1) * 1e3)
-            r["cpu_libzstd_ms"] = float(np.median(cpu))
-            r["cpu_libzstd_decoded_gbps"] = float(out_len.sum()) / (r["cpu_libzstd_ms"] * 1e-3) / 1e9
+            r[cpu_key + "_ms"] = float(np.median(cpu))
+            r[cpu_key + "_decoded_gbps"] = float(out_len.sum()) / (r[cpu_key + "_ms"] * 1e-3) / 1e9
             r["cpu_threads"] = a.cpu_threads
         res[name] = r
         del dev, pinned
     name, power = card()
-    res.update({"compressor": "zstd_1.3.8", "card": name, "power_limit_and_max_sm_clock": power, "rows": rows, "rows_per_block": a.rpb,
-                "n_blocks": int(table.n_blocks), "plain_bytes": int(table.image.size), "table_build_s": build_s, "reps": a.reps,
-                "libzstd": z.ZSTD_versionString().decode() if z is not None else "not present"})
+    res.update({"card": name, "power_limit_and_max_sm_clock": power, "rows_per_block": a.rpb, "n_blocks": int(table.n_blocks),
+                "plain_bytes": int(table.image.size), "reps": a.reps})
     ctx.close()
+    return res
+
+
+def zstd_main(a):
+    from oceanbase_b200 import capi
+    from oceanbase_b200.sstable import compress_table
+    sys.path.insert(0, os.path.join(ROOT, "tests", "golden"))
+    import make_zstd_golden as golden
+    rows = a.rows or 8_000_000
+    t0 = time.time()
+    a.table = make_table(rows, a.rpb)
+    variants = {"writer": compress_table(a.table, capi.COMPRESSOR_ZSTD_1_3_8), "libzstd1": reframe_libzstd(a.table, 1),
+                "libzstd3": reframe_libzstd(a.table, 3)}
+    build_s = time.time() - t0
+    z = golden.libzstd()
+
+    def cpu_decode():   # ZSTD_decompressDCtx, one DCtx per thread
+        d = z.ZSTD_createDCtx()
+        return lambda dst, n, src, sn: z.ZSTD_decompressDCtx(d, dst, n, src, sn)
+    res = stored_opens(a, capi.COMPRESSOR_ZSTD_1_3_8, variants, "obgpu_zstd_decompress", "zstd", cpu_decode if z else None, "cpu_libzstd")
+    res.update({"compressor": "zstd_1.3.8", "rows": rows, "table_build_s": build_s,
+                "libzstd": z.ZSTD_versionString().decode() if z is not None else "not present"})
+    return res
+
+
+def zlib_main(a):
+    import zlib
+    from oceanbase_b200 import capi
+    from oceanbase_b200.sstable import compress_table
+    sys.path.insert(0, os.path.join(ROOT, "tests"))
+    sys.path.insert(0, os.path.join(ROOT, "tests", "golden"))
+    import make_zlib_golden as golden
+    from test_gpu_lz4_blocks import _reframe_with
+    rows = a.rows or 8_000_000
+    t0 = time.time()
+    a.table = make_table(rows, a.rpb)
+    variants = {"writer": compress_table(a.table, capi.COMPRESSOR_ZLIB),
+                "zlib1": _reframe_with(a.table, lambda p: zlib.compress(p, 1)), "zlib6": _reframe_with(a.table, lambda p: zlib.compress(p, 6))}
+    build_s = time.time() - t0
+    z = golden.libz()
+
+    def cpu_decode():   # libz's uncompress: the decoded length, or -1 when it does not return Z_OK
+        def fn(dst, n, src, sn):
+            dl = C.c_ulong(n)
+            return dl.value if z.uncompress(dst, C.byref(dl), src, sn) == 0 else -1
+        return fn
+    res = stored_opens(a, capi.COMPRESSOR_ZLIB, variants, "obgpu_zlib_decompress", "zlib", cpu_decode if z else None, "cpu_libz")
+    res.update({"compressor": "zlib_1.0", "rows": rows, "table_build_s": build_s,
+                "libz": z.zlibVersion().decode() if z is not None else "not present"})
     return res
 
 
 def main():
     ap = argparse.ArgumentParser()
-    ap.add_argument("--compressor", choices=["lz4", "zstd"], default="lz4")
+    ap.add_argument("--compressor", choices=["lz4", "zstd", "zlib"], default="lz4")
     ap.add_argument("--rows", type=int, default=None)
     ap.add_argument("--rpb", type=int, default=700)
     ap.add_argument("--reps", type=int, default=3)
     ap.add_argument("--cpu-threads", type=int, default=os.cpu_count() or 1)
     ap.add_argument("--out", default=None)
     a = ap.parse_args()
-    if a.compressor == "zstd":
-        line = json.dumps(zstd_main(a))
+    if a.compressor in ("zstd", "zlib"):
+        line = json.dumps(zstd_main(a) if a.compressor == "zstd" else zlib_main(a))
         print(line)
         if a.out:
             with open(a.out, "w") as f:
