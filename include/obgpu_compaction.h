@@ -239,6 +239,26 @@ void obgpu_encoded_free(obgpu_encoded *enc);
 /* Column checksums of plain device columns (no encode). */
 int obgpu_column_checksums(obgpu_ctx *ctx, const obgpu_encode_col *cols, int32_t n_cols, int64_t total_rows, int64_t *host_checksums);
 
+/* Skip-index aggregate rows (ObSkipIndexAggregator: MIN / MAX / NULL_COUNT, what ObDataIndexBlockBuilder stores as the index
+ * row's agg_row_buf_) per micro-block of the device encoder's blocking, built on the device:
+ *   blocksstable/index_block/ob_index_block_aggregator.cpp   ObColMinAggregator / ObColMaxAggregator / ObColNullCountAggregator
+ *   blocksstable/index_block/ob_agg_row_struct.cpp:49-300    ObAggRowWriter (version 3)
+ * Consecutive blocks of rows_per_block rows; row b occupies host_out[host_offsets[b], host_offsets[b + 1]) (n_blocks + 1
+ * offsets), byte for byte obgpu_writer_table_agg_rows over the same rows -- every block gets its row, the blocks the encoder
+ * left to the host writer included. agg_cols index cols (any order, each at most once); the column index stored is that
+ * index. dev_null: 1 NULL, 2 NOP (the column is not aggregated in that block, as the writer does). host_out == NULL: only
+ * *out_size, the bytes of all rows (the writer's size-query idiom). The result is what obgpu_batch_set_agg_rows takes.
+ * OBGPU_INVALID_ARGUMENT: bad pointers, n_agg_cols <= 0, an agg_cols entry out of range or repeated, rows_per_block <= 0;
+ * OBGPU_NOT_SUPPORTED: an aggregated column not of an integer class, or a row above 65535 bytes (ObAggRowHeader::length_);
+ * OBGPU_BUF_NOT_ENOUGH: out_cap below *out_size (nothing written). The argument errors come before any launch. */
+int obgpu_agg_rows(obgpu_ctx *ctx, const obgpu_encode_col *cols, int32_t n_cols, const int32_t *agg_cols, int32_t n_agg_cols,
+                   int64_t total_rows, int64_t rows_per_block, void *host_out, int64_t out_cap, int64_t *host_offsets,
+                   int64_t *out_size);
+/* The same over a merge result: result_cols / obj_types as obgpu_merge_result_encode_ex takes them, agg_cols index result_cols. */
+int obgpu_merge_result_agg_rows(obgpu_merge_result *res, const int32_t *result_cols, const int32_t *obj_types, int32_t n_cols,
+                                const int32_t *agg_cols, int32_t n_agg_cols, int64_t rows_per_block, void *host_out,
+                                int64_t out_cap, int64_t *host_offsets, int64_t *out_size);
+
 #ifdef __cplusplus
 }
 #endif

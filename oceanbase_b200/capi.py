@@ -254,6 +254,8 @@ def declared_signatures():
         "obgpu_encoded_free": (None, [vp]),
         "obgpu_compress_blocks": (C.c_int, [vp, vp, vp, vp, i32, i32, i32, vp, i64, vp, vp, P(i64)]),
         "obgpu_column_checksums": (C.c_int, [vp, P(EncodeCol), i32, i64, vp]),
+        "obgpu_agg_rows": (C.c_int, [vp, P(EncodeCol), i32, vp, i32, i64, i64, vp, i64, vp, P(i64)]),
+        "obgpu_merge_result_agg_rows": (C.c_int, [vp, vp, vp, i32, vp, i32, i64, vp, i64, vp, P(i64)]),
         # include/obgpu_skip_index.h
         "obgpu_batch_set_agg_rows": (C.c_int, [vp, vp, vp]),
         "obgpu_batch_skip_index_filter": (C.c_int, [vp, P(Filter), vp]),

@@ -113,6 +113,20 @@ class MergeResult:
                   "obgpu_merge_result_fetch_strings", self.ctx._h)
         return heap[:need.value], off, nl[:row_count]
 
+    def agg_rows(self, result_cols: Sequence[int], obj_types: Sequence[int], agg_cols: Sequence[int], rows_per_block: int):
+        """Skip-index aggregate rows (MIN / MAX / NULL_COUNT) of the column group result_cols / obj_types (as encode_merge_result
+        takes them) per block of rows_per_block rows, built on the device: (rows uint8, offsets int64 [n_blocks + 1]), the form
+        sstable.table_agg_rows returns. agg_cols index result_cols."""
+        rc = np.ascontiguousarray(result_cols, dtype=np.int32)
+        ot = np.ascontiguousarray(obj_types, dtype=np.int32)
+        ac = np.ascontiguousarray(agg_cols, dtype=np.int32)
+        n_blocks = (self.info().out_rows + rows_per_block - 1) // rows_per_block if rows_per_block > 0 else 0
+
+        def call(out, cap, offs, size):
+            return lib.obgpu_merge_result_agg_rows(self._h, rc.ctypes.data, ot.ctypes.data, len(rc), ac.ctypes.data, len(ac),
+                                                   rows_per_block, out, cap, offs, size)
+        return _fetch_agg_rows(call, n_blocks, "obgpu_merge_result_agg_rows", self.ctx._h)
+
     def set_string_images(self, device_ptrs: Sequence[int], sizes: Sequence[int]):
         arr = (C.c_void_p * max(len(device_ptrs), 1))(*device_ptrs)
         sz = np.ascontiguousarray(sizes, dtype=np.int64)
@@ -402,6 +416,29 @@ def encode_columns(ctx, cols, total_rows: int, rows_per_block: int, rowkey_cnt: 
     check(lib.obgpu_encode_columns_ex(ctx._h, arr, None if enc is None else enc.ctypes.data, len(cols), rowkey_cnt, total_rows,
                                       rows_per_block, align, C.byref(h)), "obgpu_encode_columns_ex", ctx._h)
     return Encoded(ctx, h, len(cols), keep)
+
+
+def _fetch_agg_rows(call, n_blocks: int, what: str, ctx_h):
+    """The size query, then the rows: call(out, cap, offsets, byref(size)) is one obgpu_*agg_rows call."""
+    size = C.c_int64(0)
+    check(call(None, 0, None, C.byref(size)), what + "(size)", ctx_h)
+    out = np.zeros(max(size.value, 1), dtype=np.uint8)
+    offs = np.zeros(n_blocks + 1, dtype=np.int64)
+    check(call(out.ctypes.data, out.size, offs.ctypes.data, C.byref(size)), what, ctx_h)
+    return out[:size.value], offs
+
+
+def agg_rows(ctx, cols, agg_cols: Sequence[int], total_rows: int, rows_per_block: int):
+    """Skip-index aggregate rows (MIN / MAX / NULL_COUNT) per block of rows_per_block rows of device columns, built on the
+    device (obgpu_agg_rows): (rows uint8, offsets int64 [n_blocks + 1]), byte for byte sstable.table_agg_rows over the same
+    rows. cols as encode_columns takes them (NULL bytes: 1 NULL, 2 NOP); agg_cols index cols."""
+    arr = _encode_cols(cols)
+    ac = np.ascontiguousarray(agg_cols, dtype=np.int32)
+    n_blocks = (total_rows + rows_per_block - 1) // rows_per_block if total_rows > 0 and rows_per_block > 0 else 0
+
+    def call(out, cap, offs, size):
+        return lib.obgpu_agg_rows(ctx._h, arr, len(cols), ac.ctypes.data, len(ac), total_rows, rows_per_block, out, cap, offs, size)
+    return _fetch_agg_rows(call, n_blocks, "obgpu_agg_rows", ctx._h)
 
 
 def column_checksums(ctx, cols, total_rows: int) -> np.ndarray:

@@ -1115,16 +1115,17 @@ int obgpu_encode_columns(obgpu_ctx *ctx, const obgpu_encode_col *cols, int32_t n
   return obgpu_encode_columns_ex(ctx, cols, nullptr, n_cols, rowkey_col_cnt, total_rows, rows_per_block, align, out);
 }
 
-int obgpu_merge_result_encode_ex(obgpu_merge_result *res, const int32_t *result_cols, const int32_t *obj_types, const int32_t *encodings,
-                                 int32_t n_cols, int32_t rowkey_col_cnt, int64_t rows_per_block, int32_t align, obgpu_encoded **out) {
-  if (!res || !result_cols || !obj_types || n_cols <= 0 || n_cols > enc::kMaxCols || !out) return OBGPU_INVALID_ARGUMENT;
-  for (int c = 0; encodings && c < n_cols; ++c)
-    if (encodings[c] != OBGPU_ENC_RAW && encodings[c] != OBGPU_ENC_AUTO) return OBGPU_NOT_SUPPORTED;
+}  // extern "C"
+
+// The device columns of a merge result that result_cols names (-1 the rowkey, -2, -3 ...: the following rowkey columns, >= 0 a
+// payload column) with obj_types, and the merged row count: what the encoder and the aggregate rows read of a column group.
+static int merge_result_cols(obgpu_merge_result *res, const int32_t *result_cols, const int32_t *obj_types, int32_t n_cols,
+                             std::vector<obgpu_encode_col> &cols, int64_t &rows) {
   obgpu_merge_info info;
   int rc = obgpu_merge_result_info(res, &info);
   if (rc != OBGPU_SUCCESS) return rc;
   if (info.out_rows <= 0) return OBGPU_INVALID_ARGUMENT;
-  std::vector<obgpu_encode_col> cols((size_t)n_cols);
+  cols.assign((size_t)n_cols, obgpu_encode_col{});
   for (int i = 0; i < n_cols; ++i) {
     obgpu_encode_col &c = cols[(size_t)i];
     c.obj_type = obj_types[i];
@@ -1143,7 +1144,22 @@ int obgpu_merge_result_encode_ex(obgpu_merge_result *res, const int32_t *result_
       c.dev_null = res->out_null[(size_t)k];
     }
   }
-  return obgpu_encode_columns_ex(res->ctx, cols.data(), encodings, n_cols, rowkey_col_cnt, info.out_rows, rows_per_block, align, out);
+  rows = info.out_rows;
+  return OBGPU_SUCCESS;
+}
+
+extern "C" {
+
+int obgpu_merge_result_encode_ex(obgpu_merge_result *res, const int32_t *result_cols, const int32_t *obj_types, const int32_t *encodings,
+                                 int32_t n_cols, int32_t rowkey_col_cnt, int64_t rows_per_block, int32_t align, obgpu_encoded **out) {
+  if (!res || !result_cols || !obj_types || n_cols <= 0 || n_cols > enc::kMaxCols || !out) return OBGPU_INVALID_ARGUMENT;
+  for (int c = 0; encodings && c < n_cols; ++c)
+    if (encodings[c] != OBGPU_ENC_RAW && encodings[c] != OBGPU_ENC_AUTO) return OBGPU_NOT_SUPPORTED;
+  std::vector<obgpu_encode_col> cols;
+  int64_t rows = 0;
+  const int rc = merge_result_cols(res, result_cols, obj_types, n_cols, cols, rows);
+  if (rc != OBGPU_SUCCESS) return rc;
+  return obgpu_encode_columns_ex(res->ctx, cols.data(), encodings, n_cols, rowkey_col_cnt, rows, rows_per_block, align, out);
 }
 
 int obgpu_merge_result_encode(obgpu_merge_result *res, const int32_t *result_cols, const int32_t *obj_types, int32_t n_cols,

@@ -33,6 +33,7 @@
 #include "../../include/obgpu_scan.h"
 #include "../../include/obgpu_skip_index.h"
 #include "ob_format.h"
+#include "ob_agg_row_format.h"
 #include "scan_device.cuh"
 
 using namespace obdev;
@@ -3247,6 +3248,7 @@ int obgpu_project_datums(obgpu_batch *batch, int32_t block, int32_t col, const i
 #include "encode_kernels.cuh"   // phase B: merged columns -> SSTable bytes + column checksums
 #include "stored_blocks.cuh"    // stored (raw, LZ4- or zstd-compressed) micro-blocks -> page batch, decoded on the device
 #include "stored_compress.cuh"  // plain micro-blocks -> stored (LZ4- or zstd-compressed) form, compressed on the device
+#include "agg_rows.cuh"         // skip-index aggregate rows of the encoder's blocking, built on the device
 #include "macro_blocks.cuh"     // macro blocks (disk format) -> page batch, parsed on the device
 
 // ---- host-buffer scan pipeline (include/obgpu_pipeline.h) ------------------------------------------------

@@ -25,6 +25,7 @@
 #include <vector>
 
 #include "../../include/obgpu_writer.h"
+#include "ob_agg_row_format.h"
 #include "ob_compress_format.h"
 #include "ob_format.h"
 #include "stream_codecs_host.h"
@@ -2091,15 +2092,14 @@ int write_agg_row(std::vector<AggCellIn> cells, int version, std::vector<uint8_t
 
 // MIN / MAX / NULL_COUNT of one column over a row range (ObColMinAggregator / ObColMaxAggregator /
 // ObColNullCountAggregator, ob_index_block_aggregator.cpp): a NOP cell makes the column "not aggregated";
-// integer classes compare on the datum image, strings bytewise (binary collation), a string longer than 40 bytes
-// is kept as a 40-byte prefix with the prefix flag.
-void aggregate_column(const obgpu_col_input &in, uint32_t col_idx, int64_t row_begin, int64_t nrows,
-                      std::vector<AggCellIn> &cells) {
+// integer classes compare on the datum image (obagg::image / obagg::key), strings bytewise (binary collation), a string
+// longer than 40 bytes is kept as a 40-byte prefix with the prefix flag. img[0..1] hold the integer min / max images
+// the result points at.
+obagg::AggCol aggregate_column(const obgpu_col_input &in, uint32_t col_idx, int64_t row_begin, int64_t nrows, int64_t img[2]) {
   const int sc = store_class_of((uint8_t)in.obj_type);
   int64_t null_cnt = 0;
   bool any = false, nop = false;
-  AggCellIn mn{col_idx, OBGPU_SK_IDX_MIN, 1, 0, {}}, mx{col_idx, OBGPU_SK_IDX_MAX, 1, 0, {}};
-  AggCellIn nc{col_idx, OBGPU_SK_IDX_NULL_COUNT, 1, 0, {}};
+  obagg::AggCol a{col_idx, -1, -1, nullptr, nullptr, 0, 0, 0, 0};
   if (sc == 5) {
     StrRef lo{nullptr, 0}, hi{nullptr, 0};
     for (int64_t r = row_begin; r < row_begin + nrows; ++r) {
@@ -2111,57 +2111,76 @@ void aggregate_column(const obgpu_col_input &in, uint32_t col_idx, int64_t row_b
     }
     if (any) {
       const int64_t cap = OBGPU_SKIP_INDEX_MAX_COL_LENGTH;
-      mn.is_null = mx.is_null = 0;
-      mn.is_prefix = lo.len > cap;
-      mx.is_prefix = hi.len > cap;
-      mn.data.assign(lo.p, (size_t)std::min(lo.len, cap));
-      mx.data.assign(hi.p, (size_t)std::min(hi.len, cap));
+      a.min = (const uint8_t *)lo.p;
+      a.max = (const uint8_t *)hi.p;
+      a.min_len = (int32_t)std::min(lo.len, cap);
+      a.max_len = (int32_t)std::min(hi.len, cap);
+      a.min_prefix = lo.len > cap;
+      a.max_prefix = hi.len > cap;
     }
   } else {
     const int dl = datum_len_of((uint8_t)in.obj_type);
-    auto image = [&](int64_t v) -> int64_t {  // compare image of the datum: low dl bytes, sign-extended for signed classes
-      if (dl == 4) return sc == 1 ? (int64_t)(int32_t)(uint32_t)v : (int64_t)(uint32_t)v;
-      if (dl == 1) return (int64_t)(uint8_t)v;
-      return v;
-    };
-    auto less = [&](int64_t a, int64_t b) { return (sc == 1 || dl < 8) ? a < b : (uint64_t)a < (uint64_t)b; };
+    const bool uns = obagg::unsigned_order(sc, dl);
     int64_t lo = 0, hi = 0;
     for (int64_t r = row_begin; r < row_begin + nrows; ++r) {
       if (in.is_null && in.is_null[r]) { nop = nop || in.is_null[r] == 2; ++null_cnt; continue; }
-      const int64_t v = image(in.i64[r]);
-      if (!any || less(v, lo)) lo = v;
-      if (!any || less(hi, v)) hi = v;
+      const int64_t v = obagg::key(obagg::image(in.i64[r], sc, dl), uns);
+      if (!any || v < lo) lo = v;
+      if (!any || hi < v) hi = v;
       any = true;
     }
     if (any) {
-      mn.is_null = mx.is_null = 0;
-      mn.data.assign((const char *)&lo, (size_t)dl);
-      mx.data.assign((const char *)&hi, (size_t)dl);
+      img[0] = obagg::key(lo, uns);   // key() is its own inverse
+      img[1] = obagg::key(hi, uns);
+      a.min = (const uint8_t *)&img[0];
+      a.max = (const uint8_t *)&img[1];
+      a.min_len = a.max_len = dl;
     }
   }
-  if (!nop) {
-    nc.is_null = 0;
-    nc.data.assign((const char *)&null_cnt, 8);
+  if (nop) {
+    a.min_len = a.max_len = -1;
   } else {
-    mn.is_null = mx.is_null = 1;
+    a.has_null_count = 1;
+    a.null_count = null_cnt;
   }
-  cells.push_back(mn);
-  cells.push_back(mx);
-  cells.push_back(nc);
+  return a;
 }
 
 int block_agg_row(const obgpu_col_input *cols, int32_t n_cols, const int32_t *agg_cols, int32_t n_agg_cols,
                   int64_t row_begin, int64_t nrows, std::vector<uint8_t> &out) {
-  std::vector<AggCellIn> cells;
+  std::vector<obagg::AggCol> aggs((size_t)n_agg_cols);
+  std::vector<int64_t> images(2 * (size_t)n_agg_cols);
   for (int32_t k = 0; k < n_agg_cols; ++k) {
     const int32_t c = agg_cols[k];
     if (c < 0 || c >= n_cols) return OBGPU_INVALID_ARGUMENT;
     const int sc = store_class_of((uint8_t)cols[c].obj_type);
     if (sc == 5 ? (!cols[c].str_off || !cols[c].str_heap) : !cols[c].i64) return OBGPU_INVALID_ARGUMENT;
     if (sc != 1 && sc != 2 && sc != 5) return OBGPU_NOT_SUPPORTED;
-    aggregate_column(cols[c], (uint32_t)c, row_begin, nrows, cells);
+    aggs[(size_t)k] = aggregate_column(cols[c], (uint32_t)c, row_begin, nrows, &images[2 * (size_t)k]);
   }
-  return write_agg_row(std::move(cells), 3, out);
+  std::vector<int32_t> order((size_t)n_agg_cols);
+  for (int32_t k = 0; k < n_agg_cols; ++k) order[(size_t)k] = k;
+  std::stable_sort(order.begin(), order.end(), [&](int32_t x, int32_t y) { return aggs[(size_t)x].col_idx < aggs[(size_t)y].col_idx; });
+  if (aggs[(size_t)order.back()].col_idx >= (1u << 24)) return OBGPU_INVALID_ARGUMENT;
+  bool repeats = false;
+  for (size_t k = 1; k < order.size(); ++k) repeats = repeats || aggs[(size_t)order[k]].col_idx == aggs[(size_t)order[k - 1]].col_idx;
+  if (repeats) {   // a column named twice: its cells merge into one cell of six aggregates, which only the general path writes
+    std::vector<AggCellIn> cells;
+    for (const obagg::AggCol &a : aggs) {
+      const bool mm = a.min_len >= 0;
+      cells.push_back({a.col_idx, OBGPU_SK_IDX_MIN, !mm, a.min_prefix, mm ? std::string((const char *)a.min, (size_t)a.min_len) : ""});
+      cells.push_back({a.col_idx, OBGPU_SK_IDX_MAX, !mm, a.max_prefix, mm ? std::string((const char *)a.max, (size_t)a.max_len) : ""});
+      cells.push_back({a.col_idx, OBGPU_SK_IDX_NULL_COUNT, !a.has_null_count, 0,
+                       a.has_null_count ? std::string((const char *)&a.null_count, 8) : ""});
+    }
+    return write_agg_row(std::move(cells), obagg::kVersion, out);
+  }
+  auto col_at = [&](int k) -> const obagg::AggCol & { return aggs[(size_t)order[(size_t)k]]; };
+  obagg::Layout l;
+  if (obagg::layout(n_agg_cols, col_at, l) < 0) return OBGPU_NOT_SUPPORTED;
+  out.resize((size_t)l.size);
+  obagg::write(n_agg_cols, col_at, l, out.data());
+  return OBGPU_SUCCESS;
 }
 
 }  // namespace

@@ -146,6 +146,23 @@ static int fetch_compressed(obgpu_ctx *ctx, obgpu_encoded *enc, int32_t n_blocks
   return ret;
 }
 
+// The group's skip-index aggregate rows, built on the device from the merged stream for every block: the aggregates do not
+// depend on the encoding, so the blocks the host writer encodes get theirs here too.
+static int fetch_agg_rows(obgpu_merge_result *res, const ObGpuColumnGroup &cg, int64_t rows_per_block, int32_t n_blocks,
+                          ObGpuEncodedColumnGroup &o) {
+  const int32_t n = (int32_t)cg.cols_.size(), na = (int32_t)cg.skip_index_cols_.size();
+  int64_t size = 0;
+  int ret = obgpu_merge_result_agg_rows(res, cg.cols_.data(), cg.obj_types_.data(), n, cg.skip_index_cols_.data(), na, rows_per_block,
+                                        nullptr, 0, nullptr, &size);
+  if (OB_SUCCESS == ret) {
+    o.agg_rows_.resize((size_t)size);
+    o.agg_row_offsets_.resize((size_t)n_blocks + 1);
+    ret = obgpu_merge_result_agg_rows(res, cg.cols_.data(), cg.obj_types_.data(), n, cg.skip_index_cols_.data(), na, rows_per_block,
+                                      o.agg_rows_.data(), size, o.agg_row_offsets_.data(), &size);
+  }
+  return ret;
+}
+
 int ObGpuPartitionMajorMerger::write_column_groups(const std::vector<ObGpuColumnGroup> &groups, int64_t rows_per_block, int32_t align,
                                                    std::vector<ObGpuEncodedColumnGroup> &out, int32_t compressor) {
   int ret = OB_SUCCESS;
@@ -184,6 +201,7 @@ int ObGpuPartitionMajorMerger::write_column_groups(const std::vector<ObGpuColumn
       ret = obgpu_encoded_fetch(enc[g], o.image_.data(), info.image_size, o.offsets_.data(), o.sizes_.data(), info.n_blocks);
     }
     if (OB_SUCCESS == ret) ret = obgpu_encoded_column_checksums(enc[g], o.column_checksums_.data());
+    if (OB_SUCCESS == ret && !cg.skip_index_cols_.empty()) ret = fetch_agg_rows(result_, cg, rows_per_block, info.n_blocks, o);
     if (OB_SUCCESS == ret && info.n_host_blocks > 0) {
       // the blocks the device left out (ObRawEncoder stores a NULL-dominated column as var-length cells): their rows come
       // back as rows and go through the host writer with the group's encodings; the image is laid out again with them in place

@@ -57,6 +57,8 @@ struct ObGpuColumnGroup {
   std::vector<int32_t> obj_types_;   // OBGPU_OBJ_* of every column (integer classes)
   int32_t rowkey_col_cnt_ = 0;       // > 0 for the group that carries the rowkey (all-column / rowkey group)
   std::vector<int32_t> encodings_;   // OBGPU_ENC_RAW / OBGPU_ENC_AUTO of every column; empty: every column RAW
+  // positions in cols_ of the columns the skip index aggregates (ObSkipIndexColMeta, MIN / MAX / NULL_COUNT); empty: no rows
+  std::vector<int32_t> skip_index_cols_;
 };
 
 // What the writer of one column group produced: the micro-blocks of its SSTable + the column checksums of its rows.
@@ -66,6 +68,10 @@ struct ObGpuEncodedColumnGroup {
   std::vector<int64_t> column_checksums_;
   int64_t row_count_ = 0;
   int32_t host_encoded_blocks_ = 0;  // blocks the device left to the host writer (a NULL-dominated column stored as var cells)
+  // the skip-index aggregate row of every block (the index row's agg_row_buf_), built on the device when the group names
+  // skip_index_cols_: block b's row is agg_rows_[agg_row_offsets_[b], agg_row_offsets_[b + 1]); empty otherwise
+  std::vector<uint8_t> agg_rows_;
+  std::vector<int64_t> agg_row_offsets_;
 };
 
 class ObGpuPartitionMajorMerger {
@@ -95,6 +101,8 @@ public:
   // (ObMicroBlockCompressor): the device's blocks compressed on the device (obgpu_compress_blocks) before the fetch, the
   // blocks left to the host writer compressed by obgpu_writer_compress_blocks; byte for byte obgpu_writer_compress_blocks
   // over the plain image. OBGPU_COMPRESSOR_NONE: plain blocks.
+  // A group with skip_index_cols_ also comes back with the aggregate row of every block (obgpu_merge_result_agg_rows), the
+  // blocks left to the host writer included: byte for byte obgpu_writer_table_agg_rows over the group's rows.
   int write_column_groups(const std::vector<ObGpuColumnGroup> &groups, int64_t rows_per_block, int32_t align,
                           std::vector<ObGpuEncodedColumnGroup> &out, int32_t compressor = OBGPU_COMPRESSOR_NONE);
   void reset();
