@@ -31,7 +31,7 @@ typedef struct obgpu_host_agg {
 } obgpu_host_agg;
 
 typedef struct obgpu_host_scan_spec {
-  const void *image;          /* host memory (pinned for full copy overlap), blocks 16-byte aligned */
+  const void *image;          /* host memory (pinned for full copy overlap), blocks 16-byte aligned (compressor_type 0) */
   int64_t image_size;
   const int64_t *offsets;     /* [n_blocks] */
   const int64_t *sizes;       /* [n_blocks] */
@@ -62,6 +62,18 @@ typedef struct obgpu_host_scan_spec {
    * block first. Pays off when the scan references a fraction of the columns; CS blocks with encoded streams and HEX / STRING_DIFF /
    * STRING_PREFIX columns are still read in full once (their restatement at open). */
   int32_t zero_copy;
+  /* 0: plain blocks, 16-byte aligned (as above). OBGPU_COMPRESSOR_NONE / LZ4 / LZ4_1_9_1 / ZLIB / ZSTD_1_3_8: the blocks are in
+   * STORED form (plain ObMicroBlockHeader, payload of data_zlength_ bytes) at any byte offset, as they come from the IO buffers;
+   * every page batch is opened by obgpu_batch_open_compressed (header and payload checksums checked, decoded in HBM). Projected
+   * string columns then need a heap (out_heap): their decoded bytes exist only on the device. Other values and zero_copy with a
+   * compressor: OBGPU_NOT_SUPPORTED before any batch is opened. */
+  int32_t compressor_type;
+  /* optional [n_proj]: string column c's bytes go to out_heap[c]; its out_data slots then hold host pointers into out_heap[c]
+   * (0 for NULL rows) instead of pointers into `image`. Lifts the HEX_PACKING / STRING_DIFF / STRING_PREFIX refusal for that
+   * column. NULL array or NULL entries: pointer mode. */
+  void *const *out_heap;
+  const int64_t *out_heap_cap; /* [n_proj] bytes each heap holds; a heap that overflows: OBGPU_BUF_NOT_ENOUGH */
+  int64_t *out_heap_used;      /* optional [n_proj] out: bytes used (after OBGPU_BUF_NOT_ENOUGH: bytes claimed so far, a lower bound) */
 } obgpu_host_scan_spec;
 
 typedef struct obgpu_host_scan_result {

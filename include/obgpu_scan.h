@@ -449,6 +449,18 @@ int obgpu_batch_column_materialised(const obgpu_batch *batch, int32_t col, int32
  * when it exceeds heap_cap (host_off is valid then: call again with a larger heap). */
 int obgpu_result_fetch_strings(obgpu_result *res, int32_t i, int64_t row_begin, int64_t row_count, void *host_heap,
                                int64_t heap_cap, int64_t *host_off, int64_t *heap_bytes);
+/* Bytes the cells of rows [row_begin, row_begin + row_count) of projected string columns cols[0..n) take: bytes[j] for column
+ * cols[j]. NULL rows take 0. Keeps the per-row offsets on the device with the result for the next call. Three kernel launches and
+ * one synchronisation, whatever n and row_count. */
+int obgpu_result_string_bytes(obgpu_result *res, int32_t n, const int32_t *cols, int64_t row_begin, int64_t row_count,
+                              int64_t *bytes);
+/* The previous call's rows and columns: the bytes of column cols[j] go to host_heap[j] (exactly bytes[j] bytes).
+ * host_ptrs[j][k] is set to the host address of row k's bytes inside host_heap[j], or 0 for a NULL row (an empty string gets
+ * an address). host_ptrs and its entries may be NULL. Another (cols, rows) than the last obgpu_result_string_bytes call:
+ * OBGPU_INVALID_ARGUMENT. One kernel launch (the device writes the host addresses), then one copy of heap bytes and one of
+ * pointers per column. */
+int obgpu_result_fetch_string_heap(obgpu_result *res, int32_t n, const int32_t *cols, int64_t row_begin, int64_t row_count,
+                                   void *const *host_heap, uint64_t *const *host_ptrs);
 /* One block, the rows of row_ids (the reference call shape of a VEC_DISCRETE / VEC_CONTINUOUS decode): same outputs + the
  * ObBitVector NULL image (host_nulls, has_null may be NULL). */
 int obgpu_project_strings(obgpu_batch *batch, int32_t block, int32_t col, const int32_t *row_ids, int64_t row_cap,

@@ -78,7 +78,9 @@ class HostScanSpec(C.Structure):
                 ("agg_rows", C.c_void_p), ("agg_off", C.c_void_p), ("out_data", C.POINTER(C.c_void_p)),
                 ("out_lens", C.POINTER(C.c_void_p)), ("out_nulls", C.POINTER(C.c_void_p)), ("out_cap_rows", C.c_int64),
                 ("out_row_ids", C.c_void_p), ("out_block_begin", C.c_void_p), ("out_block_count", C.c_void_p),
-                ("no_row_output", C.c_int32), ("aggs", C.POINTER(HostAgg)), ("n_aggs", C.c_int32), ("zero_copy", C.c_int32)]
+                ("no_row_output", C.c_int32), ("aggs", C.POINTER(HostAgg)), ("n_aggs", C.c_int32), ("zero_copy", C.c_int32),
+                ("compressor_type", C.c_int32), ("out_heap", C.POINTER(C.c_void_p)), ("out_heap_cap", C.c_void_p),
+                ("out_heap_used", C.c_void_p)]
 
 
 class HostScanResult(C.Structure):
@@ -215,6 +217,8 @@ def declared_signatures():
         "obgpu_batch_column_materialised": (C.c_int, [vp, i32, P(i32)]),
         "obgpu_result_fetch_strings": (C.c_int, [vp, i32, i64, i64, vp, i64, vp, P(i64)]),
         "obgpu_project_strings": (C.c_int, [vp, i32, i32, vp, i64, vp, i64, vp, vp, P(i32), P(i64)]),
+        "obgpu_result_string_bytes": (C.c_int, [vp, i32, vp, i64, i64, vp]),
+        "obgpu_result_fetch_string_heap": (C.c_int, [vp, i32, vp, i64, i64, vp, vp]),
         "obgpu_batch_column_type": (C.c_int, [vp, i32, P(i32), P(i32)]),
         "obgpu_block_distinct_count": (C.c_int, [vp, i32, i32, P(i64)]),
         "obgpu_block_read_distinct": (C.c_int, [vp, i32, i32, u64, vp, vp, i64, P(i64)]),

@@ -3,6 +3,7 @@
 // public C-ABI of this library. No CUDA calls of its own.
 #pragma once
 #include <atomic>
+#include <memory>
 #include <mutex>
 #include <thread>
 
@@ -35,6 +36,12 @@ inline int32_t default_bpb(const obgpu_host_scan_spec *s) { return s->blocks_per
 
 // rows of a block without touching the device: the micro header's row_count_ (ob_micro_block_header.h:97-153)
 inline int64_t header_rows(const uint8_t *blk) { uint32_t r; memcpy(&r, blk + 16, 4); return r; }
+
+// compressor_type of a spec: 0 (plain blocks) or one obgpu_batch_open_compressed decodes
+inline bool compressor_ok(int32_t c) {
+  return c == 0 || c == OBGPU_COMPRESSOR_NONE || c == OBGPU_COMPRESSOR_LZ4 || c == OBGPU_COMPRESSOR_ZLIB || c == OBGPU_COMPRESSOR_ZSTD_1_3_8 ||
+         c == OBGPU_COMPRESSOR_LZ4_1_9_1;
+}
 
 inline void add128(int64_t acc[2], int64_t lo, int64_t hi) {
   const uint64_t nlo = (uint64_t)acc[0] + (uint64_t)lo;
@@ -94,6 +101,18 @@ int obgpu_pipeline_scan(obgpu_pipeline *p, const obgpu_host_scan_spec *s, obgpu_
   if (!p || !s || !res || s->n_blocks <= 0 || !s->image || !s->offsets || !s->sizes || s->n_proj < 0 || s->n_aggs < 0 || s->n_aggs > 16)
     return OBGPU_INVALID_ARGUMENT;
   if (!s->no_row_output && s->n_proj > 0 && (!s->out_data || !s->out_nulls)) return OBGPU_INVALID_ARGUMENT;
+  if (!obpipe::compressor_ok(s->compressor_type)) {
+    p->err = "compressor_type " + std::to_string(s->compressor_type) + " is not decoded on the device";
+    return OBGPU_NOT_SUPPORTED;
+  }
+  if (s->compressor_type && s->zero_copy) {
+    p->err = "zero_copy with a compressor: the decoder reads every stored byte";
+    return OBGPU_NOT_SUPPORTED;
+  }
+  const bool heaps = s->out_heap && !s->no_row_output;
+  if (heaps)
+    for (int32_t c = 0; c < s->n_proj; ++c)
+      if (s->out_heap[c] && !s->out_heap_cap) return OBGPU_INVALID_ARGUMENT;
   std::vector<int32_t> bounds;
   obpipe::batch_bounds(s->n_blocks, obpipe::default_bpb(s), std::max(0, s->ramp), bounds);
   const int32_t nb = (int32_t)bounds.size() - 1;
@@ -127,6 +146,9 @@ int obgpu_pipeline_scan(obgpu_pipeline *p, const obgpu_host_scan_spec *s, obgpu_
   std::atomic<int64_t> tail{pos};   // spare rows after the planned slices: overflowing batches move there
   std::atomic<int> first_err{OBGPU_SUCCESS};
   std::mutex mu;   // result totals / aggregates / error text
+  // heap columns: every batch claims a slice of each heap, as overflowing batches claim tail rows
+  std::unique_ptr<std::atomic<int64_t>[]> heap_used(new std::atomic<int64_t>[(size_t)std::max(1, s->n_proj)]);
+  for (int32_t c = 0; c < s->n_proj; ++c) heap_used[c] = 0;
   std::vector<int64_t> launches0;
   for (obgpu_ctx *c : p->ctxs) launches0.push_back(obgpu_ctx_launch_count(c));
 
@@ -150,7 +172,10 @@ int obgpu_pipeline_scan(obgpu_pipeline *p, const obgpu_host_scan_spec *s, obgpu_
         if (r) obgpu_result_free(r);
         if (batch) obgpu_batch_close(batch);
       };
-      int ret = s->zero_copy
+      int ret = s->compressor_type
+                    ? obgpu_batch_open_compressed(ctx, (const uint8_t *)s->image + lo, hi - lo, offs.data(), s->sizes + b0, b1 - b0, 0,
+                                                  s->compressor_type, &batch)
+                : s->zero_copy
                     ? obgpu_batch_open(ctx, (const uint8_t *)s->image + lo, hi - lo, offs.data(), s->sizes + b0, b1 - b0, 1,
                                        (const uint8_t *)s->image + lo, &batch)   // the pinned host image IS the device image
                     : obgpu_batch_open(ctx, (const uint8_t *)s->image + lo, hi - lo, offs.data(), s->sizes + b0, b1 - b0, 0, nullptr, &batch);
@@ -159,13 +184,26 @@ int obgpu_pipeline_scan(obgpu_pipeline *p, const obgpu_host_scan_spec *s, obgpu_
         ret = obgpu_batch_set_agg_rows(batch, s->agg_rows, s->agg_off + b0);
         if (ret != OBGPU_SUCCESS) { fail(ret); return; }
       }
+      std::vector<int32_t> heap_cols;   // projected string columns whose bytes go to a heap
       if (!s->no_row_output) {
-        // a string column whose values the device rebuilt (HEX_PACKING / STRING_DIFF / STRING_PREFIX) has no bytes in the caller's
-        // image to point at: such projections go through obgpu_scan + obgpu_result_fetch_strings, not through this entry
+        // a string column whose values the device rebuilt (HEX_PACKING / STRING_DIFF / STRING_PREFIX) or decoded (compressed
+        // blocks) has no bytes in the caller's image to point at: such projections need a heap
         for (int32_t c = 0; c < s->n_proj; ++c) {
-          int32_t rebuilt = 0;
+          int32_t obj_type = 0, datum_len = -1, rebuilt = 0;
+          const bool is_string = obgpu_batch_column_type(batch, s->proj_cols[c], &obj_type, &datum_len) == OBGPU_SUCCESS && datum_len == 0;
+          if (is_string && heaps && s->out_heap[c]) {
+            heap_cols.push_back(c);
+            continue;
+          }
+          if (is_string && s->compressor_type) {
+            ctx->err = "projected column " + std::to_string(c) + " (store index " + std::to_string(s->proj_cols[c]) +
+                       ") is a string column of compressed blocks: give it a heap (out_heap)";
+            fail(OBGPU_NOT_SUPPORTED);
+            return;
+          }
           if (obgpu_batch_column_materialised(batch, s->proj_cols[c], &rebuilt) == OBGPU_SUCCESS && rebuilt) {
-            ctx->err = "projected string column is HEX_PACKING / STRING_DIFF / STRING_PREFIX coded: use obgpu_result_fetch_strings";
+            ctx->err = "projected column " + std::to_string(c) +
+                       " is HEX_PACKING / STRING_DIFF / STRING_PREFIX coded: give it a heap (out_heap) or use obgpu_result_fetch_strings";
             fail(OBGPU_NOT_SUPPORTED);
             return;
           }
@@ -209,6 +247,21 @@ int obgpu_pipeline_scan(obgpu_pipeline *p, const obgpu_host_scan_spec *s, obgpu_
       const int64_t n = info.selected_rows, row0 = res->batch_row_begin[b];
       int64_t d2h = 0;
       if (!s->no_row_output && s->n_proj > 0 && n > 0) {
+        const int32_t nh = (int32_t)heap_cols.size();
+        std::vector<int64_t> hbytes((size_t)nh), hstart((size_t)nh);
+        if (nh > 0) {
+          ret = obgpu_result_string_bytes(r, nh, heap_cols.data(), 0, n, hbytes.data());
+          if (ret != OBGPU_SUCCESS) { fail(ret); return; }
+          for (int32_t j = 0; j < nh; ++j) {
+            const int32_t c = heap_cols[(size_t)j];
+            hstart[(size_t)j] = heap_used[c].fetch_add(hbytes[(size_t)j]);
+            if (hstart[(size_t)j] + hbytes[(size_t)j] > s->out_heap_cap[c]) {
+              ctx->err = "string heap of projected column " + std::to_string(c) + " is too small (out_heap_cap)";
+              fail(OBGPU_BUF_NOT_ENOUGH);
+              return;
+            }
+          }
+        }
         std::vector<int32_t> idx((size_t)s->n_proj);
         std::vector<void *> hd((size_t)s->n_proj), ha((size_t)s->n_proj);
         std::vector<uint64_t *> hn((size_t)s->n_proj);
@@ -221,7 +274,17 @@ int obgpu_pipeline_scan(obgpu_pipeline *p, const obgpu_host_scan_spec *s, obgpu_
           hn[(size_t)c] = s->out_nulls[c] ? s->out_nulls[c] + row0 / 64 : nullptr;
           d2h += n * (col.is_string ? 12 : col.elem_len) + (n + 63) / 64 * 8;
         }
+        std::vector<void *> hh((size_t)nh);
+        std::vector<uint64_t *> hp((size_t)nh);
+        for (int32_t j = 0; j < nh; ++j) {   // heap columns: only lengths and NULL words come back here, the pointers below
+          const int32_t c = heap_cols[(size_t)j];
+          hp[(size_t)j] = (uint64_t *)hd[(size_t)c];
+          hd[(size_t)c] = nullptr;
+          hh[(size_t)j] = (uint8_t *)s->out_heap[c] + hstart[(size_t)j];
+          d2h += hbytes[(size_t)j];
+        }
         ret = obgpu_result_fetch_cols(r, s->n_proj, idx.data(), 0, n, hd.data(), ha.data(), hn.data());
+        if (ret == OBGPU_SUCCESS && nh > 0) ret = obgpu_result_fetch_string_heap(r, nh, heap_cols.data(), 0, n, hh.data(), hp.data());
         if (ret != OBGPU_SUCCESS) { fail(ret); return; }
       }
       if (s->out_row_ids && n > 0) {
@@ -281,6 +344,8 @@ int obgpu_pipeline_scan(obgpu_pipeline *p, const obgpu_host_scan_spec *s, obgpu_
   for (size_t i = 1; i < p->ctxs.size(); ++i) th.emplace_back(worker, p->ctxs[i]);
   worker(p->ctxs[0]);
   for (auto &t : th) t.join();
+  if (s->out_heap_used)
+    for (int32_t c = 0; c < s->n_proj; ++c) s->out_heap_used[c] = heap_used[c].load();
   for (size_t i = 0; i < p->ctxs.size(); ++i) {
     obgpu_ctx_synchronize(p->ctxs[i]);
     res->kernel_launches += obgpu_ctx_launch_count(p->ctxs[i]) - launches0[i];

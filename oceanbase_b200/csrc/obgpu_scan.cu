@@ -1868,6 +1868,13 @@ struct obgpu_result {
   int32_t has_null[kMaxProj] = {0};
   int32_t status = 0;
   uint64_t string_base = 0;   // of the scan spec: where projected string pointers were expressed (obgpu_result_fetch_strings undoes it)
+  // obgpu_result_string_bytes: the columns and rows it sized, its device buffer (source offsets, lengths, byte offsets of every
+  // row; result_strings.cuh) and every column's first byte offset, kept for obgpu_result_fetch_string_heap
+  void *d_str = nullptr;
+  int32_t str_n = 0;
+  int32_t str_cols[kMaxProj] = {0};
+  int64_t str_row_begin = 0, str_rows = 0;
+  int64_t str_col_off[kMaxProj + 1] = {0};
 };
 
 static thread_local std::string g_last_global_err;
@@ -2819,6 +2826,7 @@ void obgpu_result_free(obgpu_result *r) {
   if (!r) return;
   cudaSetDevice(r->ctx->device);
   if (r->arena) cudaFreeAsync(r->arena, r->ctx->stream);
+  if (r->d_str) cudaFreeAsync(r->d_str, r->ctx->stream);
   delete r;
 }
 

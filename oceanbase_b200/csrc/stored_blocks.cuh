@@ -97,13 +97,17 @@ __global__ void __launch_bounds__(kCopyThreads) obgpu_macro_realign_kernel(const
   uint4 *dst = reinterpret_cast<uint4 *>(out + dst_off[blk]);
   const uint32_t sh = (uint32_t)(src & 3) * 8u;
   const uint32_t *w = reinterpret_cast<const uint32_t *>(image + (src & ~3ll));
-  const int64_t w_cap = (image_size - (src & ~3ll)) >> 2;   // whole words readable from w
+  const int64_t avail = image_size - (src & ~3ll);   // bytes readable from w
+  const int64_t w_cap = avail >> 2;                   // whole words readable from w
+  // the image may end inside a word (stored blocks lie at any byte offset): its last 1 - 3 bytes are read one by one
+  uint32_t tail = 0;
+  for (int b = 0; b < (int)(avail & 3); ++b) tail |= (uint32_t)(reinterpret_cast<const uint8_t *>(w + w_cap))[b] << (8 * b);
   for (int64_t j = threadIdx.x; j < slot / 16; j += kCopyThreads) {
     uint32_t v[5];
 #pragma unroll
     for (int k = 0; k < 5; ++k) {
       const int64_t idx = j * 4 + k;
-      v[k] = idx < w_cap ? __ldg(w + idx) : 0u;
+      v[k] = idx < w_cap ? __ldg(w + idx) : (idx == w_cap ? tail : 0u);
     }
     uint32_t o[4];
 #pragma unroll

@@ -328,7 +328,9 @@ int ObGpuSSTableBatchScanner::init(const void *image, int64_t image_size, const 
     {
       obgpu_batch *probe = nullptr;
       const int64_t zero = 0;
-      if ((ret = obgpu_batch_open(rt_.ctx(), (const char *)image + offsets[0], sizes[0], &zero, sizes, 1, 0, nullptr, &probe)) != OBGPU_SUCCESS) return ret;
+      ret = compressor_ ? obgpu_batch_open_compressed(rt_.ctx(), (const char *)image + offsets[0], sizes[0], &zero, sizes, 1, 0, compressor_, &probe)
+                        : obgpu_batch_open(rt_.ctx(), (const char *)image + offsets[0], sizes[0], &zero, sizes, 1, 0, nullptr, &probe);
+      if (ret != OBGPU_SUCCESS) return ret;
       obgpu_scan_spec ps{};
       ps.proj_cols = proj_.data();
       ps.n_proj = (int32_t)proj_.size();
@@ -359,6 +361,25 @@ int ObGpuSSTableBatchScanner::init(const void *image, int64_t image_size, const 
     h_row_ids_.assign((size_t)cap + 16, 0);
     h_block_begin_.assign((size_t)n_blocks, 0);
     std::vector<int64_t> block_count((size_t)n_blocks, 0), row_begin((size_t)nb + 1), rows((size_t)nb + 1);
+    // stored blocks: the decoded string bytes exist only on the device, so every string column gets a heap. The first size is
+    // the blocks' decoded payload (data_length_); rebuilt columns may need more: grow and rescan
+    std::vector<void *> oh(np, nullptr);
+    std::vector<int64_t> heap_cap(np, 0), heap_used(np, 0);
+    h_heap_.assign(np, {});
+    if (compressor_) {
+      int64_t payload = 64;
+      for (int32_t b = 0; b < n_blocks; ++b) {
+        int32_t dl = 0;
+        memcpy(&dl, (const char *)image + offsets[b] + 40, 4);   // ObMicroBlockHeader::data_length_
+        payload += dl;
+      }
+      for (size_t c = 0; c < np; ++c)
+        if (cols_[c].is_string) heap_cap[c] = payload;
+      hs.compressor_type = compressor_;
+      hs.out_heap = oh.data();
+      hs.out_heap_cap = heap_cap.data();
+      hs.out_heap_used = heap_used.data();
+    }
     hs.out_data = od.data();
     hs.out_lens = ol.data();
     hs.out_nulls = on.data();
@@ -370,14 +391,30 @@ int ObGpuSSTableBatchScanner::init(const void *image, int64_t image_size, const 
     hr.batch_row_begin = row_begin.data();
     hr.batch_rows = rows.data();
     hr.n_batches_cap = nb;
-    if ((ret = obgpu_pipeline_scan(pipe_, &hs, &hr)) != OBGPU_SUCCESS) return ret;
+    for (int attempt = 0;; ++attempt) {
+      for (size_t c = 0; c < np; ++c)
+        if (heap_cap[c] > 0) {
+          h_heap_[c].assign((size_t)heap_cap[c], 0);
+          oh[c] = h_heap_[c].data();
+        }
+      ret = obgpu_pipeline_scan(pipe_, &hs, &hr);
+      bool grow = false;
+      for (size_t c = 0; c < np; ++c)
+        if (heap_used[c] > heap_cap[c]) {
+          heap_cap[c] = std::max(2 * heap_cap[c], 2 * heap_used[c]);
+          grow = true;
+        }
+      if (ret != OBGPU_BUF_NOT_ENOUGH || !grow || attempt == 8) break;
+    }
+    if (ret != OBGPU_SUCCESS) return ret;
     selected_ = hr.selected_rows;
     sel_offset_.assign((size_t)n_blocks + 1, 0);
     for (int32_t b = 0; b < n_blocks; ++b) sel_offset_[(size_t)b + 1] = sel_offset_[(size_t)b] + block_count[(size_t)b];
     host_mode_ = true;
     return OB_SUCCESS;
   }
-  ret = obgpu_batch_open(rt_.ctx(), image, image_size, offsets, sizes, n_blocks, 0, nullptr, &batch_);
+  ret = compressor_ ? obgpu_batch_open_compressed(rt_.ctx(), image, image_size, offsets, sizes, n_blocks, 0, compressor_, &batch_)
+                    : obgpu_batch_open(rt_.ctx(), image, image_size, offsets, sizes, n_blocks, 0, nullptr, &batch_);
   if (ret != OBGPU_SUCCESS) return ret;
   if (use_index) {
     if (n_index_infos_ != n_blocks) return OB_INVALID_ARGUMENT;
@@ -533,14 +570,21 @@ int ObGpuSSTableBatchScanner::fetch_window(int32_t block, int64_t row_begin, int
   out.str_lens.assign(np, {});
   out.is_null.assign(np, {});
   std::vector<uint64_t> nulls((size_t)(n + 63) / 64 + 1);
+  std::vector<int32_t> heap_cols;   // stored blocks: string cells come back as bytes in win_heap_
+  std::vector<std::vector<uint64_t>> heap_ptrs;
   for (size_t c = 0; ret == OBGPU_SUCCESS && c < np; ++c) {
     out.is_null[c].assign((size_t)n, 0);
     if (cols_[c].is_string) {
       std::vector<uint64_t> ptrs((size_t)n);
       out.str_lens[c].resize((size_t)n);
-      ret = obgpu_result_fetch_col(result_, (int32_t)c, row_begin, n, ptrs.data(), out.str_lens[c].data(), nulls.data());
+      ret = obgpu_result_fetch_col(result_, (int32_t)c, row_begin, n, compressor_ ? nullptr : ptrs.data(), out.str_lens[c].data(), nulls.data());
       out.str_ptrs[c].resize((size_t)n);
-      for (int64_t i = 0; i < n; ++i) out.str_ptrs[c][(size_t)i] = reinterpret_cast<const char *>((uintptr_t)ptrs[(size_t)i]);
+      if (compressor_) {
+        heap_cols.push_back((int32_t)c);
+        heap_ptrs.push_back(std::move(ptrs));
+      } else {
+        for (int64_t i = 0; i < n; ++i) out.str_ptrs[c][(size_t)i] = reinterpret_cast<const char *>((uintptr_t)ptrs[(size_t)i]);
+      }
     } else {
       const int el = cols_[c].elem_len;
       std::vector<char> raw((size_t)n * el);
@@ -554,6 +598,24 @@ int ObGpuSSTableBatchScanner::fetch_window(int32_t block, int64_t row_begin, int
       }
     }
     for (int64_t i = 0; i < n; ++i) out.is_null[c][(size_t)i] = (nulls[(size_t)i / 64] >> (i % 64)) & 1;
+  }
+  if (ret == OBGPU_SUCCESS && !heap_cols.empty() && n > 0) {
+    const int32_t nh = (int32_t)heap_cols.size();
+    std::vector<int64_t> bytes((size_t)nh);
+    ret = obgpu_result_string_bytes(result_, nh, heap_cols.data(), row_begin, n, bytes.data());
+    std::vector<void *> heaps((size_t)nh);
+    std::vector<uint64_t *> ptrs((size_t)nh);
+    win_heap_.resize(proj_.size());
+    for (int32_t j = 0; ret == OBGPU_SUCCESS && j < nh; ++j) {
+      std::vector<char> &h = win_heap_[(size_t)heap_cols[(size_t)j]];
+      h.resize((size_t)bytes[(size_t)j] + 1);
+      heaps[(size_t)j] = h.data();
+      ptrs[(size_t)j] = heap_ptrs[(size_t)j].data();
+    }
+    if (ret == OBGPU_SUCCESS) ret = obgpu_result_fetch_string_heap(result_, nh, heap_cols.data(), row_begin, n, heaps.data(), ptrs.data());
+    for (int32_t j = 0; ret == OBGPU_SUCCESS && j < nh; ++j)
+      for (int64_t i = 0; i < n; ++i)
+        out.str_ptrs[(size_t)heap_cols[(size_t)j]][(size_t)i] = reinterpret_cast<const char *>((uintptr_t)heap_ptrs[(size_t)j][(size_t)i]);
   }
   return ret;
 }

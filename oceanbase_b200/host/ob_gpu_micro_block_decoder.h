@@ -301,6 +301,10 @@ public:
   // copies, kernels and device->host copies on n_streams streams; get_next_rows then serves every batch from host
   // memory. Call before init. (With index infos attached the single-batch path is used: the verdicts come from it.)
   void set_pipelined(int32_t n_streams, int32_t blocks_per_batch = 0) { pipe_streams_ = n_streams; pipe_bpb_ = blocks_per_batch; }
+  // Stored micro-blocks (ObMacroBlockReader's IO buffers before decompress_data): the blocks handed to init are in stored form
+  // with this common::ObCompressorType (OBGPU_COMPRESSOR_*) and are decoded on the device; 0 (the default): plain blocks. String
+  // cells then come back as bytes in scanner-owned buffers that str_ptrs point into. Call before init.
+  void set_compressor(int32_t compressor_type) { compressor_ = compressor_type; }
   // LIMIT / OFFSET pushed down to the scan (ObTableAccessContext::limit_param_): every batch is trimmed the way
   // ObBlockBatchedRowStore::get_row_ids does (access/ob_block_batched_row_store.cpp:163-186) -- the first `offset`
   // selected rows are dropped, OB_ITER_END follows the batch that reaches `limit` (limit < 0: none).
@@ -337,6 +341,9 @@ private:
   std::vector<std::vector<char>> h_data_;
   std::vector<std::vector<int32_t>> h_lens_;
   std::vector<std::vector<uint64_t>> h_nulls_;
+  std::vector<std::vector<char>> h_heap_;   // pipelined, stored blocks: string bytes per projected column
+  std::vector<std::vector<char>> win_heap_; // single batch, stored blocks: the current window's string bytes per projected column
+  int32_t compressor_ = 0;
   std::vector<int32_t> h_row_ids_;
   std::vector<int64_t> h_block_begin_;   // output row where a block's selected rows start
   ObGpuScanRuntime &rt_;
@@ -366,7 +373,7 @@ struct ObDatumRow {
 // storage::ObIStoreRowIterator / ObStoreRowIterator (access/ob_store_row_iterator.h:34-185) over the page-batch scanner: the
 // row-at-a-time contract the merge layer (ObMultipleMerge) and the compaction iterators pull through --
 // get_next_row(const ObDatumRow *&) until OB_ITER_END, reuse() to rescan, reset() to release. The row handed out stays valid until
-// the next call, string datums point into the scanned image (or the scanner's host buffers in pipelined mode).
+// the next call, string datums point into the scanned image (or the scanner's host buffers in pipelined mode or with stored blocks).
 class ObGpuStoreRowIterator {
 public:
   explicit ObGpuStoreRowIterator(ObGpuScanRuntime &rt) : scanner_(rt) {}
