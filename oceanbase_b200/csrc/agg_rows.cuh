@@ -132,61 +132,53 @@ static int agg_rows_run(obgpu_ctx *ctx, const obgpu_encode_col *cols, int32_t n_
   if (n > 0x7fffffff || n * n_agg > 0x7fffffffll * (agg::kThreads / 32)) return OBGPU_NOT_SUPPORTED;
   cudaSetDevice(ctx->device);
   const int n_chunks = (int)((n + kPrefixChunk - 1) / kPrefixChunk);
-  auto al = [](size_t x) { return (x + 255) & ~(size_t)255; };
-  size_t o = 0;
-  const size_t o_spec = o; o += al((size_t)n_agg * sizeof(agg::ColSpec));
-  const size_t o_rec = o; o += al((size_t)n * n_agg * sizeof(agg::Rec));
-  const size_t o_size = o; o += al((size_t)n * 4);
-  const size_t o_off = o; o += al((size_t)(n + 2) * 8);   // offsets [n + 1], then the status word: one copy reads total + status
-  const size_t o_chunk = o; o += al((size_t)n_chunks * 8);
-  void *arena = nullptr, *d_rows = nullptr;
-  if (cudaMallocAsync(&arena, o, ctx->stream) != cudaSuccess) {
-    ctx->err = "aggregate-row scratch";
-    return OBGPU_ALLOCATE_MEMORY_FAILED;
+  Scratch arena(ctx);
+  const size_t o_spec = arena.take((size_t)n_agg * sizeof(agg::ColSpec));
+  const size_t o_rec = arena.take((size_t)n * n_agg * sizeof(agg::Rec));
+  const size_t o_size = arena.take((size_t)n * 4);
+  const size_t o_off = arena.take((size_t)(n + 2) * 8);   // offsets [n + 1], then the status word: one copy reads total + status
+  const size_t o_chunk = arena.take((size_t)n_chunks * 8);
+  CUDA_TRY(ctx, arena.alloc());
+  agg::ColSpec *d_spec = arena.at<agg::ColSpec>(o_spec);
+  agg::Rec *d_rec = arena.at<agg::Rec>(o_rec);
+  uint32_t *d_size = arena.at<uint32_t>(o_size);
+  int64_t *d_off = arena.at<int64_t>(o_off);
+  unsigned long long *d_status = (unsigned long long *)(d_off + n + 1), *d_chunk = arena.at<unsigned long long>(o_chunk);
+  CUDA_TRY(ctx, cudaMemcpyAsync(d_spec, spec.data(), spec.size() * sizeof(agg::ColSpec), cudaMemcpyHostToDevice, ctx->stream));
+  CUDA_TRY(ctx, cudaMemsetAsync(d_status, 0, 8, ctx->stream));
+  const int64_t warps = n * n_agg;
+  const unsigned grid_blocks = (unsigned)((n + agg::kThreads - 1) / agg::kThreads);
+  agg::obgpu_agg_reduce_kernel<<<(unsigned)((warps + agg::kThreads / 32 - 1) / (agg::kThreads / 32)), agg::kThreads, 0, ctx->stream>>>(
+      d_spec, n_agg, n, total_rows, rows_per_block, d_rec);
+  agg::obgpu_agg_size_kernel<<<grid_blocks, agg::kThreads, 0, ctx->stream>>>(d_spec, d_rec, n_agg, n, total_rows, rows_per_block, d_size,
+                                                                             d_status);
+  obgpu_prefix_local_kernel<<<n_chunks, 256, 0, ctx->stream>>>(d_size, (int)n, d_off, d_chunk);
+  obgpu_prefix_fix_kernel<<<n_chunks + 1, 256, 0, ctx->stream>>>((int)n, n_chunks, d_off, d_chunk);
+  ctx->launches += 4;
+  int64_t *hp = (int64_t *)ctx->h_pinned;
+  CUDA_TRY(ctx, cudaGetLastError());
+  CUDA_TRY(ctx, cudaMemcpyAsync(hp, d_off + n, 16, cudaMemcpyDeviceToHost, ctx->stream));
+  CUDA_TRY(ctx, cudaStreamSynchronize(ctx->stream));
+  const int64_t total = hp[0];
+  if (hp[1] != 0) {
+    ctx->err = "an aggregate row exceeds 65535 bytes";
+    return OBGPU_NOT_SUPPORTED;
   }
-  uint8_t *a = (uint8_t *)arena;
-  agg::ColSpec *d_spec = (agg::ColSpec *)(a + o_spec);
-  agg::Rec *d_rec = (agg::Rec *)(a + o_rec);
-  uint32_t *d_size = (uint32_t *)(a + o_size);
-  int64_t *d_off = (int64_t *)(a + o_off);
-  unsigned long long *d_status = (unsigned long long *)(d_off + n + 1), *d_chunk = (unsigned long long *)(a + o_chunk);
-  int ret = OBGPU_SUCCESS;
-  auto fail = [&](int code, const char *what) { ctx->err = what; ret = code; };
-  do {
-    if (cudaMemcpyAsync(d_spec, spec.data(), spec.size() * sizeof(agg::ColSpec), cudaMemcpyHostToDevice, ctx->stream) != cudaSuccess ||
-        cudaMemsetAsync(d_status, 0, 8, ctx->stream) != cudaSuccess) { fail(OBGPU_ERR_SYS, "aggregate-row set-up"); break; }
-    const int64_t warps = n * n_agg;
-    const unsigned grid_blocks = (unsigned)((n + agg::kThreads - 1) / agg::kThreads);
-    agg::obgpu_agg_reduce_kernel<<<(unsigned)((warps + agg::kThreads / 32 - 1) / (agg::kThreads / 32)), agg::kThreads, 0, ctx->stream>>>(
-        d_spec, n_agg, n, total_rows, rows_per_block, d_rec);
-    agg::obgpu_agg_size_kernel<<<grid_blocks, agg::kThreads, 0, ctx->stream>>>(d_spec, d_rec, n_agg, n, total_rows, rows_per_block, d_size,
-                                                                               d_status);
-    obgpu_prefix_local_kernel<<<n_chunks, 256, 0, ctx->stream>>>(d_size, (int)n, d_off, d_chunk);
-    obgpu_prefix_fix_kernel<<<n_chunks + 1, 256, 0, ctx->stream>>>((int)n, n_chunks, d_off, d_chunk);
-    ctx->launches += 4;
-    int64_t *hp = (int64_t *)ctx->h_pinned;
-    if (cudaGetLastError() != cudaSuccess || cudaMemcpyAsync(hp, d_off + n, 16, cudaMemcpyDeviceToHost, ctx->stream) != cudaSuccess ||
-        cudaStreamSynchronize(ctx->stream) != cudaSuccess) { fail(OBGPU_ERR_SYS, "aggregate-row sizes"); break; }
-    const int64_t total = hp[0];
-    if (hp[1] != 0) { fail(OBGPU_NOT_SUPPORTED, "an aggregate row exceeds 65535 bytes"); break; }
-    *out_size = total;
-    if (!host_out) break;
-    if (out_cap < total) { fail(OBGPU_BUF_NOT_ENOUGH, "output capacity below the aggregate rows' size"); break; }
-    if (cudaMallocAsync(&d_rows, (size_t)std::max<int64_t>(total, 1), ctx->stream) != cudaSuccess) {
-      fail(OBGPU_ALLOCATE_MEMORY_FAILED, "aggregate rows");
-      break;
-    }
-    agg::obgpu_agg_write_kernel<<<grid_blocks, agg::kThreads, 0, ctx->stream>>>(d_spec, d_rec, n_agg, n, total_rows, rows_per_block, d_off,
-                                                                                (uint8_t *)d_rows);
-    ctx->launches++;
-    if (cudaGetLastError() != cudaSuccess ||
-        cudaMemcpyAsync(host_out, d_rows, (size_t)total, cudaMemcpyDeviceToHost, ctx->stream) != cudaSuccess ||
-        cudaMemcpyAsync(host_offsets, d_off, (size_t)(n + 1) * 8, cudaMemcpyDeviceToHost, ctx->stream) != cudaSuccess ||
-        cudaStreamSynchronize(ctx->stream) != cudaSuccess) { fail(OBGPU_ERR_SYS, "aggregate-row write"); break; }
-  } while (0);
-  if (d_rows) cudaFreeAsync(d_rows, ctx->stream);
-  cudaFreeAsync(arena, ctx->stream);
-  return ret;
+  *out_size = total;
+  if (!host_out) return OBGPU_SUCCESS;
+  if (out_cap < total) {
+    ctx->err = "output capacity below the aggregate rows' size";
+    return OBGPU_BUF_NOT_ENOUGH;
+  }
+  Scratch rows(ctx);
+  CUDA_TRY(ctx, rows.alloc((size_t)std::max<int64_t>(total, 1)));
+  agg::obgpu_agg_write_kernel<<<grid_blocks, agg::kThreads, 0, ctx->stream>>>(d_spec, d_rec, n_agg, n, total_rows, rows_per_block, d_off, rows.p);
+  ctx->launches++;
+  CUDA_TRY(ctx, cudaGetLastError());
+  CUDA_TRY(ctx, cudaMemcpyAsync(host_out, rows.p, (size_t)total, cudaMemcpyDeviceToHost, ctx->stream));
+  CUDA_TRY(ctx, cudaMemcpyAsync(host_offsets, d_off, (size_t)(n + 1) * 8, cudaMemcpyDeviceToHost, ctx->stream));
+  CUDA_TRY(ctx, cudaStreamSynchronize(ctx->stream));
+  return OBGPU_SUCCESS;
 }
 
 extern "C" {

@@ -21,26 +21,19 @@ __global__ void __launch_bounds__(256) obgpu_survey_kernel(const uint8_t *image,
   out[2 * i + 1] = f.ncol | (verdict << 16);
 }
 
-// ctx->err = the CUDA error's text; returns the OB code of a failed CUDA call
-static int cuda_failure(obgpu_ctx *ctx, cudaError_t e) {
-  ctx->err = cudaGetErrorString(e);
-  return e == cudaErrorMemoryAllocation ? OBGPU_ALLOCATE_MEMORY_FAILED : OBGPU_ERR_SYS;
-}
-
-// Survey fetch: clears zero_bytes of d_rec, enqueues `launch` (one per-block survey kernel writing d_rec), copies out.size()
-// records of d_rec back into `out`, synchronises once and frees d_rec, whatever failed.
+// Survey fetch: allocates `bytes` of device records and clears the first zero_bytes, enqueues `launch(d_rec)` (one per-block survey
+// kernel writing them), copies out.size() records back into `out` and synchronises once.
 template <class R, class Launch>
-static cudaError_t survey_fetch(obgpu_ctx *ctx, void *d_rec, size_t zero_bytes, std::vector<R> &out, Launch launch) {
-  cudaError_t e = zero_bytes ? cudaMemsetAsync(d_rec, 0, zero_bytes, ctx->stream) : cudaSuccess;
-  if (e == cudaSuccess) {
-    launch();
-    ctx->launches++;
-    e = cudaGetLastError();
-  }
-  if (e == cudaSuccess) e = cudaMemcpyAsync(out.data(), d_rec, out.size() * sizeof(R), cudaMemcpyDeviceToHost, ctx->stream);
-  if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->stream);
-  cudaFreeAsync(d_rec, ctx->stream);
-  return e;
+static int survey_fetch(obgpu_ctx *ctx, size_t bytes, size_t zero_bytes, std::vector<R> &out, Launch launch) {
+  Scratch rec(ctx);
+  CUDA_TRY(ctx, rec.alloc(bytes));
+  if (zero_bytes) CUDA_TRY(ctx, cudaMemsetAsync(rec.p, 0, zero_bytes, ctx->stream));
+  launch(rec.at<uint32_t>(0));
+  ctx->launches++;
+  CUDA_TRY(ctx, cudaGetLastError());
+  CUDA_TRY(ctx, cudaMemcpyAsync(out.data(), rec.p, out.size() * sizeof(R), cudaMemcpyDeviceToHost, ctx->stream));
+  CUDA_TRY(ctx, cudaStreamSynchronize(ctx->stream));
+  return OBGPU_SUCCESS;
 }
 
 // Slot layout of a rewritten image: block i at off[i], in a slot of size[i] bytes rounded up to 128. Returns the image's bytes.
@@ -54,15 +47,14 @@ static uint64_t slot_layout(const Size *size, int32_t n, Off *off) {
   return pos;
 }
 
-// Install: the batch takes d_new, a rewritten image of `bytes` bytes, with block i at off[i] and size[i] bytes long. Enqueues the
-// uploads of the device block tables and frees the image the batch owned before once the stream is past it. The batch owns d_new
-// even when an upload fails.
-static cudaError_t install_image(obgpu_ctx *ctx, obgpu_batch *b, uint8_t *d_new, uint64_t bytes, const uint64_t *off, const uint32_t *size) {
+// Install: the batch takes the allocation of `img`, a rewritten image of `bytes` bytes, with block i at off[i] and size[i] bytes
+// long. Enqueues the uploads of the device block tables and frees the image the batch owned before once the stream is past it.
+static int install_image(obgpu_ctx *ctx, obgpu_batch *b, Scratch &img, uint64_t bytes, const uint64_t *off, const uint32_t *size) {
   const int32_t n = b->n_blocks;
-  cudaError_t e = cudaMemcpyAsync(b->d_blk_off, off, (size_t)n * 8, cudaMemcpyHostToDevice, ctx->stream);
-  if (e == cudaSuccess) e = cudaMemcpyAsync(b->d_blk_size, size, (size_t)n * 4, cudaMemcpyHostToDevice, ctx->stream);
+  CUDA_TRY(ctx, cudaMemcpyAsync(b->d_blk_off, off, (size_t)n * 8, cudaMemcpyHostToDevice, ctx->stream));
+  CUDA_TRY(ctx, cudaMemcpyAsync(b->d_blk_size, size, (size_t)n * 4, cudaMemcpyHostToDevice, ctx->stream));
   if (b->own_image && b->d_image) cudaFreeAsync((void *)b->d_image, ctx->stream);
-  b->d_image = d_new;
+  b->d_image = (const uint8_t *)img.release();
   b->own_image = true;
   b->image_size = (int64_t)bytes;
   b->max_block_bytes = 0;
@@ -71,20 +63,18 @@ static cudaError_t install_image(obgpu_ctx *ctx, obgpu_batch *b, uint8_t *d_new,
     b->sizes[(size_t)i] = size[i];
     b->max_block_bytes = std::max<uint32_t>(b->max_block_bytes, (size[i] + 15u) & ~15u);
   }
-  return e;
+  return OBGPU_SUCCESS;
 }
 
 // CS blocks with non-RAW integer streams -> a RAW restatement of the batch's image (stream_codecs.cuh), in place of
 // the caller's image for every later kernel. Runs on the ctx stream after the image is resident; synchronises.
 static int cs_restate_batch(obgpu_ctx *ctx, obgpu_batch *b) {
   const int32_t n = b->n_blocks;
-  uint32_t *d_sv = nullptr;
   std::vector<uint32_t> sv((size_t)n * 4);
-  CUDA_TRY(ctx, cudaMallocAsync((void **)&d_sv, (size_t)n * 16, ctx->stream));
-  cudaError_t e = survey_fetch(ctx, d_sv, 0, sv, [&] {
+  int ret = survey_fetch(ctx, (size_t)n * 16, 0, sv, [&](uint32_t *d_sv) {
     obcs::cs_survey_kernel<<<(unsigned)((n + 127) / 128), 128, 0, ctx->stream>>>(b->d_image, b->d_blk_off, b->d_blk_size, n, d_sv);
   });
-  if (e != cudaSuccess) { ctx->err = cudaGetErrorString(e); return OBGPU_ERR_SYS; }
+  if (ret != OBGPU_SUCCESS) return ret;
   bool any = false;
   for (int32_t i = 0; i < n; ++i) {
     const uint32_t flags = sv[(size_t)4 * i + 2];
@@ -106,40 +96,33 @@ static int cs_restate_batch(obgpu_ctx *ctx, obgpu_batch *b) {
     scr += 4ull * sv[(size_t)4 * i + 3];
   }
   const uint64_t pos = slot_layout(nsz.data(), n, tab.data());
-  uint8_t *d_new = nullptr, *d_scr = nullptr;
-  uint64_t *d_tab = nullptr;
-  uint32_t *d_nsz = nullptr;
-  obcs::StreamJob *d_jobs = nullptr;
-  int *d_status = nullptr;
-  e = cudaMallocAsync((void **)&d_new, (size_t)pos + 64, ctx->stream);
-  if (e == cudaSuccess) e = cudaMallocAsync((void **)&d_scr, (size_t)scr + 16, ctx->stream);
-  if (e == cudaSuccess) e = cudaMallocAsync((void **)&d_tab, (size_t)n * 24, ctx->stream);
-  if (e == cudaSuccess) e = cudaMallocAsync((void **)&d_nsz, (size_t)n * 4, ctx->stream);
-  if (e == cudaSuccess) e = cudaMallocAsync((void **)&d_jobs, (size_t)(jobs + 1) * sizeof(obcs::StreamJob), ctx->stream);
-  if (e == cudaSuccess) e = cudaMallocAsync((void **)&d_status, 16, ctx->stream);
-  if (e == cudaSuccess) e = cudaMallocAsync((void **)&b->d_xf, (size_t)n * sizeof(obcs::XformRec), ctx->stream);
-  if (e == cudaSuccess) e = cudaMemsetAsync(d_status, 0, 16, ctx->stream);
-  if (e == cudaSuccess) e = cudaMemsetAsync(d_new, 0, (size_t)pos + 64, ctx->stream);   // block padding and tail slack read as zero
-  if (e == cudaSuccess) e = cudaMemcpyAsync(d_tab, tab.data(), (size_t)n * 24, cudaMemcpyHostToDevice, ctx->stream);
-  if (e == cudaSuccess) e = cudaMemcpyAsync(d_nsz, nsz.data(), (size_t)n * 4, cudaMemcpyHostToDevice, ctx->stream);
-  if (e == cudaSuccess) {
-    obcs::cs_rewrite_kernel<<<(unsigned)((n + 127) / 128), 128, 0, ctx->stream>>>(b->d_image, b->d_blk_off, b->d_blk_size, n, d_new, d_tab, d_nsz,
-                                                                              d_tab + n, d_jobs, d_scr, d_tab + 2 * (size_t)n, b->d_xf, d_status);
-    if (jobs > 0)
-      obcs::cs_decode_kernel<<<(unsigned)((jobs + 127) / 128), 128, 0, ctx->stream>>>(b->d_image, d_new, d_jobs, (int64_t)jobs, d_status);
-    ctx->launches += jobs > 0 ? 2 : 1;
-    e = cudaGetLastError();
-  }
+  Scratch img(ctx), scratch(ctx), tabs(ctx), sizes(ctx), job_list(ctx), status(ctx);
+  CUDA_TRY(ctx, img.alloc((size_t)pos + 64));
+  CUDA_TRY(ctx, scratch.alloc((size_t)scr + 16));
+  CUDA_TRY(ctx, tabs.alloc((size_t)n * 24));
+  CUDA_TRY(ctx, sizes.alloc((size_t)n * 4));
+  CUDA_TRY(ctx, job_list.alloc((size_t)(jobs + 1) * sizeof(obcs::StreamJob)));
+  CUDA_TRY(ctx, status.alloc(16));
+  CUDA_TRY(ctx, cudaMallocAsync((void **)&b->d_xf, (size_t)n * sizeof(obcs::XformRec), ctx->stream));
+  uint8_t *d_new = img.p;
+  uint64_t *d_tab = tabs.at<uint64_t>(0);
+  uint32_t *d_nsz = sizes.at<uint32_t>(0);
+  obcs::StreamJob *d_jobs = job_list.at<obcs::StreamJob>(0);
+  int *d_status = status.at<int>(0);
+  CUDA_TRY(ctx, cudaMemsetAsync(d_status, 0, 16, ctx->stream));
+  CUDA_TRY(ctx, cudaMemsetAsync(d_new, 0, (size_t)pos + 64, ctx->stream));   // block padding and tail slack read as zero
+  CUDA_TRY(ctx, cudaMemcpyAsync(d_tab, tab.data(), (size_t)n * 24, cudaMemcpyHostToDevice, ctx->stream));
+  CUDA_TRY(ctx, cudaMemcpyAsync(d_nsz, nsz.data(), (size_t)n * 4, cudaMemcpyHostToDevice, ctx->stream));
+  obcs::cs_rewrite_kernel<<<(unsigned)((n + 127) / 128), 128, 0, ctx->stream>>>(b->d_image, b->d_blk_off, b->d_blk_size, n, d_new, d_tab, d_nsz,
+                                                                            d_tab + n, d_jobs, scratch.p, d_tab + 2 * (size_t)n, b->d_xf, d_status);
+  if (jobs > 0)
+    obcs::cs_decode_kernel<<<(unsigned)((jobs + 127) / 128), 128, 0, ctx->stream>>>(b->d_image, d_new, d_jobs, (int64_t)jobs, d_status);
+  ctx->launches += jobs > 0 ? 2 : 1;
+  CUDA_TRY(ctx, cudaGetLastError());
   int st = 0;
-  if (e == cudaSuccess) e = cudaMemcpyAsync(&st, d_status, 4, cudaMemcpyDeviceToHost, ctx->stream);
-  if (e == cudaSuccess) {
-    e = install_image(ctx, b, d_new, pos, tab.data(), nsz.data());
-    d_new = nullptr;
-  }
-  if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->stream);
-  for (void *p : {(void *)d_new, (void *)d_scr, (void *)d_tab, (void *)d_nsz, (void *)d_jobs, (void *)d_status})
-    if (p) cudaFreeAsync(p, ctx->stream);
-  if (e != cudaSuccess) return cuda_failure(ctx, e);
+  CUDA_TRY(ctx, cudaMemcpyAsync(&st, d_status, 4, cudaMemcpyDeviceToHost, ctx->stream));
+  if ((ret = install_image(ctx, b, img, pos, tab.data(), nsz.data())) != OBGPU_SUCCESS) return ret;
+  CUDA_TRY(ctx, cudaStreamSynchronize(ctx->stream));
   if (st != 0) {
     ctx->err = "CS integer stream does not decode (corrupt or unsupported codec)";
     return (st & obcs::XF_CORRUPT) ? OBGPU_INVALID_DATA : OBGPU_NOT_SUPPORTED;
@@ -152,21 +135,17 @@ static int cs_restate_batch(obgpu_ctx *ctx, obgpu_batch *b) {
 // kinds of blocks); synchronises.
 static int pax_materialise_batch(obgpu_ctx *ctx, obgpu_batch *b) {
   const int32_t n = b->n_blocks;
-  uint32_t *d_flag = nullptr;
   std::vector<uint32_t> flag(1);
-  CUDA_TRY(ctx, cudaMallocAsync((void **)&d_flag, 16, ctx->stream));
-  cudaError_t e = survey_fetch(ctx, d_flag, 16, flag, [&] {
+  int ret = survey_fetch(ctx, 16, 16, flag, [&](uint32_t *d_flag) {
     obmat::mat_probe_kernel<<<(unsigned)((n + 255) / 256), 256, 0, ctx->stream>>>(b->d_image, b->d_blk_off, b->d_blk_size, n, d_flag);
   });
-  if (e != cudaSuccess) { ctx->err = cudaGetErrorString(e); return OBGPU_ERR_SYS; }
+  if (ret != OBGPU_SUCCESS) return ret;
   if (!(flag[0] & obmat::MF_ANY)) return OBGPU_SUCCESS;
-  uint32_t *d_sv = nullptr;
   std::vector<uint32_t> sv((size_t)n * 4);
-  CUDA_TRY(ctx, cudaMallocAsync((void **)&d_sv, (size_t)n * 16, ctx->stream));
-  e = survey_fetch(ctx, d_sv, 0, sv, [&] {
+  ret = survey_fetch(ctx, (size_t)n * 16, 0, sv, [&](uint32_t *d_sv) {
     obmat::mat_survey_kernel<<<(unsigned)(((int64_t)n * 32 + 127) / 128), 128, 0, ctx->stream>>>(b->d_image, b->d_blk_off, b->d_blk_size, n, d_sv);
   });
-  if (e != cudaSuccess) { ctx->err = cudaGetErrorString(e); return OBGPU_ERR_SYS; }
+  if (ret != OBGPU_SUCCESS) return ret;
   std::vector<uint64_t> tab((size_t)n * 2);   // [new_off][job_base]
   std::vector<uint32_t> nsz((size_t)n);
   uint64_t jobs = 0;
@@ -182,45 +161,37 @@ static int pax_materialise_batch(obgpu_ctx *ctx, obgpu_batch *b) {
   const bool carried = b->d_xf != nullptr;
   std::vector<obcs::XformRec> xf((size_t)n);
   if (carried) {
-    e = cudaMemcpyAsync(xf.data(), b->d_xf, (size_t)n * sizeof(obcs::XformRec), cudaMemcpyDeviceToHost, ctx->stream);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->stream);
-    if (e != cudaSuccess) { ctx->err = cudaGetErrorString(e); return OBGPU_ERR_SYS; }
+    CUDA_TRY(ctx, cudaMemcpyAsync(xf.data(), b->d_xf, (size_t)n * sizeof(obcs::XformRec), cudaMemcpyDeviceToHost, ctx->stream));
+    CUDA_TRY(ctx, cudaStreamSynchronize(ctx->stream));
   } else {
     for (int32_t i = 0; i < n; ++i) { xf[(size_t)i].orig_off = (uint64_t)b->offsets[(size_t)i]; xf[(size_t)i].str_delta = 0; }
   }
-  uint8_t *d_new = nullptr;
-  uint64_t *d_tab = nullptr;
-  uint32_t *d_nsz = nullptr;
-  obmat::MatJob *d_jobs = nullptr;
-  int *d_status = nullptr;
-  e = cudaMallocAsync((void **)&d_new, (size_t)pos + 64, ctx->stream);
-  if (e == cudaSuccess) e = cudaMallocAsync((void **)&d_tab, (size_t)n * 16, ctx->stream);
-  if (e == cudaSuccess) e = cudaMallocAsync((void **)&d_nsz, (size_t)n * 4, ctx->stream);
-  if (e == cudaSuccess) e = cudaMallocAsync((void **)&d_jobs, (size_t)(jobs + 1) * sizeof(obmat::MatJob), ctx->stream);
-  if (e == cudaSuccess) e = cudaMallocAsync((void **)&d_status, 16, ctx->stream);
-  if (e == cudaSuccess && !carried) e = cudaMallocAsync((void **)&b->d_xf, (size_t)n * sizeof(obcs::XformRec), ctx->stream);
-  if (e == cudaSuccess) e = cudaMemsetAsync(d_status, 0, 16, ctx->stream);
-  if (e == cudaSuccess) e = cudaMemsetAsync(d_new, 0, (size_t)pos + 64, ctx->stream);
-  if (e == cudaSuccess) e = cudaMemcpyAsync(d_tab, tab.data(), (size_t)n * 16, cudaMemcpyHostToDevice, ctx->stream);
-  if (e == cudaSuccess) e = cudaMemcpyAsync(d_nsz, nsz.data(), (size_t)n * 4, cudaMemcpyHostToDevice, ctx->stream);
-  if (e == cudaSuccess) {
-    obmat::mat_rewrite_kernel<<<(unsigned)(((int64_t)n * 32 + 127) / 128), 128, 0, ctx->stream>>>(b->d_image, b->d_blk_off, b->d_blk_size, n, d_new,
-                                                                                             d_tab, d_nsz, d_tab + n, d_jobs);
-    obmat::mat_decode_kernel<<<(unsigned)(((int64_t)jobs * 32 + 127) / 128), 128, 0, ctx->stream>>>(b->d_image, d_new, d_jobs, (int64_t)jobs, d_status);
-    ctx->launches += 2;
-    e = cudaGetLastError();
-  }
+  Scratch img(ctx), tabs(ctx), sizes(ctx), job_list(ctx), status(ctx);
+  CUDA_TRY(ctx, img.alloc((size_t)pos + 64));
+  CUDA_TRY(ctx, tabs.alloc((size_t)n * 16));
+  CUDA_TRY(ctx, sizes.alloc((size_t)n * 4));
+  CUDA_TRY(ctx, job_list.alloc((size_t)(jobs + 1) * sizeof(obmat::MatJob)));
+  CUDA_TRY(ctx, status.alloc(16));
+  if (!carried) CUDA_TRY(ctx, cudaMallocAsync((void **)&b->d_xf, (size_t)n * sizeof(obcs::XformRec), ctx->stream));
+  uint8_t *d_new = img.p;
+  uint64_t *d_tab = tabs.at<uint64_t>(0);
+  uint32_t *d_nsz = sizes.at<uint32_t>(0);
+  obmat::MatJob *d_jobs = job_list.at<obmat::MatJob>(0);
+  int *d_status = status.at<int>(0);
+  CUDA_TRY(ctx, cudaMemsetAsync(d_status, 0, 16, ctx->stream));
+  CUDA_TRY(ctx, cudaMemsetAsync(d_new, 0, (size_t)pos + 64, ctx->stream));
+  CUDA_TRY(ctx, cudaMemcpyAsync(d_tab, tab.data(), (size_t)n * 16, cudaMemcpyHostToDevice, ctx->stream));
+  CUDA_TRY(ctx, cudaMemcpyAsync(d_nsz, nsz.data(), (size_t)n * 4, cudaMemcpyHostToDevice, ctx->stream));
+  obmat::mat_rewrite_kernel<<<(unsigned)(((int64_t)n * 32 + 127) / 128), 128, 0, ctx->stream>>>(b->d_image, b->d_blk_off, b->d_blk_size, n, d_new,
+                                                                                           d_tab, d_nsz, d_tab + n, d_jobs);
+  obmat::mat_decode_kernel<<<(unsigned)(((int64_t)jobs * 32 + 127) / 128), 128, 0, ctx->stream>>>(b->d_image, d_new, d_jobs, (int64_t)jobs, d_status);
+  ctx->launches += 2;
+  CUDA_TRY(ctx, cudaGetLastError());
   int st = 0;
-  if (e == cudaSuccess) e = cudaMemcpyAsync(&st, d_status, 4, cudaMemcpyDeviceToHost, ctx->stream);
-  if (e == cudaSuccess) {
-    e = install_image(ctx, b, d_new, pos, tab.data(), nsz.data());
-    d_new = nullptr;
-  }
-  if (e == cudaSuccess && !carried) e = cudaMemcpyAsync(b->d_xf, xf.data(), (size_t)n * sizeof(obcs::XformRec), cudaMemcpyHostToDevice, ctx->stream);
-  if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->stream);
-  for (void *p : {(void *)d_new, (void *)d_tab, (void *)d_nsz, (void *)d_jobs, (void *)d_status})
-    if (p) cudaFreeAsync(p, ctx->stream);
-  if (e != cudaSuccess) return cuda_failure(ctx, e);
+  CUDA_TRY(ctx, cudaMemcpyAsync(&st, d_status, 4, cudaMemcpyDeviceToHost, ctx->stream));
+  if ((ret = install_image(ctx, b, img, pos, tab.data(), nsz.data())) != OBGPU_SUCCESS) return ret;
+  if (!carried) CUDA_TRY(ctx, cudaMemcpyAsync(b->d_xf, xf.data(), (size_t)n * sizeof(obcs::XformRec), cudaMemcpyHostToDevice, ctx->stream));
+  CUDA_TRY(ctx, cudaStreamSynchronize(ctx->stream));
   if (st != 0) {
     ctx->err = "HEX_PACKING / STRING_DIFF / STRING_PREFIX column does not decode (corrupt micro block)";
     return OBGPU_INVALID_DATA;
@@ -252,8 +223,7 @@ static int fill_batch(obgpu_ctx *ctx, obgpu_batch *b, const void *image, int64_t
   // device tables: [blk_off u64 x n][bm_word_off i64 x (n + 1)][blk_size u32 x n] ... [row_start i64 x (n + 1)]
   const size_t tb_rs = (((size_t)n_blocks * (8 + 4) + ((size_t)n_blocks + 1) * 8) + 15) & ~(size_t)15;  // row_start follows
   const size_t tb = tb_rs + ((size_t)n_blocks + 1) * 8 + 64;
-  cudaError_t e = cudaMallocAsync(&b->d_tables, tb, ctx->stream);
-  if (e != cudaSuccess) { ctx->err = cudaGetErrorString(e); return OBGPU_ALLOCATE_MEMORY_FAILED; }
+  CUDA_TRY(ctx, cudaMallocAsync(&b->d_tables, tb, ctx->stream));
   uint8_t *dt = (uint8_t *)b->d_tables;
   b->d_blk_off = (uint64_t *)dt;
   b->d_bm_word_off = (int64_t *)(dt + (size_t)n_blocks * 8);
@@ -285,16 +255,13 @@ static int fill_batch(obgpu_ctx *ctx, obgpu_batch *b, const void *image, int64_t
   } else {
     any_cs = true;   // no host view: the survey kernel of the restatement looks at every block's store type
     any_mat = true;  // ... and the probe kernel of the materialisation at every block's column types
-    uint32_t *d_sv = nullptr;
     std::vector<uint32_t> sv((size_t)n_blocks * 2);
-    e = cudaMemcpyAsync(b->d_tables, stage.data(), tb_rs, cudaMemcpyHostToDevice, ctx->stream);
-    if (e == cudaSuccess) e = cudaMallocAsync((void **)&d_sv, (size_t)n_blocks * 8, ctx->stream);
-    if (e == cudaSuccess)
-      e = survey_fetch(ctx, d_sv, 0, sv, [&] {
-        obgpu_survey_kernel<<<(unsigned)((n_blocks + 255) / 256), 256, 0, ctx->stream>>>((const uint8_t *)image, b->d_blk_off, b->d_blk_size,
-                                                                                         n_blocks, d_sv);
-      });
-    if (e != cudaSuccess) return cuda_failure(ctx, e);
+    CUDA_TRY(ctx, cudaMemcpyAsync(b->d_tables, stage.data(), tb_rs, cudaMemcpyHostToDevice, ctx->stream));
+    const int ret = survey_fetch(ctx, (size_t)n_blocks * 8, 0, sv, [&](uint32_t *d_sv) {
+      obgpu_survey_kernel<<<(unsigned)((n_blocks + 255) / 256), 256, 0, ctx->stream>>>((const uint8_t *)image, b->d_blk_off, b->d_blk_size,
+                                                                                       n_blocks, d_sv);
+    });
+    if (ret != OBGPU_SUCCESS) return ret;
     for (int32_t i = 0; i < n_blocks; ++i) {
       const uint32_t verdict = sv[(size_t)2 * i + 1] >> 16;
       if (verdict == obf::HDR_INVALID || verdict == obf::HDR_EXTENT) { ctx->err = "invalid micro block header"; return OBGPU_INVALID_DATA; }
@@ -325,22 +292,17 @@ static int fill_batch(obgpu_ctx *ctx, obgpu_batch *b, const void *image, int64_t
     rs[0] = 0;
     for (int32_t i = 0; i < n_blocks; ++i) rs[i + 1] = rs[i] + b->row_count[(size_t)i];
   }
-  e = cudaMemcpyAsync(b->d_tables, stage.data(), tb, cudaMemcpyHostToDevice, ctx->stream);
-  if (e == cudaSuccess) {
-    if (image_on_device) {
-      b->d_image = (const uint8_t *)image;
-    } else {
-      void *di = nullptr;
-      e = cudaMallocAsync(&di, (size_t)image_size + 64, ctx->stream);
-      if (e == cudaSuccess) {
-        b->d_image = (const uint8_t *)di;
-        b->own_image = true;
-        e = cudaMemsetAsync((uint8_t *)di + image_size, 0, 64, ctx->stream);
-        if (e == cudaSuccess) e = cudaMemcpyAsync(di, image, (size_t)image_size, cudaMemcpyHostToDevice, ctx->stream);
-      }
-    }
+  CUDA_TRY(ctx, cudaMemcpyAsync(b->d_tables, stage.data(), tb, cudaMemcpyHostToDevice, ctx->stream));
+  if (image_on_device) {
+    b->d_image = (const uint8_t *)image;
+  } else {
+    void *di = nullptr;
+    CUDA_TRY(ctx, cudaMallocAsync(&di, (size_t)image_size + 64, ctx->stream));
+    b->d_image = (const uint8_t *)di;
+    b->own_image = true;
+    CUDA_TRY(ctx, cudaMemsetAsync((uint8_t *)di + image_size, 0, 64, ctx->stream));
+    CUDA_TRY(ctx, cudaMemcpyAsync(di, image, (size_t)image_size, cudaMemcpyHostToDevice, ctx->stream));
   }
-  if (e != cudaSuccess) return cuda_failure(ctx, e);
   int ret;
   // CS blocks whose integer streams carry codecs are restated as RAW once, here (the reference's full_transform at cache fill)
   if (any_cs && (ret = cs_restate_batch(ctx, b)) != OBGPU_SUCCESS) return ret;
@@ -359,30 +321,26 @@ static int fill_batch(obgpu_ctx *ctx, obgpu_batch *b, const void *image, int64_t
   const bool pipe = pipe_wanted(b->max_rows);
   const size_t stage_bytes = pipe ? (size_t)n_blocks * b->max_cols * sizeof(StageRec) : 0;
   constexpr size_t kSpanRows = 8;
-  e = cudaMallocAsync(&dp, plan_bytes + stage_bytes + rows_bytes + rec_bytes + (size_t)b->max_cols * 4 * kSpanRows + 64, ctx->stream);
-  if (e == cudaSuccess) {
-    b->d_plans = (ColDesc *)dp;
-    b->d_stage = pipe ? (StageRec *)((uint8_t *)dp + plan_bytes) : nullptr;
-    b->d_rows = (uint32_t *)((uint8_t *)dp + plan_bytes + stage_bytes);
-    b->d_recs = (BlockRec *)((uint8_t *)dp + plan_bytes + stage_bytes + rows_bytes);
-    uint32_t *d_span = (uint32_t *)((uint8_t *)dp + plan_bytes + stage_bytes + rows_bytes + rec_bytes);
-    // per-column reductions of the index kernel: [region span][dictionary size][type min][type max][RLE runs][projection span][materialised]
-    // [stage record gaps: SR_NOT_FILTER | SR_NOT_FLAT]
-    e = cudaMemsetAsync(d_span, 0, (size_t)b->max_cols * 4 * kSpanRows, ctx->stream);
-    if (e == cudaSuccess) e = cudaMemsetAsync(d_span + 2 * (size_t)b->max_cols, 0xff, (size_t)b->max_cols * 4, ctx->stream);
-    const int64_t nthreads = (int64_t)n_blocks * b->max_cols;
-    obgpu_index_kernel<<<(unsigned)((nthreads + 255) / 256), 256, 0, ctx->stream>>>(
-        b->d_image, b->d_blk_off, b->d_blk_size, b->d_bm_word_off, n_blocks, (int)b->max_cols, b->d_plans,
-        b->d_rows, b->d_recs, b->d_stage, d_span);
-    if (e == cudaSuccess) e = cudaGetLastError();
-    ctx->launches++;
-    b->col_span.assign((size_t)b->max_cols * kSpanRows, 0);
-    if (e == cudaSuccess)
-      e = cudaMemcpyAsync(b->col_span.data(), d_span, (size_t)b->max_cols * 4 * kSpanRows, cudaMemcpyDeviceToHost, ctx->stream);
-  }
+  CUDA_TRY(ctx, cudaMallocAsync(&dp, plan_bytes + stage_bytes + rows_bytes + rec_bytes + (size_t)b->max_cols * 4 * kSpanRows + 64, ctx->stream));
+  b->d_plans = (ColDesc *)dp;
+  b->d_stage = pipe ? (StageRec *)((uint8_t *)dp + plan_bytes) : nullptr;
+  b->d_rows = (uint32_t *)((uint8_t *)dp + plan_bytes + stage_bytes);
+  b->d_recs = (BlockRec *)((uint8_t *)dp + plan_bytes + stage_bytes + rows_bytes);
+  uint32_t *d_span = (uint32_t *)((uint8_t *)dp + plan_bytes + stage_bytes + rows_bytes + rec_bytes);
+  // per-column reductions of the index kernel: [region span][dictionary size][type min][type max][RLE runs][projection span][materialised]
+  // [stage record gaps: SR_NOT_FILTER | SR_NOT_FLAT]
+  CUDA_TRY(ctx, cudaMemsetAsync(d_span, 0, (size_t)b->max_cols * 4 * kSpanRows, ctx->stream));
+  CUDA_TRY(ctx, cudaMemsetAsync(d_span + 2 * (size_t)b->max_cols, 0xff, (size_t)b->max_cols * 4, ctx->stream));
+  const int64_t nthreads = (int64_t)n_blocks * b->max_cols;
+  obgpu_index_kernel<<<(unsigned)((nthreads + 255) / 256), 256, 0, ctx->stream>>>(
+      b->d_image, b->d_blk_off, b->d_blk_size, b->d_bm_word_off, n_blocks, (int)b->max_cols, b->d_plans,
+      b->d_rows, b->d_recs, b->d_stage, d_span);
+  ctx->launches++;
+  CUDA_TRY(ctx, cudaGetLastError());
+  b->col_span.assign((size_t)b->max_cols * kSpanRows, 0);
+  CUDA_TRY(ctx, cudaMemcpyAsync(b->col_span.data(), d_span, (size_t)b->max_cols * 4 * kSpanRows, cudaMemcpyDeviceToHost, ctx->stream));
   // `stage` is pageable: the copy above is staged synchronously by the runtime before returning
-  if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->stream);
-  if (e != cudaSuccess) return cuda_failure(ctx, e);
+  CUDA_TRY(ctx, cudaStreamSynchronize(ctx->stream));
   const size_t mc = b->max_cols;
   b->col_pspan.assign(b->col_span.begin() + 5 * mc, b->col_span.begin() + 6 * mc);
   b->col_stage_gaps.assign(b->col_span.begin() + 7 * mc, b->col_span.begin() + 8 * mc);

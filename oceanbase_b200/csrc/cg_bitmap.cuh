@@ -73,20 +73,23 @@ extern "C" {
 int obgpu_cg_bitmap_create(obgpu_ctx *ctx, int64_t n_rows, int32_t all_true, obgpu_cg_bitmap **out) {
   if (!ctx || !out || n_rows < 0) return OBGPU_INVALID_ARGUMENT;
   cudaSetDevice(ctx->device);
-  obgpu_cg_bitmap *bm = new (std::nothrow) obgpu_cg_bitmap();
+  std::unique_ptr<obgpu_cg_bitmap> bm(new (std::nothrow) obgpu_cg_bitmap());
   if (!bm) return OBGPU_ALLOCATE_MEMORY_FAILED;
   bm->ctx = ctx;
   bm->n_rows = n_rows;
   const size_t words = (size_t)((n_rows + 31) / 32) + 2;
-  if (cudaMallocAsync((void **)&bm->d_words, words * 4, ctx->stream) != cudaSuccess) { delete bm; return OBGPU_ALLOCATE_MEMORY_FAILED; }
-  cudaMemsetAsync(bm->d_words, all_true ? 0xff : 0, words * 4, ctx->stream);
+  Scratch w(ctx);
+  CUDA_TRY(ctx, w.alloc(words * 4));
+  uint32_t *d_words = w.at<uint32_t>(0);
+  CUDA_TRY(ctx, cudaMemsetAsync(d_words, all_true ? 0xff : 0, words * 4, ctx->stream));
   if (all_true && (n_rows & 31)) {   // bits past the range stay clear (popcounts, folds of neighbours)
     const uint32_t last = (1u << (n_rows & 31)) - 1u;
-    cudaMemcpyAsync(bm->d_words + n_rows / 32, &last, 4, cudaMemcpyHostToDevice, ctx->stream);
-    cudaStreamSynchronize(ctx->stream);
+    CUDA_TRY(ctx, cudaMemcpyAsync(d_words + n_rows / 32, &last, 4, cudaMemcpyHostToDevice, ctx->stream));
+    CUDA_TRY(ctx, cudaStreamSynchronize(ctx->stream));
   }
-  if (all_true) cudaMemsetAsync(bm->d_words + (n_rows + 31) / 32, 0, 8, ctx->stream);
-  *out = bm;
+  if (all_true) CUDA_TRY(ctx, cudaMemsetAsync(d_words + (n_rows + 31) / 32, 0, 8, ctx->stream));
+  bm->d_words = (uint32_t *)w.release();
+  *out = bm.release();
   return OBGPU_SUCCESS;
 }
 
@@ -117,10 +120,10 @@ int obgpu_cg_bitmap_popcnt(obgpu_cg_bitmap *bm, int64_t from, int64_t to, int64_
   cudaSetDevice(ctx->device);
   *count = 0;
   if (to == from) return OBGPU_SUCCESS;
-  TempDev tmp(ctx);
+  Scratch tmp(ctx);
   CUDA_TRY(ctx, tmp.alloc(64));
   CUDA_TRY(ctx, cudaMemsetAsync(tmp.p, 0, 64, ctx->stream));
-  cgbm::popcnt_kernel<<<std::min<int64_t>(1024, ((to - from) / 32 + 256) / 256), 256, 0, ctx->stream>>>(bm->d_words, from, to, (unsigned long long *)tmp.p);
+  cgbm::popcnt_kernel<<<std::min<int64_t>(1024, ((to - from) / 32 + 256) / 256), 256, 0, ctx->stream>>>(bm->d_words, from, to, tmp.at<unsigned long long>(0));
   ctx->launches++;
   unsigned long long c = 0;
   CUDA_TRY(ctx, cudaMemcpyAsync(&c, tmp.p, 8, cudaMemcpyDeviceToHost, ctx->stream));
@@ -134,9 +137,9 @@ int obgpu_cg_bitmap_fetch(obgpu_cg_bitmap *bm, int64_t from, int64_t count, uint
   if (count == 0) return OBGPU_SUCCESS;
   obgpu_ctx *ctx = bm->ctx;
   cudaSetDevice(ctx->device);
-  TempDev tmp(ctx);
+  Scratch tmp(ctx);
   CUDA_TRY(ctx, tmp.alloc((size_t)count));
-  cgbm::expand_kernel<<<(unsigned)((count + 255) / 256), 256, 0, ctx->stream>>>(bm->d_words, from, count, (uint8_t *)tmp.p);
+  cgbm::expand_kernel<<<(unsigned)((count + 255) / 256), 256, 0, ctx->stream>>>(bm->d_words, from, count, tmp.p);
   ctx->launches++;
   CUDA_TRY(ctx, cudaMemcpyAsync(host_bitmap_bytes, tmp.p, (size_t)count, cudaMemcpyDeviceToHost, ctx->stream));
   CUDA_TRY(ctx, cudaStreamSynchronize(ctx->stream));

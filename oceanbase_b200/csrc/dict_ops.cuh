@@ -201,12 +201,13 @@ int obgpu_block_read_distinct(obgpu_batch *b, int32_t block, int32_t col, uint64
   if (d.sc == 5 && !lens) return OBGPU_INVALID_ARGUMENT;
   if (d.dict_count == 0) return OBGPU_SUCCESS;
   obgpu_ctx *ctx = c.ctx;
-  TempDev tmp(ctx);
+  Scratch tmp(ctx);
   const size_t n = d.dict_count;
-  CUDA_TRY(ctx, tmp.alloc(64 + n * 12));
-  int *d_status = (int *)tmp.p;
-  uint64_t *d_vals = (uint64_t *)((uint8_t *)tmp.p + 64);
-  int32_t *d_lens = (int32_t *)((uint8_t *)tmp.p + 64 + n * 8);
+  const size_t o_status = tmp.take(64, 8), o_vals = tmp.take(n * 8, 8), o_lens = tmp.take(n * 4, 4);
+  CUDA_TRY(ctx, tmp.alloc());
+  int *d_status = tmp.at<int>(o_status);
+  uint64_t *d_vals = tmp.at<uint64_t>(o_vals);
+  int32_t *d_lens = tmp.at<int32_t>(o_lens);
   CUDA_TRY(ctx, cudaMemsetAsync(tmp.p, 0, 64, ctx->stream));
   dictops::read_distinct_kernel<<<1, 128, 0, ctx->stream>>>(c.a, block, col, d_vals, d_lens, d_status);
   ctx->launches++;
@@ -236,11 +237,12 @@ int obgpu_block_read_reference(obgpu_batch *b, int32_t block, int32_t col, const
   if (ret != OBGPU_SUCCESS || !row_ids || !refs || row_cap < 0) return ret != OBGPU_SUCCESS ? ret : OBGPU_INVALID_ARGUMENT;
   if (row_cap == 0) return OBGPU_SUCCESS;
   obgpu_ctx *ctx = c.ctx;
-  TempDev tmp(ctx);
-  CUDA_TRY(ctx, tmp.alloc(64 + (size_t)row_cap * 8));
-  int *d_status = (int *)tmp.p;
-  int32_t *d_rid = (int32_t *)((uint8_t *)tmp.p + 64);
-  uint32_t *d_refs = (uint32_t *)((uint8_t *)tmp.p + 64 + (size_t)row_cap * 4);
+  Scratch tmp(ctx);
+  const size_t o_status = tmp.take(64, 4), o_rid = tmp.take((size_t)row_cap * 4, 4), o_refs = tmp.take((size_t)row_cap * 4, 4);
+  CUDA_TRY(ctx, tmp.alloc());
+  int *d_status = tmp.at<int>(o_status);
+  int32_t *d_rid = tmp.at<int32_t>(o_rid);
+  uint32_t *d_refs = tmp.at<uint32_t>(o_refs);
   CUDA_TRY(ctx, cudaMemsetAsync(tmp.p, 0, 64, ctx->stream));
   CUDA_TRY(ctx, cudaMemcpyAsync(d_rid, row_ids, (size_t)row_cap * 4, cudaMemcpyHostToDevice, ctx->stream));
   dictops::read_reference_kernel<<<1, 128, 0, ctx->stream>>>(c.a, block, col, d_rid, row_cap, d_refs, d_status);
@@ -270,10 +272,11 @@ int obgpu_filter_dict_pass(obgpu_batch *b, int32_t block, int32_t col, const uin
   }
   if (count == 0) return OBGPU_SUCCESS;
   obgpu_ctx *ctx = c.ctx;
-  TempDev tmp(ctx);
-  const size_t o_pass = 64, o_out = o_pass + (((size_t)n_entries + 63) & ~(size_t)63) + 64;
-  CUDA_TRY(ctx, tmp.alloc(o_out + (size_t)count));
-  uint8_t *base = (uint8_t *)tmp.p;
+  Scratch tmp(ctx);
+  tmp.take(64, 64);   // status
+  const size_t o_pass = tmp.take((size_t)n_entries + 64, 64), o_out = tmp.take((size_t)count, 64);
+  CUDA_TRY(ctx, tmp.alloc());
+  uint8_t *base = tmp.p;
   CUDA_TRY(ctx, cudaMemsetAsync(base, 0, 64, ctx->stream));
   if (n_entries) CUDA_TRY(ctx, cudaMemcpyAsync(base + o_pass, entry_pass, (size_t)n_entries, cudaMemcpyHostToDevice, ctx->stream));
   dictops::dict_pass_kernel<<<1, 128, 0, ctx->stream>>>(c.a, block, col, base + o_pass, n_entries, null_pass, start, count, base + o_out, (int *)base);
@@ -320,12 +323,12 @@ static int group_by_common(obgpu_batch *b, int32_t block0, int32_t n_blocks, int
   *total_groups = G;
   if (host_group_off) memcpy(host_group_off, goff.data(), ((size_t)n_blocks + 1) * 8);
   if (G > out_cap_groups) return OBGPU_BUF_NOT_ENOUGH;
-  TempDev tmp(ctx);
-  const size_t o_goff = 64, o_rid = o_goff + (((size_t)n_blocks + 1) * 8 + 63 & ~(size_t)63);
-  const size_t o_out = o_rid + (((size_t)(row_ids ? row_cap : 0) * 4 + 63) & ~(size_t)63);
-  const size_t out_bytes = (size_t)n_aggs * (size_t)G * 16;
-  CUDA_TRY(ctx, tmp.alloc(o_out + out_bytes));
-  uint8_t *base = (uint8_t *)tmp.p;
+  Scratch tmp(ctx);
+  tmp.take(64, 64);   // status
+  const size_t o_goff = tmp.take(((size_t)n_blocks + 1) * 8, 64), o_rid = tmp.take((size_t)(row_ids ? row_cap : 0) * 4, 64);
+  const size_t out_bytes = (size_t)n_aggs * (size_t)G * 16, o_out = tmp.take(out_bytes, 64);
+  CUDA_TRY(ctx, tmp.alloc());
+  uint8_t *base = tmp.p;
   CUDA_TRY(ctx, cudaMemsetAsync(base, 0, o_out + out_bytes, ctx->stream));
   CUDA_TRY(ctx, cudaMemcpyAsync(base + o_goff, goff.data(), ((size_t)n_blocks + 1) * 8, cudaMemcpyHostToDevice, ctx->stream));
   if (row_ids && row_cap > 0) CUDA_TRY(ctx, cudaMemcpyAsync(base + o_rid, row_ids, (size_t)row_cap * 4, cudaMemcpyHostToDevice, ctx->stream));

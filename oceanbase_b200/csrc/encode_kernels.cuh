@@ -975,27 +975,25 @@ int obgpu_encode_columns_ex(obgpu_ctx *ctx, const obgpu_encode_col *cols, const 
   const uint32_t lw_max = (uint32_t)(((slot_cap / 4 + enc::kThreads - 1) / enc::kThreads) | 1);
   const uint32_t *d_xpow = enc_xpow_table(ctx);
   if (!d_xpow) return OBGPU_ALLOCATE_MEMORY_FAILED;
-  obgpu_encoded *e = new obgpu_encoded();
+  std::unique_ptr<obgpu_encoded> e(new obgpu_encoded());
   e->ctx = ctx;
   e->n_cols = n_cols;
   e->n_blocks = (int32_t)n_blocks64;
   e->total_rows = total_rows;
-  auto al = [](size_t x) { return (x + 255) & ~(size_t)255; };
-  size_t o = 0;
-  const size_t o_ctl = o; o += al(256 + (size_t)n_cols * 8);
-  const size_t o_flags = o; o += al((size_t)n_blocks64 * 8);
-  const size_t o_off = o; o += al((size_t)n_blocks64 * 8);
-  const size_t o_size = o; o += al((size_t)n_blocks64 * 4);
-  const size_t o_img = o; o += al((size_t)n_blocks64 * (size_t)slot_cap);
-  cudaError_t err = cudaMallocAsync(&e->arena, o, ctx->stream);
-  if (err != cudaSuccess) { ctx->err = cudaGetErrorString(err); delete e; return OBGPU_ALLOCATE_MEMORY_FAILED; }
-  uint8_t *a = (uint8_t *)e->arena;
+  Scratch arena(ctx);
+  const size_t o_ctl = arena.take(256 + (size_t)n_cols * 8);
+  const size_t o_flags = arena.take((size_t)n_blocks64 * 8);
+  const size_t o_off = arena.take((size_t)n_blocks64 * 8);
+  const size_t o_size = arena.take((size_t)n_blocks64 * 4);
+  const size_t o_img = arena.take((size_t)n_blocks64 * (size_t)slot_cap);
+  CUDA_TRY(ctx, arena.alloc());
+  uint8_t *a = arena.p;
   e->d_totals = (unsigned long long *)(a + o_ctl);
   e->d_checksums = (unsigned long long *)(a + o_ctl + 256);
   e->d_off = (int64_t *)(a + o_off);
   e->d_size = (uint32_t *)(a + o_size);
   e->d_image = a + o_img;
-  cudaMemsetAsync(a, 0, o_off, ctx->stream);   // totals, ticket, checksums, look-back flags
+  CUDA_TRY(ctx, cudaMemsetAsync(a, 0, o_off, ctx->stream));   // totals, ticket, checksums, look-back flags
   p.rowkey_cnt = rowkey_col_cnt;
   p.n_blocks = e->n_blocks;
   p.want_checksums = 1;
@@ -1015,13 +1013,12 @@ int obgpu_encode_columns_ex(obgpu_ctx *ctx, const obgpu_encode_col *cols, const 
   p.xpow32 = d_xpow;
   // the AUTO instantiation only when some column asks for it: RAW-only calls keep the RAW kernel
   auto kernel = n_auto ? enc::obgpu_encode_blocks_kernel<true, true> : enc::obgpu_encode_blocks_kernel<true, false>;
-  err = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-  if (err != cudaSuccess) { ctx->err = cudaGetErrorString(err); obgpu_encoded_free(e); return OBGPU_ERR_SYS; }
+  CUDA_TRY(ctx, cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   kernel<<<(unsigned)e->n_blocks, enc::kThreads, smem, ctx->stream>>>(p);
   ctx->launches++;
-  err = cudaGetLastError();
-  if (err != cudaSuccess) { ctx->err = cudaGetErrorString(err); obgpu_encoded_free(e); return OBGPU_ERR_SYS; }
-  *out = e;
+  CUDA_TRY(ctx, cudaGetLastError());
+  e->arena = arena.release();
+  *out = e.release();
   return OBGPU_SUCCESS;
 }
 
@@ -1094,19 +1091,18 @@ int obgpu_column_checksums(obgpu_ctx *ctx, const obgpu_encode_col *cols, int32_t
   int rc = enc_fill_cols(p, cols, n_cols);
   if (rc != OBGPU_SUCCESS) return rc;
   cudaSetDevice(ctx->device);
-  unsigned long long *d = nullptr;
-  CUDA_TRY(ctx, cudaMallocAsync((void **)&d, (size_t)n_cols * 8, ctx->stream));
-  cudaMemsetAsync(d, 0, (size_t)n_cols * 8, ctx->stream);
+  Scratch sums(ctx);
+  CUDA_TRY(ctx, sums.alloc((size_t)n_cols * 8));
+  unsigned long long *d = sums.at<unsigned long long>(0);
+  CUDA_TRY(ctx, cudaMemsetAsync(d, 0, (size_t)n_cols * 8, ctx->stream));
   p.total_rows = total_rows;
   p.checksums = d;
   const int64_t want = (total_rows + enc::kCkThreads * 8 - 1) / (enc::kCkThreads * 8);
   const unsigned grid = (unsigned)std::max<int64_t>(1, std::min<int64_t>(want, (int64_t)ctx->sm_count * 8));
   enc::obgpu_column_checksum_kernel<<<grid, enc::kCkThreads, 0, ctx->stream>>>(p);
   ctx->launches++;
-  cudaError_t err = cudaMemcpyAsync(host_checksums, d, (size_t)n_cols * 8, cudaMemcpyDeviceToHost, ctx->stream);
-  if (err == cudaSuccess) err = cudaStreamSynchronize(ctx->stream);
-  cudaFreeAsync(d, ctx->stream);
-  if (err != cudaSuccess) { ctx->err = cudaGetErrorString(err); return OBGPU_ERR_SYS; }
+  CUDA_TRY(ctx, cudaMemcpyAsync(host_checksums, d, (size_t)n_cols * 8, cudaMemcpyDeviceToHost, ctx->stream));
+  CUDA_TRY(ctx, cudaStreamSynchronize(ctx->stream));
   return OBGPU_SUCCESS;
 }
 

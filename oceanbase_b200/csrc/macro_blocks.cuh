@@ -102,66 +102,72 @@ int obgpu_batch_open_macro_blocks(obgpu_ctx *ctx, const void *macro_image, int64
       image_size < macro_block_size * (int64_t)n_macro_blocks)
     return OBGPU_INVALID_ARGUMENT;
   cudaSetDevice(ctx->device);
-  DeviceImage img;
+  DeviceImage img(ctx);
   int ret = stage_image(ctx, macro_image, image_size, image_on_device, "device-resident macro blocks must be 16-byte aligned", img);
   if (ret != OBGPU_SUCCESS) return ret;
   const uint8_t *d_macro = img.d;
-  void *d_small = nullptr, *d_tab = nullptr;
   std::vector<int32_t> counts((size_t)n_macro_blocks + 1), comps((size_t)n_macro_blocks);
   std::vector<int64_t> first((size_t)n_macro_blocks + 1);
   int64_t n_micro = 0;
-  auto fail = [&](int code, const char *what) { if (what) ctx->err = what; ret = code; };
-  do {
-    // [counts i32 x n][status i32][first i64 x (n + 1), 16-byte aligned][compressor i32 x n]
-    const size_t first_at = (((size_t)n_macro_blocks + 1) * 4 + 15) / 16 * 16, comps_at = first_at + ((size_t)n_macro_blocks + 1) * 8;
-    if (cudaMallocAsync(&d_small, comps_at + (size_t)n_macro_blocks * 4 + 64, ctx->stream) != cudaSuccess) { fail(OBGPU_ALLOCATE_MEMORY_FAILED, "macro survey tables"); break; }
-    int32_t *d_counts = (int32_t *)d_small, *d_status = d_counts + n_macro_blocks;
-    int64_t *d_first = (int64_t *)((uint8_t *)d_small + first_at);
-    int32_t *d_comps = (int32_t *)((uint8_t *)d_small + comps_at);
-    cudaMemsetAsync(d_status, 0, 4, ctx->stream);
-    mb::obgpu_macro_survey_kernel<<<(unsigned)((n_macro_blocks + 127) / 128), 128, 0, ctx->stream>>>(d_macro, macro_block_size, n_macro_blocks, d_counts,
-                                                                                                     d_comps, d_status);
-    ctx->launches++;
-    if (cudaMemcpyAsync(counts.data(), d_counts, ((size_t)n_macro_blocks + 1) * 4, cudaMemcpyDeviceToHost, ctx->stream) != cudaSuccess ||
-        cudaMemcpyAsync(comps.data(), d_comps, (size_t)n_macro_blocks * 4, cudaMemcpyDeviceToHost, ctx->stream) != cudaSuccess ||
-        cudaStreamSynchronize(ctx->stream) != cudaSuccess) { fail(OBGPU_ERR_SYS, "macro survey"); break; }
-    if (counts[(size_t)n_macro_blocks] != mb::kStOk) {
-      fail(counts[(size_t)n_macro_blocks] == mb::kStCompressed ? OBGPU_NOT_SUPPORTED : OBGPU_INVALID_DATA,
-           counts[(size_t)n_macro_blocks] == mb::kStCompressed ? "compressed or encrypted macro block" : "macro block header is invalid");
-      break;
+  // [counts i32 x n][status i32][first i64 x (n + 1), 16-byte aligned by the padding of the counts][compressor i32 x n]
+  Scratch small(ctx);
+  const size_t o_counts = small.take(((size_t)n_macro_blocks + 1) * 4, 16), o_first = small.take(((size_t)n_macro_blocks + 1) * 8, 8);
+  const size_t o_comps = small.take((size_t)n_macro_blocks * 4 + 64, 4);
+  CUDA_TRY(ctx, small.alloc());
+  int32_t *d_counts = small.at<int32_t>(o_counts), *d_status = d_counts + n_macro_blocks;
+  int64_t *d_first = small.at<int64_t>(o_first);
+  int32_t *d_comps = small.at<int32_t>(o_comps);
+  CUDA_TRY(ctx, cudaMemsetAsync(d_status, 0, 4, ctx->stream));
+  mb::obgpu_macro_survey_kernel<<<(unsigned)((n_macro_blocks + 127) / 128), 128, 0, ctx->stream>>>(d_macro, macro_block_size, n_macro_blocks, d_counts,
+                                                                                                   d_comps, d_status);
+  ctx->launches++;
+  CUDA_TRY(ctx, cudaMemcpyAsync(counts.data(), d_counts, ((size_t)n_macro_blocks + 1) * 4, cudaMemcpyDeviceToHost, ctx->stream));
+  CUDA_TRY(ctx, cudaMemcpyAsync(comps.data(), d_comps, (size_t)n_macro_blocks * 4, cudaMemcpyDeviceToHost, ctx->stream));
+  CUDA_TRY(ctx, cudaStreamSynchronize(ctx->stream));
+  if (counts[(size_t)n_macro_blocks] != mb::kStOk) {
+    const bool compressed = counts[(size_t)n_macro_blocks] == mb::kStCompressed;
+    ctx->err = compressed ? "compressed or encrypted macro block" : "macro block header is invalid";
+    return compressed ? OBGPU_NOT_SUPPORTED : OBGPU_INVALID_DATA;
+  }
+  // one SSTable has one compressor: the macro blocks that are not NONE must agree (NONE ones hold raw blocks only)
+  int32_t compressor = OBGPU_COMPRESSOR_NONE;
+  bool mixed = false;
+  for (int32_t c : comps)
+    if (c != OBGPU_COMPRESSOR_NONE) {
+      mixed = mixed || (compressor != OBGPU_COMPRESSOR_NONE && c != compressor);
+      compressor = c;
     }
-    // one SSTable has one compressor: the macro blocks that are not NONE must agree (NONE ones hold raw blocks only)
-    int32_t compressor = OBGPU_COMPRESSOR_NONE;
-    bool mixed = false;
-    for (int32_t c : comps)
-      if (c != OBGPU_COMPRESSOR_NONE) {
-        mixed = mixed || (compressor != OBGPU_COMPRESSOR_NONE && c != compressor);
-        compressor = c;
-      }
-    if (mixed) { fail(OBGPU_NOT_SUPPORTED, "macro blocks of one open use different compressors"); break; }
-    for (int32_t i = 0; i < n_macro_blocks; ++i) { first[(size_t)i] = n_micro; n_micro += counts[(size_t)i]; }
-    first[(size_t)n_macro_blocks] = n_micro;
-    if (n_micro <= 0 || n_micro > 0x7fffffff) { fail(OBGPU_INVALID_DATA, "macro blocks hold no micro-block"); break; }
-    if (cudaMallocAsync(&d_tab, (size_t)n_micro * 16 + 64, ctx->stream) != cudaSuccess) { fail(OBGPU_ALLOCATE_MEMORY_FAILED, "micro-block tables"); break; }
-    int64_t *d_src = (int64_t *)d_tab, *d_sizes = d_src + n_micro;
-    cudaMemcpyAsync(d_first, first.data(), ((size_t)n_macro_blocks + 1) * 8, cudaMemcpyHostToDevice, ctx->stream);
-    mb::obgpu_macro_walk_kernel<<<(unsigned)((n_macro_blocks + 63) / 64), 64, 0, ctx->stream>>>(d_macro, macro_block_size, n_macro_blocks, d_first, d_src, d_sizes, d_status);
-    ctx->launches++;
-    int32_t st = 0;
-    if (cudaMemcpyAsync(&st, d_status, 4, cudaMemcpyDeviceToHost, ctx->stream) != cudaSuccess ||
-        cudaStreamSynchronize(ctx->stream) != cudaSuccess) { fail(OBGPU_ERR_SYS, "macro walk"); break; }
-    if (st != mb::kStOk) { fail(OBGPU_INVALID_DATA, "micro-block chain of a macro block is inconsistent"); break; }
-    // NONE macro blocks were checked by the walk (every block raw); the others admit raw and compressed blocks alike
-    obgpu_batch *b = nullptr;
-    ret = open_stored_blocks(ctx, d_macro, image_size, d_src, d_sizes, (int32_t)n_micro, compressor, &b);
-    if (ret != OBGPU_SUCCESS) break;
-    *out = b;
-    if (n_micro_out) *n_micro_out = (int32_t)n_micro;
-  } while (0);
-  if (d_small) cudaFreeAsync(d_small, ctx->stream);
-  if (d_tab) cudaFreeAsync(d_tab, ctx->stream);
-  if (img.tmp) cudaFreeAsync(img.tmp, ctx->stream);
-  return ret;
+  if (mixed) {
+    ctx->err = "macro blocks of one open use different compressors";
+    return OBGPU_NOT_SUPPORTED;
+  }
+  for (int32_t i = 0; i < n_macro_blocks; ++i) { first[(size_t)i] = n_micro; n_micro += counts[(size_t)i]; }
+  first[(size_t)n_macro_blocks] = n_micro;
+  if (n_micro <= 0 || n_micro > 0x7fffffff) {
+    ctx->err = "macro blocks hold no micro-block";
+    return OBGPU_INVALID_DATA;
+  }
+  Scratch tab(ctx);   // [src][sizes]
+  const size_t o_src = tab.take((size_t)n_micro * 8, 8), o_sizes = tab.take((size_t)n_micro * 8 + 64, 8);
+  CUDA_TRY(ctx, tab.alloc());
+  int64_t *d_src = tab.at<int64_t>(o_src), *d_sizes = tab.at<int64_t>(o_sizes);
+  CUDA_TRY(ctx, cudaMemcpyAsync(d_first, first.data(), ((size_t)n_macro_blocks + 1) * 8, cudaMemcpyHostToDevice, ctx->stream));
+  mb::obgpu_macro_walk_kernel<<<(unsigned)((n_macro_blocks + 63) / 64), 64, 0, ctx->stream>>>(d_macro, macro_block_size, n_macro_blocks, d_first, d_src, d_sizes, d_status);
+  ctx->launches++;
+  int32_t st = 0;
+  CUDA_TRY(ctx, cudaMemcpyAsync(&st, d_status, 4, cudaMemcpyDeviceToHost, ctx->stream));
+  CUDA_TRY(ctx, cudaStreamSynchronize(ctx->stream));
+  if (st != mb::kStOk) {
+    ctx->err = "micro-block chain of a macro block is inconsistent";
+    return OBGPU_INVALID_DATA;
+  }
+  // NONE macro blocks were checked by the walk (every block raw); the others admit raw and compressed blocks alike
+  obgpu_batch *b = nullptr;
+  ret = open_stored_blocks(ctx, d_macro, image_size, d_src, d_sizes, (int32_t)n_micro, compressor, &b);
+  if (ret != OBGPU_SUCCESS) return ret;
+  *out = b;
+  if (n_micro_out) *n_micro_out = (int32_t)n_micro;
+  return OBGPU_SUCCESS;
 }
 
 }  // extern "C"

@@ -170,29 +170,35 @@ int obgpu_merge_decoded_distributed(obgpu_ctx *ctx, obgpu_comm *comm, const obgp
   const int world = comm->world, rank = comm->rank, S = samples_per_run;
   cudaSetDevice(ctx->device);
   cudaStream_t st = ctx->stream;
-#define NCCL_TRY(expr) do { const ncclResult_t r__ = (expr); if (r__ != ncclSuccess) { ctx->err = std::string(#expr) + ": " + (a.GetErrorString ? a.GetErrorString(r__) : "nccl error"); cleanup(); return OBGPU_ERR_SYS; } } while (0)
-#define CU_TRY(expr) do { const cudaError_t e__ = (expr); if (e__ != cudaSuccess) { ctx->err = std::string(#expr) + ": " + cudaGetErrorString(e__); cleanup(); return e__ == cudaErrorMemoryAllocation ? OBGPU_ALLOCATE_MEMORY_FAILED : OBGPU_ERR_SYS; } } while (0)
-  std::vector<void *> temps;
-  auto cleanup = [&]() { for (void *p : temps) cudaFreeAsync(p, st); temps.clear(); };
-  auto dalloc = [&](size_t bytes) -> void * {
-    void *p = nullptr;
-    if (cudaMallocAsync(&p, bytes ? bytes : 16, st) != cudaSuccess) return nullptr;
-    temps.push_back(p);
-    return p;
+#define NCCL_TRY(expr)                                                                                                          \
+  if (const ncclResult_t r__ = (expr); r__ != ncclSuccess) {                                                                    \
+    ctx->err = std::string(#expr) + ": " + (a.GetErrorString ? a.GetErrorString(r__) : "nccl error");                         \
+    return OBGPU_ERR_SYS;                                                                                                       \
+  } else (void)0
+  // every device buffer of the call; freed on the stream when it returns, after the kernels and transfers that use them
+  std::deque<Scratch> bufs;
+  auto dalloc = [&](size_t bytes, auto *&p) {
+    Scratch &s = bufs.emplace_back(ctx);
+    const cudaError_t e = s.alloc(bytes);
+    p = s.at<std::remove_reference_t<decltype(*p)>>(0);
+    return e;
   };
   const size_t slots = (size_t)n_runs_total * S;
-  int64_t *d_cand = (int64_t *)dalloc(slots * 8), *d_all = (int64_t *)dalloc(slots * 8 * world), *d_sorted = (int64_t *)dalloc(slots * 8 * world);
-  int64_t *d_split = (int64_t *)dalloc((size_t)std::max(world - 1, 1) * 8);
-  long long *d_tab = (long long *)dalloc(((size_t)n_runs_total * world + 2 * (size_t)n_runs_total + 2) * 8);   // cnt | held | owner | valid
-  int64_t *d_bounds = (int64_t *)dalloc((size_t)std::max(n_local, 1) * (world + 1) * 8);
-  if (!d_cand || !d_all || !d_sorted || !d_split || !d_tab || !d_bounds) { ctx->err = "out of device memory"; cleanup(); return OBGPU_ALLOCATE_MEMORY_FAILED; }
+  int64_t *d_cand, *d_all, *d_sorted, *d_split, *d_bounds;
+  long long *d_tab;   // cnt | held | owner | valid
+  CUDA_TRY(ctx, dalloc(slots * 8, d_cand));
+  CUDA_TRY(ctx, dalloc(slots * 8 * world, d_all));
+  CUDA_TRY(ctx, dalloc(slots * 8 * world, d_sorted));
+  CUDA_TRY(ctx, dalloc((size_t)std::max(world - 1, 1) * 8, d_split));
+  CUDA_TRY(ctx, dalloc(((size_t)n_runs_total * world + 2 * (size_t)n_runs_total + 2) * 8, d_tab));
+  CUDA_TRY(ctx, dalloc((size_t)std::max(n_local, 1) * (world + 1) * 8, d_bounds));
   long long *d_cnt = d_tab, *d_held = d_tab + (size_t)n_runs_total * world, *d_owner = d_held + n_runs_total, *d_valid = d_owner + n_runs_total;
-  CU_TRY(cudaMemsetAsync(d_tab, 0, ((size_t)n_runs_total * world + 2 * (size_t)n_runs_total + 2) * 8, st));
+  CUDA_TRY(ctx, cudaMemsetAsync(d_tab, 0, ((size_t)n_runs_total * world + 2 * (size_t)n_runs_total + 2) * 8, st));
   // 1. candidates (slots of runs held elsewhere stay INT64_MAX)
   {
     std::vector<int64_t> fill(slots, INT64_MAX);
-    CU_TRY(cudaMemcpyAsync(d_cand, fill.data(), slots * 8, cudaMemcpyHostToDevice, st));
-    CU_TRY(cudaStreamSynchronize(st));   // `fill` is pageable
+    CUDA_TRY(ctx, cudaMemcpyAsync(d_cand, fill.data(), slots * 8, cudaMemcpyHostToDevice, st));
+    CUDA_TRY(ctx, cudaStreamSynchronize(st));   // `fill` is pageable
   }
   long long valid = 0;
   for (int q = 0; q < n_local; ++q) {
@@ -201,16 +207,16 @@ int obgpu_merge_decoded_distributed(obgpu_ctx *ctx, obgpu_comm *comm, const obgp
     ctx->launches++;
     valid += std::min<int64_t>(S, local_runs[q].n);
   }
-  CU_TRY(cudaMemcpyAsync(d_valid, &valid, 8, cudaMemcpyHostToDevice, st));
+  CUDA_TRY(ctx, cudaMemcpyAsync(d_valid, &valid, 8, cudaMemcpyHostToDevice, st));
   // 2. gather, sort, splitters -- device only
   NCCL_TRY(a.AllGather(d_cand, d_all, slots, ncclInt64, comm->comm, st));
   NCCL_TRY(a.AllReduce(d_valid, d_valid, 1, ncclInt64, ncclSum, comm->comm, st));
   {
     size_t tmp_bytes = 0;
-    cub::DeviceRadixSort::SortKeys(nullptr, tmp_bytes, d_all, d_sorted, (int64_t)(slots * world), 0, 64, st);
-    void *d_tmp = dalloc(tmp_bytes);
-    if (!d_tmp) { cleanup(); return OBGPU_ALLOCATE_MEMORY_FAILED; }
-    CU_TRY(cub::DeviceRadixSort::SortKeys(d_tmp, tmp_bytes, d_all, d_sorted, (int64_t)(slots * world), 0, 64, st));
+    CUDA_TRY(ctx, cub::DeviceRadixSort::SortKeys(nullptr, tmp_bytes, d_all, d_sorted, (int64_t)(slots * world), 0, 64, st));
+    uint8_t *d_tmp;
+    CUDA_TRY(ctx, dalloc(tmp_bytes, d_tmp));
+    CUDA_TRY(ctx, cub::DeviceRadixSort::SortKeys(d_tmp, tmp_bytes, d_all, d_sorted, (int64_t)(slots * world), 0, 64, st));
     ctx->launches += 3;
   }
   if (world > 1) {
@@ -227,13 +233,13 @@ int obgpu_merge_decoded_distributed(obgpu_ctx *ctx, obgpu_comm *comm, const obgp
   NCCL_TRY(a.AllReduce(d_tab, d_tab, (size_t)n_runs_total * world + 2 * (size_t)n_runs_total, ncclInt64, ncclSum, comm->comm, st));
   std::vector<long long> h_tab((size_t)n_runs_total * world + 2 * (size_t)n_runs_total);
   std::vector<int64_t> h_bounds((size_t)std::max(n_local, 1) * (world + 1)), h_split((size_t)std::max(world - 1, 1));
-  CU_TRY(cudaMemcpyAsync(h_tab.data(), d_tab, h_tab.size() * 8, cudaMemcpyDeviceToHost, st));
-  CU_TRY(cudaMemcpyAsync(h_bounds.data(), d_bounds, h_bounds.size() * 8, cudaMemcpyDeviceToHost, st));
-  if (world > 1) CU_TRY(cudaMemcpyAsync(h_split.data(), d_split, (size_t)(world - 1) * 8, cudaMemcpyDeviceToHost, st));
-  CU_TRY(cudaStreamSynchronize(st));   // the one sizing synchronisation
+  CUDA_TRY(ctx, cudaMemcpyAsync(h_tab.data(), d_tab, h_tab.size() * 8, cudaMemcpyDeviceToHost, st));
+  CUDA_TRY(ctx, cudaMemcpyAsync(h_bounds.data(), d_bounds, h_bounds.size() * 8, cudaMemcpyDeviceToHost, st));
+  if (world > 1) CUDA_TRY(ctx, cudaMemcpyAsync(h_split.data(), d_split, (size_t)(world - 1) * 8, cudaMemcpyDeviceToHost, st));
+  CUDA_TRY(ctx, cudaStreamSynchronize(st));   // the one sizing synchronisation
   const long long *h_cnt = h_tab.data(), *h_held = h_cnt + (size_t)n_runs_total * world, *h_owner = h_held + n_runs_total;
   for (int q = 0; q < n_runs_total; ++q)
-    if (h_held[q] != 1) { ctx->err = "every run index must be held by exactly one rank"; cleanup(); return OBGPU_INVALID_ARGUMENT; }
+    if (h_held[q] != 1) { ctx->err = "every run index must be held by exactly one rank"; return OBGPU_INVALID_ARGUMENT; }
   if (splitters_out) for (int j = 0; j + 1 < world; ++j) splitters_out[j] = h_split[(size_t)j];
   // 4. pack + exchange. One buffer per (run, peer): [key | vals x n_cols | more_keys x n_more] int64, then [flag | ext x n_cols] bytes
   const size_t n64 = 1 + (size_t)n_cols + (size_t)n_more_keys;
@@ -267,23 +273,23 @@ int obgpu_merge_decoded_distributed(obgpu_ctx *ctx, obgpu_comm *comm, const obgp
           continue;
         }
         if (n == 0) continue;
-        uint8_t *buf = (uint8_t *)dalloc((size_t)n * row_bytes);
-        if (!buf) { ctx->err = "out of device memory"; cleanup(); return OBGPU_ALLOCATE_MEMORY_FAILED; }
+        uint8_t *buf;
+        CUDA_TRY(ctx, dalloc((size_t)n * row_bytes, buf));
         int64_t *i64 = (int64_t *)buf;
         uint8_t *u8 = buf + (size_t)n * 8 * n64;
-        CU_TRY(cudaMemcpyAsync(i64, src.key + lo, (size_t)n * 8, cudaMemcpyDeviceToDevice, st));
-        for (int c = 0; c < n_cols; ++c) CU_TRY(cudaMemcpyAsync(i64 + (size_t)(1 + c) * n, src.vals[c] + lo, (size_t)n * 8, cudaMemcpyDeviceToDevice, st));
-        for (int c = 0; c < n_more_keys; ++c) CU_TRY(cudaMemcpyAsync(i64 + (size_t)(1 + n_cols + c) * n, src.more_keys[c] + lo, (size_t)n * 8, cudaMemcpyDeviceToDevice, st));
-        if (src.flag) CU_TRY(cudaMemcpyAsync(u8, src.flag + lo, (size_t)n, cudaMemcpyDeviceToDevice, st));
-        else CU_TRY(cudaMemsetAsync(u8, OBGPU_DF_INSERT, (size_t)n, st));
-        for (int c = 0; c < n_cols; ++c) CU_TRY(cudaMemcpyAsync(u8 + (size_t)(1 + c) * n, src.ext[c] + lo, (size_t)n, cudaMemcpyDeviceToDevice, st));
+        CUDA_TRY(ctx, cudaMemcpyAsync(i64, src.key + lo, (size_t)n * 8, cudaMemcpyDeviceToDevice, st));
+        for (int c = 0; c < n_cols; ++c) CUDA_TRY(ctx, cudaMemcpyAsync(i64 + (size_t)(1 + c) * n, src.vals[c] + lo, (size_t)n * 8, cudaMemcpyDeviceToDevice, st));
+        for (int c = 0; c < n_more_keys; ++c) CUDA_TRY(ctx, cudaMemcpyAsync(i64 + (size_t)(1 + n_cols + c) * n, src.more_keys[c] + lo, (size_t)n * 8, cudaMemcpyDeviceToDevice, st));
+        if (src.flag) CUDA_TRY(ctx, cudaMemcpyAsync(u8, src.flag + lo, (size_t)n, cudaMemcpyDeviceToDevice, st));
+        else CUDA_TRY(ctx, cudaMemsetAsync(u8, OBGPU_DF_INSERT, (size_t)n, st));
+        for (int c = 0; c < n_cols; ++c) CUDA_TRY(ctx, cudaMemcpyAsync(u8 + (size_t)(1 + c) * n, src.ext[c] + lo, (size_t)n, cudaMemcpyDeviceToDevice, st));
         sends.push_back(Xfer{buf, (size_t)n * row_bytes, j});
       }
     } else {
       const int64_t n = h_cnt[(size_t)g * world + rank];
       if (n > 0) {
-        uint8_t *buf = (uint8_t *)dalloc((size_t)n * row_bytes);
-        if (!buf) { ctx->err = "out of device memory"; cleanup(); return OBGPU_ALLOCATE_MEMORY_FAILED; }
+        uint8_t *buf;
+        CUDA_TRY(ctx, dalloc((size_t)n * row_bytes, buf));
         const int64_t *i64 = (const int64_t *)buf;
         const uint8_t *u8 = buf + (size_t)n * 8 * n64;
         r.n = n;
@@ -306,11 +312,8 @@ int obgpu_merge_decoded_distributed(obgpu_ctx *ctx, obgpu_comm *comm, const obgp
     NCCL_TRY(a.GroupEnd());
   }
   // 5. local merge of this rank's range (stream ordered after the exchange)
-  const int ret = obgpu_merge_decoded(ctx, runs.data(), n_runs_total, n_cols, default_vals, default_null, out);
-  cleanup();   // stream-ordered frees: the merge kernels that read the buffers are already enqueued
 #undef NCCL_TRY
-#undef CU_TRY
-  return ret;
+  return obgpu_merge_decoded(ctx, runs.data(), n_runs_total, n_cols, default_vals, default_null, out);
 }
 
 }  // extern "C"

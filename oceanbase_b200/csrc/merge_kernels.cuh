@@ -14,6 +14,7 @@
 // HBM-bound: (rowkey, source) pairs are read and written once per pass (16 B per row per pass),
 // payload cells are gathered once.
 #pragma once
+#include <deque>
 #include <functional>
 
 #include <cub/device/device_radix_sort.cuh>
@@ -819,18 +820,16 @@ int obgpu_batch_decode_columns_tagged(obgpu_batch *b, int32_t n_cols, const int3
   }
   obgpu_ctx *ctx = b->ctx;
   cudaSetDevice(ctx->device);
-  int *d_status = nullptr;
-  cudaError_t e = cudaMallocAsync((void **)&d_status, 64, ctx->stream);
-  if (e != cudaSuccess) { ctx->err = cudaGetErrorString(e); return OBGPU_ALLOCATE_MEMORY_FAILED; }
-  cudaMemsetAsync(d_status, 0, 4, ctx->stream);
+  Scratch tmp(ctx);
+  CUDA_TRY(ctx, tmp.alloc(64));
+  int *d_status = tmp.at<int>(0);
+  CUDA_TRY(ctx, cudaMemsetAsync(d_status, 0, 4, ctx->stream));
   mrg::decode_cols_kernel<<<b->n_blocks, 128, 0, ctx->stream>>>(b->d_image, b->d_recs, b->d_plans, (int)b->max_cols, dc,
                                                                 b->d_row_start, d_status);
   ctx->launches++;
   int status = 0;
-  cudaMemcpyAsync(&status, d_status, 4, cudaMemcpyDeviceToHost, ctx->stream);
-  e = cudaStreamSynchronize(ctx->stream);
-  cudaFreeAsync(d_status, ctx->stream);
-  if (e != cudaSuccess) { ctx->err = cudaGetErrorString(e); return OBGPU_ERR_SYS; }
+  CUDA_TRY(ctx, cudaMemcpyAsync(&status, d_status, 4, cudaMemcpyDeviceToHost, ctx->stream));
+  CUDA_TRY(ctx, cudaStreamSynchronize(ctx->stream));
   return check_status(ctx, status);
 }
 
@@ -857,7 +856,8 @@ int obgpu_merge_decoded(obgpu_ctx *ctx, const obgpu_merge_run *runs, int32_t n_r
     N += runs[r].n;
   }
   cudaSetDevice(ctx->device);
-  obgpu_merge_result *res = new (std::nothrow) obgpu_merge_result();
+  std::unique_ptr<obgpu_merge_result> owner(new (std::nothrow) obgpu_merge_result());
+  obgpu_merge_result *res = owner.get();
   if (!res) return OBGPU_ALLOCATE_MEMORY_FAILED;
   res->ctx = ctx;
   res->n_cols = n_cols;
@@ -865,28 +865,27 @@ int obgpu_merge_decoded(obgpu_ctx *ctx, const obgpu_merge_run *runs, int32_t n_r
   const int64_t n_tiles = (N + mrg::kFuseTile - 1) / mrg::kFuseTile;
   res->n_tiles = n_tiles;
   // ---- arena -----------------------------------------------------------------------------------------
-  auto al = [](size_t x) { return (x + 255) & ~(size_t)255; };
-  size_t o = 0;
+  Scratch arena(ctx);
   // single-column rowkeys merge in one pass (bucket_merge_kernel) and need no ping-pong buffers
   const bool bucket_path = n_more == 0 && n_runs >= 2 && n_runs <= mrg::kMaxRuns && N > 0 && getenv("OBGPU_MERGE_PAIRWISE") == nullptr;
-  const size_t o_k0 = o; o += al(bucket_path ? 0 : (size_t)N * 8);
-  const size_t o_s0 = o; o += al(bucket_path ? 0 : (size_t)N * 8);
-  const size_t o_k1 = o; o += al((size_t)N * 8);
-  const size_t o_s1 = o; o += al((size_t)N * 8);
-  const size_t o_emit = o; o += al((size_t)N * (bucket_path ? 2 : 1));   // emit flags, or the emitting heads' ranks inside their bucket
-  const size_t o_stats = o; o += al(64);
+  const size_t o_k0 = arena.take(bucket_path ? 0 : (size_t)N * 8);
+  const size_t o_s0 = arena.take(bucket_path ? 0 : (size_t)N * 8);
+  const size_t o_k1 = arena.take((size_t)N * 8);
+  const size_t o_s1 = arena.take((size_t)N * 8);
+  const size_t o_emit = arena.take((size_t)N * (bucket_path ? 2 : 1));   // emit flags, or the emitting heads' ranks inside their bucket
+  const size_t o_stats = arena.take(64);
   const size_t tbl_entries = (size_t)n_runs * 2 + (size_t)n_runs * n_cols * 2 + (size_t)n_cols * 2 + (size_t)n_runs * n_more + (size_t)n_more;
-  const size_t o_tbl = o; o += al(tbl_entries * 8);
-  const size_t o_def = o; o += al((size_t)n_cols * 9 + 16);
-  const size_t o_pairs = o; o += al(sizeof(mrg::Pair) * (size_t)(n_runs + 1) * 8);
+  const size_t o_tbl = arena.take(tbl_entries * 8);
+  const size_t o_def = arena.take((size_t)n_cols * 9 + 16);
+  const size_t o_pairs = arena.take(sizeof(mrg::Pair) * (size_t)(n_runs + 1) * 8);
   const size_t max_tiles = (size_t)(N / mrg::kTile) + (size_t)n_runs + 2;
-  const size_t o_split = o; o += al((max_tiles + 1) * 8);
-  const size_t o_okey = o; o += al((size_t)N * 8);
+  const size_t o_split = arena.take((max_tiles + 1) * 8);
+  const size_t o_okey = arena.take((size_t)N * 8);
   std::vector<size_t> o_ov((size_t)n_cols), o_on((size_t)n_cols);
-  for (int c = 0; c < n_cols; ++c) { o_ov[(size_t)c] = o; o += al((size_t)N * 8); }
-  for (int c = 0; c < n_cols; ++c) { o_on[(size_t)c] = o; o += al((size_t)N); }
+  for (int c = 0; c < n_cols; ++c) o_ov[(size_t)c] = arena.take((size_t)N * 8);
+  for (int c = 0; c < n_cols; ++c) o_on[(size_t)c] = arena.take((size_t)N);
   std::vector<size_t> o_om((size_t)n_more);
-  for (int c = 0; c < n_more; ++c) { o_om[(size_t)c] = o; o += al((size_t)N * 8); }
+  for (int c = 0; c < n_more; ++c) o_om[(size_t)c] = arena.take((size_t)N * 8);
   // single-pass K-way merge (single-column rowkeys, see bucket_merge_kernel): samples, splitter bounds, bucket offsets
   int bk_chunk = 1;
   while (bk_chunk * 2 * n_runs <= mrg::kBucketMean) bk_chunk *= 2;
@@ -906,24 +905,25 @@ int obgpu_merge_decoded(obgpu_ctx *ctx, const obgpu_merge_run *runs, int32_t n_r
   }
   const int64_t n_buckets = bucket_path ? std::max<int64_t>(1, (n_samples + bk_every - 1) / bk_every) : 0;
   size_t sort_tmp = 0;
-  if (bucket_path) cub::DeviceRadixSort::SortKeys(nullptr, sort_tmp, (const int64_t *)nullptr, (int64_t *)nullptr, n_samples, 0, 64, ctx->stream);
-  const size_t o_smp = o; o += al((size_t)n_samples * 8);
-  const size_t o_sorted = o; o += al((size_t)n_samples * 8);
-  const size_t o_sorttmp = o; o += al(sort_tmp);
-  const size_t o_bounds = o; o += al((size_t)(n_buckets + 1) * (size_t)n_runs * 8);
-  const size_t o_bsize = o; o += al((size_t)(n_buckets + 1) * 4);
-  const size_t o_bout = o; o += al((size_t)(n_buckets + 2) * 8);
+  if (bucket_path)
+    CUDA_TRY(ctx, cub::DeviceRadixSort::SortKeys(nullptr, sort_tmp, (const int64_t *)nullptr, (int64_t *)nullptr, n_samples, 0, 64, ctx->stream));
+  const size_t o_smp = arena.take((size_t)n_samples * 8);
+  const size_t o_sorted = arena.take((size_t)n_samples * 8);
+  const size_t o_sorttmp = arena.take(sort_tmp);
+  const size_t o_bounds = arena.take((size_t)(n_buckets + 1) * (size_t)n_runs * 8);
+  const size_t o_bsize = arena.take((size_t)(n_buckets + 1) * 4);
+  const size_t o_bout = arena.take((size_t)(n_buckets + 2) * 8);
   const size_t n_bchunks = (size_t)((n_buckets + kPrefixChunk - 1) / kPrefixChunk);
-  const size_t o_bchunk = o; o += al((n_bchunks + 1) * 8);
+  const size_t o_bchunk = arena.take((n_bchunks + 1) * 8);
   const int64_t n_units = bucket_path ? n_buckets : n_tiles;   // emit counts / output offsets per bucket (single pass) or per tile
-  const size_t o_cnt = o; o += al(((size_t)n_units + 1) * 4);
-  const size_t o_off = o; o += al(((size_t)n_units + 2) * 8);
+  const size_t o_cnt = arena.take(((size_t)n_units + 1) * 4);
+  const size_t o_off = arena.take(((size_t)n_units + 2) * 8);
   const size_t n_chunks = (size_t)((n_units + kPrefixChunk - 1) / kPrefixChunk);
-  const size_t o_chunk = o; o += al((n_chunks + 1) * 8);
+  const size_t o_chunk = arena.take((n_chunks + 1) * 8);
   if (bucket_path) res->n_tiles = n_units;
-  cudaError_t e = cudaMallocAsync(&res->arena, o + 256, ctx->stream);
-  if (e != cudaSuccess) { ctx->err = cudaGetErrorString(e); delete res; return OBGPU_ALLOCATE_MEMORY_FAILED; }
-  uint8_t *a = (uint8_t *)res->arena;
+  arena.take(256);   // tail slack
+  CUDA_TRY(ctx, arena.alloc());
+  uint8_t *a = arena.p;
   int64_t *k0 = (int64_t *)(a + o_k0), *k1 = (int64_t *)(a + o_k1);
   uint64_t *s0 = (uint64_t *)(a + o_s0), *s1 = (uint64_t *)(a + o_s1);
   uint8_t *emit = a + o_emit;
@@ -932,7 +932,7 @@ int obgpu_merge_decoded(obgpu_ctx *ctx, const obgpu_merge_run *runs, int32_t n_r
   res->d_stats = (unsigned long long *)(a + o_stats);
   res->d_status = (int *)(a + o_stats + 32);
   res->d_out_key = (int64_t *)(a + o_okey);
-  cudaMemsetAsync(a + o_stats, 0, 64, ctx->stream);
+  CUDA_TRY(ctx, cudaMemsetAsync(a + o_stats, 0, 64, ctx->stream));
   // ---- pointer tables (host -> device) ------------------------------------------------------------------
   std::vector<uint64_t> tbl(tbl_entries, 0);
   size_t t = 0;
@@ -995,25 +995,24 @@ int obgpu_merge_decoded(obgpu_ctx *ctx, const obgpu_merge_run *runs, int32_t n_r
   std::vector<size_t> pass_at;
   for (auto &ps : passes) { pass_at.push_back(all_pairs.size()); all_pairs.insert(all_pairs.end(), ps.begin(), ps.end()); }
   // one pinned-free upload: tables, defaults, pairs are small pageable buffers -> synchronous staging is fine
-  cudaMemcpyAsync(d_tbl, tbl.data(), tbl_entries * 8, cudaMemcpyHostToDevice, ctx->stream);
-  cudaMemcpyAsync(a + o_def, defs.data(), defs.size(), cudaMemcpyHostToDevice, ctx->stream);
+  CUDA_TRY(ctx, cudaMemcpyAsync(d_tbl, tbl.data(), tbl_entries * 8, cudaMemcpyHostToDevice, ctx->stream));
+  CUDA_TRY(ctx, cudaMemcpyAsync(a + o_def, defs.data(), defs.size(), cudaMemcpyHostToDevice, ctx->stream));
   if (!all_pairs.empty())
-    cudaMemcpyAsync(a + o_pairs, all_pairs.data(), all_pairs.size() * sizeof(mrg::Pair), cudaMemcpyHostToDevice, ctx->stream);
-  e = cudaStreamSynchronize(ctx->stream);
-  if (e != cudaSuccess) { ctx->err = cudaGetErrorString(e); obgpu_merge_result_free(res); return OBGPU_ERR_SYS; }
+    CUDA_TRY(ctx, cudaMemcpyAsync(a + o_pairs, all_pairs.data(), all_pairs.size() * sizeof(mrg::Pair), cudaMemcpyHostToDevice, ctx->stream));
+  CUDA_TRY(ctx, cudaStreamSynchronize(ctx->stream));
   // ---- launches ----------------------------------------------------------------------------------------------
   std::function<void(const mrg::RunsDev &)> bk_launch;
   if (bucket_path) {
     static bool attr_set = false;   // 63 KB of dynamic shared memory per CTA
     const size_t bk_smem = (size_t)mrg::kBucketCap * 21;
     if (!attr_set) {
-      cudaFuncSetAttribute(mrg::bucket_merge_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bk_smem);
+      CUDA_TRY(ctx, cudaFuncSetAttribute(mrg::bucket_merge_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bk_smem));
       attr_set = true;
     }
     int64_t *smp = (int64_t *)(a + o_smp), *sorted = (int64_t *)(a + o_sorted), *bounds = (int64_t *)(a + o_bounds), *bout = (int64_t *)(a + o_bout);
     uint32_t *bsize = (uint32_t *)(a + o_bsize);
     mrg::bucket_sample_kernel<<<(unsigned)((n_samples + 255) / 256), 256, 0, ctx->stream>>>(br, n_samples, smp);
-    cub::DeviceRadixSort::SortKeys(a + o_sorttmp, sort_tmp, (const int64_t *)smp, sorted, n_samples, 0, 64, ctx->stream);
+    CUDA_TRY(ctx, cub::DeviceRadixSort::SortKeys(a + o_sorttmp, sort_tmp, (const int64_t *)smp, sorted, n_samples, 0, 64, ctx->stream));
     const int64_t nb_threads = (n_buckets + 1) * n_runs;
     mrg::bucket_bounds_kernel<<<(unsigned)((nb_threads + 255) / 256), 256, 0, ctx->stream>>>(br, sorted, bk_every, n_buckets, bounds);
     mrg::bucket_size_kernel<<<(unsigned)((n_buckets + 255) / 256), 256, 0, ctx->stream>>>(bounds, n_runs, n_buckets, bsize, res->d_status);
@@ -1083,12 +1082,12 @@ int obgpu_merge_decoded(obgpu_ctx *ctx, const obgpu_merge_run *runs, int32_t n_r
         res->d_stats);
     ctx->launches += 4;
   } else {
-    cudaMemsetAsync(res->d_tile_off, 0, 16, ctx->stream);
+    CUDA_TRY(ctx, cudaMemsetAsync(res->d_tile_off, 0, 16, ctx->stream));
   }
-  e = cudaGetLastError();
-  if (e != cudaSuccess) { ctx->err = cudaGetErrorString(e); obgpu_merge_result_free(res); return OBGPU_ERR_SYS; }
+  CUDA_TRY(ctx, cudaGetLastError());
   for (int c = 0; c < n_cols; ++c) { res->vals_view.push_back(res->out_vals[(size_t)c]); res->null_view.push_back(res->out_null[(size_t)c]); }
-  *out = res;
+  res->arena = arena.release();
+  *out = owner.release();
   return OBGPU_SUCCESS;
 }
 
@@ -1110,23 +1109,22 @@ int obgpu_merge_runs_keys(obgpu_ctx *ctx, obgpu_batch *const *batches, int32_t n
   for (int r = 0; r < n_runs; ++r)
     if (!batches[r] || batches[r]->ctx != ctx) return OBGPU_INVALID_ARGUMENT;
   cudaSetDevice(ctx->device);
-  std::vector<void *> temps;
-  auto release = [&]() { for (void *t : temps) cudaFreeAsync(t, ctx->stream); };
+  std::deque<Scratch> bufs;   // freed on the stream after the merge kernels are enqueued
   std::vector<obgpu_merge_run> runs((size_t)n_runs);
   std::vector<std::vector<const int64_t *>> vals((size_t)n_runs);
   std::vector<std::vector<const uint8_t *>> exts((size_t)n_runs);
-  int ret = OBGPU_SUCCESS;
-  for (int r = 0; r < n_runs && ret == OBGPU_SUCCESS; ++r) {
+  for (int r = 0; r < n_runs; ++r) {
     obgpu_batch *b = batches[r];
     const int64_t n = b->total_rows;
     const int n_dec = n_rowkey_cols + (flag_col >= 0 ? 1 : 0) + n_cols;
     // one allocation per run: n_dec value arrays, n_dec ext arrays, the narrowed flag bytes
-    void *buf = nullptr;
-    const size_t per = ((size_t)n * 8 + 255) & ~(size_t)255, per_e = ((size_t)n + 255) & ~(size_t)255;
-    cudaError_t e = cudaMallocAsync(&buf, (per + per_e) * (size_t)n_dec + per_e + 256, ctx->stream);
-    if (e != cudaSuccess) { ctx->err = cudaGetErrorString(e); ret = OBGPU_ALLOCATE_MEMORY_FAILED; break; }
-    temps.push_back(buf);
-    uint8_t *base = (uint8_t *)buf;
+    Scratch &buf = bufs.emplace_back(ctx);
+    size_t o_v[mrg::kMaxDecodeCols], o_e[mrg::kMaxDecodeCols];
+    for (int i = 0; i < n_dec; ++i) o_v[i] = buf.take((size_t)n * 8);
+    for (int i = 0; i < n_dec; ++i) o_e[i] = buf.take((size_t)n);
+    const size_t o_flag = buf.take((size_t)n);
+    buf.take(256);   // tail slack
+    CUDA_TRY(ctx, buf.alloc());
     int32_t dcols[mrg::kMaxDecodeCols];
     int64_t *dv[mrg::kMaxDecodeCols];
     uint8_t *de[mrg::kMaxDecodeCols];
@@ -1136,12 +1134,14 @@ int obgpu_merge_runs_keys(obgpu_ctx *ctx, obgpu_batch *const *batches, int32_t n
     for (int c = 0; c < n_cols; ++c) dcols[k++] = cols[c];
     for (int c = 0; c < n_more; ++c) dcols[k++] = rowkey_cols[1 + c];   // remaining rowkey columns last
     for (int i = 0; i < n_dec; ++i) {
-      dv[i] = (int64_t *)(base + per * (size_t)i);
-      de[i] = base + per * (size_t)n_dec + per_e * (size_t)i;
+      dv[i] = buf.at<int64_t>(o_v[i]);
+      de[i] = buf.at<uint8_t>(o_e[i]);
     }
-    uint8_t *flag8 = base + (per + per_e) * (size_t)n_dec;
-    if (n > 0) ret = obgpu_batch_decode_columns_tagged(b, n_dec, dcols, r, dv, de);
-    if (ret != OBGPU_SUCCESS) break;
+    uint8_t *flag8 = buf.at<uint8_t>(o_flag);
+    if (n > 0) {
+      const int ret = obgpu_batch_decode_columns_tagged(b, n_dec, dcols, r, dv, de);
+      if (ret != OBGPU_SUCCESS) return ret;
+    }
     obgpu_merge_run &run = runs[(size_t)r];
     run.n = n;
     run.key = dv[0];
@@ -1165,20 +1165,19 @@ int obgpu_merge_runs_keys(obgpu_ctx *ctx, obgpu_batch *const *batches, int32_t n
     run.more_keys = n_more > 0 ? mores[(size_t)r].data() : nullptr;
     run.n_more_keys = n_more;
   }
-  if (ret == OBGPU_SUCCESS) ret = obgpu_merge_decoded(ctx, runs.data(), n_runs, n_cols, default_vals, default_null, out);
-  if (ret == OBGPU_SUCCESS) {   // string references of run r carry tag r and point into that batch's image
-    for (int r = 0; r < n_runs; ++r) {
-      (*out)->string_images.push_back(batches[r]->d_image);
-      (*out)->string_image_sizes.push_back((uint64_t)batches[r]->image_size);
-    }
-    for (int c = 0; c < n_cols; ++c) {
-      const uint32_t col = (uint32_t)cols[c];
-      const uint8_t t = col < batches[0]->col_types.size() ? batches[0]->col_types[col] : 0xff;
-      (*out)->col_is_string.push_back(t != 0xff && obf::store_class_of(t) == 5);
-    }
+  const int ret = obgpu_merge_decoded(ctx, runs.data(), n_runs, n_cols, default_vals, default_null, out);
+  if (ret != OBGPU_SUCCESS) return ret;
+  // string references of run r carry tag r and point into that batch's image
+  for (int r = 0; r < n_runs; ++r) {
+    (*out)->string_images.push_back(batches[r]->d_image);
+    (*out)->string_image_sizes.push_back((uint64_t)batches[r]->image_size);
   }
-  release();  // stream-ordered: the merge kernels were enqueued before these frees
-  return ret;
+  for (int c = 0; c < n_cols; ++c) {
+    const uint32_t col = (uint32_t)cols[c];
+    const uint8_t t = col < batches[0]->col_types.size() ? batches[0]->col_types[col] : 0xff;
+    (*out)->col_is_string.push_back(t != 0xff && obf::store_class_of(t) == 5);
+  }
+  return OBGPU_SUCCESS;
 }
 
 int obgpu_merge_result_set_string_images(obgpu_merge_result *res, const void *const *dev_images, const int64_t *image_sizes,
@@ -1212,46 +1211,41 @@ int obgpu_merge_result_fetch_strings(obgpu_merge_result *res, int32_t col, int64
   if (!res->col_is_string.empty() && !res->col_is_string[(size_t)col]) { ctx->err = "not a string column"; return OBGPU_INVALID_ARGUMENT; }
   const int64_t n = row_count;
   const int n_chunks = (int)((n + kPrefixChunk - 1) / kPrefixChunk);
-  auto al = [](size_t x) { return (x + 255) & ~(size_t)255; };
-  const size_t o_len = 0, o_off = al((size_t)n * 4), o_chunk = o_off + al(((size_t)n + 1) * 8);
-  const size_t o_img = o_chunk + al(((size_t)n_chunks + 2) * 8), o_isz = o_img + al(res->string_images.size() * 8);
-  const size_t o_st = o_isz + al(res->string_image_sizes.size() * 8);
-  uint8_t *tmp = nullptr;
-  CUDA_TRY(ctx, cudaMallocAsync((void **)&tmp, o_st + 256, ctx->stream));
+  Scratch scratch(ctx);
+  const size_t o_len = scratch.take((size_t)n * 4), o_off = scratch.take(((size_t)n + 1) * 8), o_chunk = scratch.take(((size_t)n_chunks + 2) * 8);
+  const size_t o_img = scratch.take(res->string_images.size() * 8), o_isz = scratch.take(res->string_image_sizes.size() * 8);
+  const size_t o_st = scratch.take(256);
+  CUDA_TRY(ctx, scratch.alloc());
+  uint8_t *tmp = scratch.p;
   const int64_t *refs = res->out_vals[(size_t)col] + row_begin;
   const uint8_t *nulls = res->out_null[(size_t)col] + row_begin;
   int64_t *d_off = (int64_t *)(tmp + o_off);
-  cudaMemsetAsync(tmp + o_st, 0, 4, ctx->stream);
-  cudaMemcpyAsync(tmp + o_img, res->string_images.data(), res->string_images.size() * 8, cudaMemcpyHostToDevice, ctx->stream);
-  cudaMemcpyAsync(tmp + o_isz, res->string_image_sizes.data(), res->string_image_sizes.size() * 8, cudaMemcpyHostToDevice, ctx->stream);
+  CUDA_TRY(ctx, cudaMemsetAsync(tmp + o_st, 0, 4, ctx->stream));
+  CUDA_TRY(ctx, cudaMemcpyAsync(tmp + o_img, res->string_images.data(), res->string_images.size() * 8, cudaMemcpyHostToDevice, ctx->stream));
+  CUDA_TRY(ctx, cudaMemcpyAsync(tmp + o_isz, res->string_image_sizes.data(), res->string_image_sizes.size() * 8, cudaMemcpyHostToDevice, ctx->stream));
   mrg::ref_len_kernel<<<(unsigned)((n + 255) / 256), 256, 0, ctx->stream>>>(refs, nulls, n, (uint32_t *)(tmp + o_len));
   obgpu_prefix_local_kernel<<<n_chunks, 256, 0, ctx->stream>>>((const uint32_t *)(tmp + o_len), (int)n, d_off,
                                                               (unsigned long long *)(tmp + o_chunk));
   obgpu_prefix_fix_kernel<<<n_chunks + 1, 256, 0, ctx->stream>>>((int)n, n_chunks, d_off, (const unsigned long long *)(tmp + o_chunk));
   ctx->launches += 3;
-  cudaMemcpyAsync(host_off, d_off, ((size_t)n + 1) * 8, cudaMemcpyDeviceToHost, ctx->stream);
-  if (host_null) cudaMemcpyAsync(host_null, nulls, (size_t)n, cudaMemcpyDeviceToHost, ctx->stream);
-  cudaError_t e = cudaStreamSynchronize(ctx->stream);
-  if (e != cudaSuccess) { ctx->err = cudaGetErrorString(e); cudaFreeAsync(tmp, ctx->stream); return OBGPU_ERR_SYS; }
+  CUDA_TRY(ctx, cudaMemcpyAsync(host_off, d_off, ((size_t)n + 1) * 8, cudaMemcpyDeviceToHost, ctx->stream));
+  if (host_null) CUDA_TRY(ctx, cudaMemcpyAsync(host_null, nulls, (size_t)n, cudaMemcpyDeviceToHost, ctx->stream));
+  CUDA_TRY(ctx, cudaStreamSynchronize(ctx->stream));
   const int64_t total = host_off[n];
   *heap_bytes = total;
-  if (total > heap_cap || (total > 0 && !host_heap)) { cudaFreeAsync(tmp, ctx->stream); return OBGPU_BUF_NOT_ENOUGH; }
+  if (total > heap_cap || (total > 0 && !host_heap)) return OBGPU_BUF_NOT_ENOUGH;
   int status = 0;
   if (total > 0) {
-    uint8_t *d_heap = nullptr;
-    e = cudaMallocAsync((void **)&d_heap, (size_t)total + 16, ctx->stream);
-    if (e != cudaSuccess) { ctx->err = cudaGetErrorString(e); cudaFreeAsync(tmp, ctx->stream); return OBGPU_ALLOCATE_MEMORY_FAILED; }
+    Scratch heap(ctx);
+    CUDA_TRY(ctx, heap.alloc((size_t)total + 16));
     mrg::ref_gather_kernel<<<(unsigned)((n * 32 + 255) / 256), 256, 0, ctx->stream>>>(
         refs, nulls, n, (const uint8_t *const *)(tmp + o_img), (const uint64_t *)(tmp + o_isz), (int)res->string_images.size(), d_off,
-        d_heap, (int *)(tmp + o_st));
+        heap.p, (int *)(tmp + o_st));
     ctx->launches++;
-    cudaMemcpyAsync(host_heap, d_heap, (size_t)total, cudaMemcpyDeviceToHost, ctx->stream);
-    cudaMemcpyAsync(&status, tmp + o_st, 4, cudaMemcpyDeviceToHost, ctx->stream);
-    e = cudaStreamSynchronize(ctx->stream);
-    cudaFreeAsync(d_heap, ctx->stream);
+    CUDA_TRY(ctx, cudaMemcpyAsync(host_heap, heap.p, (size_t)total, cudaMemcpyDeviceToHost, ctx->stream));
+    CUDA_TRY(ctx, cudaMemcpyAsync(&status, tmp + o_st, 4, cudaMemcpyDeviceToHost, ctx->stream));
+    CUDA_TRY(ctx, cudaStreamSynchronize(ctx->stream));
   }
-  cudaFreeAsync(tmp, ctx->stream);
-  if (e != cudaSuccess) { ctx->err = cudaGetErrorString(e); return OBGPU_ERR_SYS; }
   return check_status(ctx, status);
 }
 
@@ -1270,11 +1264,10 @@ int obgpu_merge_result_info(obgpu_merge_result *res, obgpu_merge_info *info) {
     unsigned long long st[2] = {0, 0};
     int64_t total = 0;
     int status = 0;
-    cudaMemcpyAsync(st, res->d_stats, 16, cudaMemcpyDeviceToHost, ctx->stream);
-    cudaMemcpyAsync(&status, res->d_status, 4, cudaMemcpyDeviceToHost, ctx->stream);
-    cudaMemcpyAsync(&total, res->d_tile_off + res->n_tiles, 8, cudaMemcpyDeviceToHost, ctx->stream);
-    const cudaError_t e = cudaStreamSynchronize(ctx->stream);
-    if (e != cudaSuccess) { ctx->err = cudaGetErrorString(e); return OBGPU_ERR_SYS; }
+    CUDA_TRY(ctx, cudaMemcpyAsync(st, res->d_stats, 16, cudaMemcpyDeviceToHost, ctx->stream));
+    CUDA_TRY(ctx, cudaMemcpyAsync(&status, res->d_status, 4, cudaMemcpyDeviceToHost, ctx->stream));
+    CUDA_TRY(ctx, cudaMemcpyAsync(&total, res->d_tile_off + res->n_tiles, 8, cudaMemcpyDeviceToHost, ctx->stream));
+    CUDA_TRY(ctx, cudaStreamSynchronize(ctx->stream));
     const int ret = check_status(ctx, status);
     if (ret != OBGPU_SUCCESS) return ret;
     res->info.in_rows = res->in_rows;
@@ -1307,13 +1300,12 @@ int obgpu_merge_result_fetch(obgpu_merge_result *res, int32_t col, int64_t row_b
   obgpu_ctx *ctx = res->ctx;
   if (row_count == 0) return OBGPU_SUCCESS;
   const int64_t *src = col == -1 ? res->d_out_key : (col < -1 ? res->out_more[(size_t)(-col - 2)] : res->out_vals[(size_t)col]);
-  if (host_vals) cudaMemcpyAsync(host_vals, src + row_begin, (size_t)row_count * 8, cudaMemcpyDeviceToHost, ctx->stream);
+  if (host_vals) CUDA_TRY(ctx, cudaMemcpyAsync(host_vals, src + row_begin, (size_t)row_count * 8, cudaMemcpyDeviceToHost, ctx->stream));
   if (host_null) {
     if (col < 0) memset(host_null, 0, (size_t)row_count);
-    else cudaMemcpyAsync(host_null, res->out_null[(size_t)col] + row_begin, (size_t)row_count, cudaMemcpyDeviceToHost, ctx->stream);
+    else CUDA_TRY(ctx, cudaMemcpyAsync(host_null, res->out_null[(size_t)col] + row_begin, (size_t)row_count, cudaMemcpyDeviceToHost, ctx->stream));
   }
-  const cudaError_t e = cudaStreamSynchronize(ctx->stream);
-  if (e != cudaSuccess) { ctx->err = cudaGetErrorString(e); return OBGPU_ERR_SYS; }
+  CUDA_TRY(ctx, cudaStreamSynchronize(ctx->stream));
   return OBGPU_SUCCESS;
 }
 

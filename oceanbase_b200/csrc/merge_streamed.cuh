@@ -64,71 +64,68 @@ extern "C" int obgpu_merge_runs_streamed(int device, int32_t n_streams, const ob
       const bool has_lo = i > 0, has_hi = i + 1 < R;
       const int64_t lo = has_lo ? cuts[(size_t)i - 1] : 0, hi = has_hi ? cuts[(size_t)i] : 0;
       std::vector<obgpu_batch *> batches((size_t)n_runs, nullptr);
-      std::vector<void *> bufs;
       std::vector<obgpu_merge_run> mr((size_t)n_runs);
       std::vector<std::vector<const int64_t *>> vptr((size_t)n_runs);
       std::vector<std::vector<const uint8_t *>> eptr((size_t)n_runs);
       obgpu_merge_result *res = nullptr;
-      int64_t *d_cut = nullptr;
-      ret = cudaMallocAsync((void **)&d_cut, 16 * (size_t)n_runs + 16, ctx->stream) == cudaSuccess ? OBGPU_SUCCESS : OBGPU_ALLOCATE_MEMORY_FAILED;
-      std::vector<int64_t> h_cut((size_t)n_runs * 2, 0);
-      for (int r = 0; r < n_runs && ret == OBGPU_SUCCESS; ++r) {
-        const obgpu_stream_run &sr = runs[r];
-        const int64_t *ek = sr.end_keys;
-        const int32_t b0 = has_lo ? (int32_t)(std::upper_bound(ek, ek + sr.n_blocks, lo) - ek) : 0;             // first block whose last key > lo
-        const int32_t b1 = has_hi ? std::min<int32_t>(sr.n_blocks, (int32_t)(std::lower_bound(ek, ek + sr.n_blocks, hi) - ek) + 1) : sr.n_blocks;
-        mr[(size_t)r] = obgpu_merge_run{};
-        vptr[(size_t)r].assign((size_t)std::max(n_cols, 1), nullptr);
-        eptr[(size_t)r].assign((size_t)std::max(n_cols, 1), nullptr);
-        mr[(size_t)r].vals = vptr[(size_t)r].data();
-        mr[(size_t)r].ext = eptr[(size_t)r].data();
-        if (b0 >= b1) continue;
-        const int64_t o0 = sr.offsets[b0], o1 = sr.offsets[b1 - 1] + sr.sizes[b1 - 1];
-        std::vector<int64_t> offs((size_t)(b1 - b0));
-        for (int32_t k = b0; k < b1; ++k) offs[(size_t)(k - b0)] = sr.offsets[k] - o0;
-        ret = obgpu_batch_open(ctx, (const uint8_t *)sr.image + o0, o1 - o0, offs.data(), sr.sizes + b0, b1 - b0, 0, nullptr, &batches[(size_t)r]);
-        if (ret != OBGPU_SUCCESS) break;
-        int64_t rows = 0;
-        obgpu_batch_total_rows(batches[(size_t)r], &rows);
-        std::vector<int32_t> dc;
-        dc.push_back(rowkey_col);
-        if (flag_col >= 0) dc.push_back(flag_col);
-        for (int c = 0; c < n_cols; ++c) dc.push_back(cols[c]);
-        std::vector<int64_t *> dv((size_t)n_dec);
-        std::vector<uint8_t *> de((size_t)n_dec);
-        for (int c = 0; c < n_dec && ret == OBGPU_SUCCESS; ++c) {
-          void *v = nullptr, *e = nullptr;
-          if (cudaMallocAsync(&v, (size_t)rows * 8 + 16, ctx->stream) != cudaSuccess || cudaMallocAsync(&e, (size_t)rows + 16, ctx->stream) != cudaSuccess)
-            ret = OBGPU_ALLOCATE_MEMORY_FAILED;
-          if (v) bufs.push_back(v);
-          if (e) bufs.push_back(e);
-          dv[(size_t)c] = (int64_t *)v;
-          de[(size_t)c] = (uint8_t *)e;
-        }
-        if (ret != OBGPU_SUCCESS) break;
-        ret = obgpu_batch_decode_columns(batches[(size_t)r], n_dec, dc.data(), dv.data(), de.data());
-        if (ret != OBGPU_SUCCESS) break;
-        mstream::cut_kernel<<<1, 1, 0, ctx->stream>>>(dv[0], rows, lo, has_lo ? 1 : 0, hi, has_hi ? 1 : 0, d_cut + 2 * r);
-        ctx->launches++;
-        // the flag column decodes to int64 images: narrow it to the ObDmlFlag byte per row the merge takes
-        uint8_t *flag8 = nullptr;
-        if (flag_col >= 0) {
-          flag8 = de[1];   // the flag column's ext array is not needed (flags are never NULL): reuse it for the narrowed bytes
-          mrg::narrow_flag_kernel<<<(unsigned)((rows + 255) / 256), 256, 0, ctx->stream>>>(dv[1], rows, flag8);
+      Scratch cut(ctx);
+      std::deque<Scratch> bufs;   // the decoded columns of the runs
+      // every run's blocks of the range, opened, decoded and cut to (lo, hi], then merged into res
+      ret = [&]() -> int {
+        CUDA_TRY(ctx, cut.alloc(16 * (size_t)n_runs + 16));
+        int64_t *d_cut = cut.at<int64_t>(0);
+        std::vector<int64_t> h_cut((size_t)n_runs * 2, 0);
+        for (int r = 0; r < n_runs; ++r) {
+          const obgpu_stream_run &sr = runs[r];
+          const int64_t *ek = sr.end_keys;
+          const int32_t b0 = has_lo ? (int32_t)(std::upper_bound(ek, ek + sr.n_blocks, lo) - ek) : 0;             // first block whose last key > lo
+          const int32_t b1 = has_hi ? std::min<int32_t>(sr.n_blocks, (int32_t)(std::lower_bound(ek, ek + sr.n_blocks, hi) - ek) + 1) : sr.n_blocks;
+          mr[(size_t)r] = obgpu_merge_run{};
+          vptr[(size_t)r].assign((size_t)std::max(n_cols, 1), nullptr);
+          eptr[(size_t)r].assign((size_t)std::max(n_cols, 1), nullptr);
+          mr[(size_t)r].vals = vptr[(size_t)r].data();
+          mr[(size_t)r].ext = eptr[(size_t)r].data();
+          if (b0 >= b1) continue;
+          const int64_t o0 = sr.offsets[b0], o1 = sr.offsets[b1 - 1] + sr.sizes[b1 - 1];
+          std::vector<int64_t> offs((size_t)(b1 - b0));
+          for (int32_t k = b0; k < b1; ++k) offs[(size_t)(k - b0)] = sr.offsets[k] - o0;
+          int rc = obgpu_batch_open(ctx, (const uint8_t *)sr.image + o0, o1 - o0, offs.data(), sr.sizes + b0, b1 - b0, 0, nullptr, &batches[(size_t)r]);
+          if (rc != OBGPU_SUCCESS) return rc;
+          int64_t rows = 0;
+          obgpu_batch_total_rows(batches[(size_t)r], &rows);
+          std::vector<int32_t> dc;
+          dc.push_back(rowkey_col);
+          if (flag_col >= 0) dc.push_back(flag_col);
+          for (int c = 0; c < n_cols; ++c) dc.push_back(cols[c]);
+          std::vector<int64_t *> dv((size_t)n_dec);
+          std::vector<uint8_t *> de((size_t)n_dec);
+          for (int c = 0; c < n_dec; ++c) {
+            Scratch &v = bufs.emplace_back(ctx);
+            CUDA_TRY(ctx, v.alloc((size_t)rows * 8 + 16));
+            Scratch &e = bufs.emplace_back(ctx);
+            CUDA_TRY(ctx, e.alloc((size_t)rows + 16));
+            dv[(size_t)c] = v.at<int64_t>(0);
+            de[(size_t)c] = e.p;
+          }
+          rc = obgpu_batch_decode_columns(batches[(size_t)r], n_dec, dc.data(), dv.data(), de.data());
+          if (rc != OBGPU_SUCCESS) return rc;
+          mstream::cut_kernel<<<1, 1, 0, ctx->stream>>>(dv[0], rows, lo, has_lo ? 1 : 0, hi, has_hi ? 1 : 0, d_cut + 2 * r);
           ctx->launches++;
+          // the flag column decodes to int64 images: narrow it to the ObDmlFlag byte per row the merge takes
+          uint8_t *flag8 = nullptr;
+          if (flag_col >= 0) {
+            flag8 = de[1];   // the flag column's ext array is not needed (flags are never NULL): reuse it for the narrowed bytes
+            mrg::narrow_flag_kernel<<<(unsigned)((rows + 255) / 256), 256, 0, ctx->stream>>>(dv[1], rows, flag8);
+            ctx->launches++;
+          }
+          mr[(size_t)r].key = dv[0];
+          mr[(size_t)r].flag = flag8;
+          mr[(size_t)r].n = rows;   // cut below
+          const int first = flag_col >= 0 ? 2 : 1;
+          for (int c = 0; c < n_cols; ++c) { vptr[(size_t)r][(size_t)c] = dv[(size_t)(first + c)]; eptr[(size_t)r][(size_t)c] = de[(size_t)(first + c)]; }
         }
-        mr[(size_t)r].key = dv[0];
-        mr[(size_t)r].flag = flag8;
-        mr[(size_t)r].n = rows;   // cut below
-        const int first = flag_col >= 0 ? 2 : 1;
-        for (int c = 0; c < n_cols; ++c) { vptr[(size_t)r][(size_t)c] = dv[(size_t)(first + c)]; eptr[(size_t)r][(size_t)c] = de[(size_t)(first + c)]; }
-      }
-      if (ret == OBGPU_SUCCESS) {
-        if (cudaMemcpyAsync(h_cut.data(), d_cut, 16 * (size_t)n_runs, cudaMemcpyDeviceToHost, ctx->stream) != cudaSuccess ||
-            cudaStreamSynchronize(ctx->stream) != cudaSuccess)
-          ret = OBGPU_ERR_SYS;
-      }
-      if (ret == OBGPU_SUCCESS) {
+        CUDA_TRY(ctx, cudaMemcpyAsync(h_cut.data(), d_cut, 16 * (size_t)n_runs, cudaMemcpyDeviceToHost, ctx->stream));
+        CUDA_TRY(ctx, cudaStreamSynchronize(ctx->stream));
         for (int r = 0; r < n_runs; ++r) {
           if (!batches[(size_t)r]) { mr[(size_t)r].n = 0; continue; }
           const int64_t r0 = h_cut[(size_t)2 * r], r1 = h_cut[(size_t)2 * r + 1];
@@ -137,8 +134,8 @@ extern "C" int obgpu_merge_runs_streamed(int device, int32_t n_streams, const ob
           if (mr[(size_t)r].flag) mr[(size_t)r].flag += r0;
           for (int c = 0; c < n_cols; ++c) { vptr[(size_t)r][(size_t)c] += r0; eptr[(size_t)r][(size_t)c] += r0; }
         }
-        ret = obgpu_merge_decoded(ctx, mr.data(), n_runs, n_cols, default_vals, default_null, &res);
-      }
+        return obgpu_merge_decoded(ctx, mr.data(), n_runs, n_cols, default_vals, default_null, &res);
+      }();
       obgpu_merge_info info{};
       if (ret == OBGPU_SUCCESS) ret = obgpu_merge_result_info(res, &info);
       // ranges leave in order
@@ -152,8 +149,6 @@ extern "C" int obgpu_merge_runs_streamed(int device, int32_t n_streams, const ob
       }
       cv.notify_all();
       if (res) obgpu_merge_result_free(res);
-      for (void *p : bufs) cudaFreeAsync(p, ctx->stream);
-      if (d_cut) cudaFreeAsync(d_cut, ctx->stream);
       for (obgpu_batch *b : batches) if (b) obgpu_batch_close(b);
       if (ret != OBGPU_SUCCESS) break;
     }

@@ -26,6 +26,7 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <memory>
 #include <new>
 #include <string>
 #include <vector>
@@ -1766,14 +1767,13 @@ __global__ void __launch_bounds__(kThreads) obgpu_bitmap_row_ids_kernel(const ui
 // =================================================================================================
 // Host side
 // =================================================================================================
+// The one way host code handles a CUDA call's result: on failure, ctx->err = "<call>: <error text>" and the enclosing function
+// returns the call's code
 #define CUDA_TRY(ctx, expr)                                                                       \
-  do {                                                                                            \
-    cudaError_t e__ = (expr);                                                                     \
-    if (e__ != cudaSuccess) {                                                                     \
-      (ctx)->err = std::string(#expr) + ": " + cudaGetErrorString(e__);                           \
-      return e__ == cudaErrorMemoryAllocation ? OBGPU_ALLOCATE_MEMORY_FAILED : OBGPU_ERR_SYS;     \
-    }                                                                                             \
-  } while (0)
+  if (const cudaError_t e__ = (expr); e__ != cudaSuccess) {                                       \
+    (ctx)->err = std::string(#expr) + ": " + cudaGetErrorString(e__);                             \
+    return e__ == cudaErrorMemoryAllocation ? OBGPU_ALLOCATE_MEMORY_FAILED : OBGPU_ERR_SYS;       \
+  } else (void)0
 
 #include "skip_index.cuh"
 
@@ -1791,6 +1791,29 @@ struct obgpu_ctx {
   static constexpr int kProfRing = 256;
   cudaEvent_t ev0[kProfRing] = {nullptr}, ev1[kProfRing] = {nullptr};
   int64_t prof_count = 0;
+};
+
+// Device scratch of one host call: slices reserved with take(), then one cudaMallocAsync of their total on the ctx stream.
+// The destructor frees it on the same stream, so any return after work was enqueued is safe: the free is ordered after that
+// work. release() hands the allocation to an owner that outlives the call.
+struct Scratch {
+  obgpu_ctx *ctx;
+  size_t bytes = 0;
+  uint8_t *p = nullptr;
+  explicit Scratch(obgpu_ctx *c) : ctx(c) {}
+  Scratch(const Scratch &) = delete;
+  Scratch &operator=(const Scratch &) = delete;
+  ~Scratch() { if (p) cudaFreeAsync(p, ctx->stream); }
+  // a slice of `n` bytes at an `align`-aligned offset, padded to a multiple of `align` (a power of two)
+  size_t take(size_t n, size_t align = 256) {
+    const size_t o = (bytes + align - 1) & ~(align - 1);
+    bytes = o + ((n + align - 1) & ~(align - 1));
+    return o;
+  }
+  cudaError_t alloc() { return cudaMallocAsync((void **)&p, bytes ? bytes : 16, ctx->stream); }
+  cudaError_t alloc(size_t n) { take(n, 1); return alloc(); }   // an arena of one slice
+  template <class T> T *at(size_t off) const { return reinterpret_cast<T *>(p + off); }
+  void *release() { void *q = p; p = nullptr; return q; }
 };
 
 struct obgpu_batch {
@@ -1851,7 +1874,6 @@ struct obgpu_result {
   obgpu_batch *batch = nullptr;
   obgpu_ctx *ctx = nullptr;
   void *arena = nullptr;
-  size_t arena_bytes = 0;
   int32_t n_proj = 0;
   ResultCol cols[kMaxProj];
   int32_t *d_has_null = nullptr;
@@ -1910,7 +1932,11 @@ int obgpu_ctx_create(int device, obgpu_ctx **out) {
   c->stream = c->own_stream;
   cudaDeviceGetAttribute(&c->max_smem_optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, device);
   cudaDeviceGetAttribute(&c->sm_count, cudaDevAttrMultiProcessorCount, device);
-  cudaMallocHost(&c->h_pinned, 4096);
+  if (cudaMallocHost(&c->h_pinned, 4096) != cudaSuccess) {
+    g_last_global_err = "cudaMallocHost of the pinned staging buffer failed";
+    obgpu_ctx_destroy(c);
+    return OBGPU_ALLOCATE_MEMORY_FAILED;
+  }
   // keep freed result arenas in the stream-ordered pool: steady-state scans do no cudaMalloc
   cudaMemPool_t pool;
   if (cudaDeviceGetDefaultMemPool(&pool, device) == cudaSuccess) {
@@ -2513,14 +2539,6 @@ __global__ void __launch_bounds__(256) obgpu_format_datums_kernel(const void *da
   out12[3 * k + 2] = pack;
 }
 
-struct TempDev {
-  obgpu_ctx *ctx;
-  void *p = nullptr;
-  explicit TempDev(obgpu_ctx *c) : ctx(c) {}
-  cudaError_t alloc(size_t bytes) { return cudaMallocAsync(&p, bytes ? bytes : 16, ctx->stream); }
-  ~TempDev() { if (p) cudaFreeAsync(p, ctx->stream); }
-};
-
 static int check_status(obgpu_ctx *ctx, int status) {
   if (status & ST_CORRUPT) { ctx->err = "corrupt micro block seen on device"; return OBGPU_INVALID_DATA; }
   if (status & ST_UNSUPPORTED) { ctx->err = "column encoding / type not handled by the device path"; return OBGPU_NOT_SUPPORTED; }
@@ -2585,7 +2603,7 @@ static int scan_common(obgpu_batch *b, const obgpu_scan_spec *spec, const obgpu_
   memset(&p, 0, sizeof(p));
   int ret = build_filter(ctx, b, spec->filter, p);
   if (ret != OBGPU_SUCCESS) return ret;
-  obgpu_result *r = new (std::nothrow) obgpu_result();
+  std::unique_ptr<obgpu_result> r(new (std::nothrow) obgpu_result());
   if (!r) return OBGPU_ALLOCATE_MEMORY_FAILED;
   r->batch = b;
   r->ctx = ctx;
@@ -2594,9 +2612,9 @@ static int scan_common(obgpu_batch *b, const obgpu_scan_spec *spec, const obgpu_
   // column types were captured at open time (an SSTable has one schema; 0xff = blocks disagree)
   for (int c = 0; c < spec->n_proj; ++c) {
     const int32_t col = spec->proj_cols[c];
-    if (col < 0 || (uint32_t)col >= b->max_cols) { delete r; return OBGPU_INVALID_ARGUMENT; }
+    if (col < 0 || (uint32_t)col >= b->max_cols) return OBGPU_INVALID_ARGUMENT;
     const int ui = used_index(p, col);
-    if (ui < 0) { delete r; return OBGPU_NOT_SUPPORTED; }
+    if (ui < 0) return OBGPU_NOT_SUPPORTED;
     p.used_in_proj[ui] = 1;
     p.proj_used[c] = (int16_t)ui;
   }
@@ -2613,45 +2631,40 @@ static int scan_common(obgpu_batch *b, const obgpu_scan_spec *spec, const obgpu_
   layout_pipe(b, p, ctx->max_smem_optin);
   if ((int)p.smem_total > ctx->max_smem_optin && !p.pipe_project) {
     ctx->err = "scan working set exceeds shared memory";
-    delete r;
     return OBGPU_NOT_SUPPORTED;
   }
   // ---- result arena: [zeroed region | data] ---------------------------------------------------------
   const int32_t n = b->n_blocks;
-  size_t off = 0;
-  auto take = [&](size_t bytes) { const size_t o = off; off += (bytes + 255) & ~(size_t)255; return o; };
-  const size_t o_misc = take(256 + kMaxProj * 4);  // status, has_null
+  Scratch arena(ctx);
+  const size_t o_misc = arena.take(256 + kMaxProj * 4);  // status, has_null
   size_t o_nulls[kMaxProj];
   const size_t null_bytes = (size_t)((r->cap + 63) / 64) * 8;
-  for (int c = 0; c < spec->n_proj; ++c) o_nulls[c] = take(null_bytes);
-  const size_t zero_bytes = off;
-  const size_t o_counts = take((size_t)n * 4);
-  const size_t o_chunk = take(((size_t)n / kPrefixChunk + 2) * 8);
-  const size_t o_sel = take(((size_t)n + 1) * 8);
-  const size_t o_bm = take((size_t)b->bm_word_off[(size_t)n] * 4 + 4);
-  const size_t o_rid = spec->want_row_ids ? take((size_t)r->cap * 4) : 0;
+  for (int c = 0; c < spec->n_proj; ++c) o_nulls[c] = arena.take(null_bytes);
+  const size_t zero_bytes = arena.bytes;
+  const size_t o_counts = arena.take((size_t)n * 4);
+  const size_t o_chunk = arena.take(((size_t)n / kPrefixChunk + 2) * 8);
+  const size_t o_sel = arena.take(((size_t)n + 1) * 8);
+  const size_t o_bm = arena.take((size_t)b->bm_word_off[(size_t)n] * 4 + 4);
+  const size_t o_rid = spec->want_row_ids ? arena.take((size_t)r->cap * 4) : 0;
   const bool use_skip = b->d_agg != nullptr && p.n_nodes > 0;
-  const size_t o_blk_const = use_skip ? take((size_t)n) : 0;
-  const size_t o_leaf_const = use_skip ? take((size_t)n * (size_t)p.n_nodes) : 0;
+  const size_t o_blk_const = use_skip ? arena.take((size_t)n) : 0;
+  const size_t o_leaf_const = use_skip ? arena.take((size_t)n * (size_t)p.n_nodes) : 0;
   size_t o_data[kMaxProj], o_lens[kMaxProj];
   for (int c = 0; c < spec->n_proj; ++c) {
     const int t = b->col_types[(size_t)spec->proj_cols[c]];
     o_data[c] = 0;
     o_lens[c] = 0;
     const int sc = obf::store_class_of((uint8_t)t);
-    if (sc == 0) { ctx->err = "projected column type not handled by the device path"; delete r; return OBGPU_NOT_SUPPORTED; }
+    if (sc == 0) { ctx->err = "projected column type not handled by the device path"; return OBGPU_NOT_SUPPORTED; }
     r->cols[c].obj_type = t;
     r->cols[c].is_string = sc == 5;
     r->cols[c].elem_len = sc == 5 ? 8 : obf::datum_len_of((uint8_t)t);
-    o_data[c] = take((size_t)r->cap * (size_t)r->cols[c].elem_len);
-    if (sc == 5) o_lens[c] = take((size_t)r->cap * 4);
+    o_data[c] = arena.take((size_t)r->cap * (size_t)r->cols[c].elem_len);
+    if (sc == 5) o_lens[c] = arena.take((size_t)r->cap * 4);
   }
-  r->arena_bytes = off;
-  cudaError_t e = cudaMallocAsync(&r->arena, r->arena_bytes, ctx->stream);
-  if (e != cudaSuccess) { ctx->err = cudaGetErrorString(e); delete r; return OBGPU_ALLOCATE_MEMORY_FAILED; }
-  uint8_t *a = (uint8_t *)r->arena;
-  e = cudaMemsetAsync(a, 0, zero_bytes, ctx->stream);
-  if (e != cudaSuccess) { ctx->err = cudaGetErrorString(e); obgpu_result_free(r); return OBGPU_ERR_SYS; }
+  CUDA_TRY(ctx, arena.alloc());
+  uint8_t *a = arena.p;
+  CUDA_TRY(ctx, cudaMemsetAsync(a, 0, zero_bytes, ctx->stream));
   p.image = b->d_image;
   p.blk_off = b->d_blk_off;
   p.blk_size = b->d_blk_size;
@@ -2703,7 +2716,6 @@ static int scan_common(obgpu_batch *b, const obgpu_scan_spec *spec, const obgpu_
     const uint32_t cw_total = p.cw_bytes * (uint32_t)kWarps;
     if ((int)cw_total > ctx->max_smem_optin) {
       ctx->err = "filter working set exceeds shared memory";
-      obgpu_result_free(r);
       return OBGPU_NOT_SUPPORTED;
     }
     if (p.pipe_count) {
@@ -2743,13 +2755,14 @@ static int scan_common(obgpu_batch *b, const obgpu_scan_spec *spec, const obgpu_
       ctx->launches++;
     }
   }
-  e = cudaGetLastError();
+  const cudaError_t launched = cudaGetLastError();
   if (ctx->profiling) {
     cudaEventRecord(ctx->ev1[pslot], ctx->stream);
     ctx->prof_count++;
   }
-  if (e != cudaSuccess) { ctx->err = cudaGetErrorString(e); obgpu_result_free(r); return OBGPU_ERR_SYS; }
-  *out = r;
+  CUDA_TRY(ctx, launched);
+  r->arena = arena.release();
+  *out = r.release();
   return OBGPU_SUCCESS;
 }
 
@@ -2798,15 +2811,14 @@ int obgpu_batch_skip_index_filter(obgpu_batch *b, const obgpu_filter *filter, ui
   p.plans = b->d_plans;
   p.rows = b->d_rows;
   p.max_cols = (int32_t)b->max_cols;
-  uint8_t *verdicts = nullptr;   // [n block verdicts][n x n_nodes node verdicts]
-  CUDA_TRY(ctx, cudaMallocAsync((void **)&verdicts, (size_t)n * (size_t)(1 + p.n_nodes) + 16, ctx->stream));
+  Scratch tmp(ctx);   // [n block verdicts][n x n_nodes node verdicts]
+  CUDA_TRY(ctx, tmp.alloc((size_t)n * (size_t)(1 + p.n_nodes) + 16));
+  uint8_t *verdicts = tmp.p;
   skipidx::skip_index_kernel<<<(n + 127) / 128, 128, 0, ctx->stream>>>(p, b->d_agg, b->d_agg_off, verdicts, verdicts + n, nullptr);
   ctx->launches++;
-  cudaError_t e = cudaGetLastError();
-  if (e == cudaSuccess) e = cudaMemcpyAsync(block_mask, verdicts, (size_t)n, cudaMemcpyDeviceToHost, ctx->stream);
-  if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->stream);
-  cudaFreeAsync(verdicts, ctx->stream);
-  if (e != cudaSuccess) { ctx->err = cudaGetErrorString(e); return OBGPU_ERR_SYS; }
+  CUDA_TRY(ctx, cudaGetLastError());
+  CUDA_TRY(ctx, cudaMemcpyAsync(block_mask, verdicts, (size_t)n, cudaMemcpyDeviceToHost, ctx->stream));
+  CUDA_TRY(ctx, cudaStreamSynchronize(ctx->stream));
   return OBGPU_SUCCESS;
 }
 
@@ -2895,8 +2907,9 @@ int obgpu_result_aggregate(obgpu_result *r, int32_t kind, int32_t col_a, int32_t
     const int ret = obgpu_result_info_get(r, &info);
     if (ret != OBGPU_SUCCESS) return ret;
   }
-  unsigned long long *d_out = nullptr;
-  CUDA_TRY(ctx, cudaMallocAsync((void **)&d_out, 32, ctx->stream));
+  Scratch tmp(ctx);
+  CUDA_TRY(ctx, tmp.alloc(32));
+  unsigned long long *d_out = tmp.at<unsigned long long>(0);
   CUDA_TRY(ctx, cudaMemsetAsync(d_out, 0, 32, ctx->stream));
   if (kind == OBGPU_AGG_MIN) CUDA_TRY(ctx, cudaMemsetAsync(d_out, 0xff, 8, ctx->stream));
   const int a_sgn = obf::store_class_of((uint8_t)a.obj_type) == 1, b_sgn = obf::store_class_of((uint8_t)b.obj_type) == 1;
@@ -2907,7 +2920,6 @@ int obgpu_result_aggregate(obgpu_result *r, int32_t kind, int32_t col_a, int32_t
   unsigned long long h[2] = {0, 0};
   CUDA_TRY(ctx, cudaMemcpyAsync(h, d_out, 16, cudaMemcpyDeviceToHost, ctx->stream));
   CUDA_TRY(ctx, cudaStreamSynchronize(ctx->stream));
-  cudaFreeAsync(d_out, ctx->stream);
   if ((kind == OBGPU_AGG_MIN || kind == OBGPU_AGG_MAX) && (a_sgn || a.elem_len < 8)) h[0] ^= 1ull << 63;
   out[0] = (int64_t)h[0];
   out[1] = (int64_t)h[1];
@@ -2978,11 +2990,12 @@ int obgpu_result_fetch_datums(obgpu_result *r, int32_t i, int64_t row_begin, int
   obgpu_ctx *ctx = r->ctx;
   cudaSetDevice(ctx->device);
   if (row_count == 0) return OBGPU_SUCCESS;
-  TempDev tmp(ctx);
-  const size_t o_slots = ((size_t)row_count * 12 + 255) & ~(size_t)255;
-  CUDA_TRY(ctx, tmp.alloc(o_slots + (c.is_string ? 0 : (size_t)row_count * 8)));
-  uint8_t *d12 = (uint8_t *)tmp.p;
-  uint64_t *dslots = c.is_string ? nullptr : (uint64_t *)((uint8_t *)tmp.p + o_slots);
+  Scratch tmp(ctx);
+  const size_t o12 = tmp.take((size_t)row_count * 12);
+  const size_t o_slots = c.is_string ? 0 : tmp.take((size_t)row_count * 8);
+  CUDA_TRY(ctx, tmp.alloc());
+  uint8_t *d12 = tmp.at<uint8_t>(o12);
+  uint64_t *dslots = c.is_string ? nullptr : tmp.at<uint64_t>(o_slots);
   obgpu_format_datums_kernel<<<(unsigned)((row_count + 255) / 256), 256, 0, ctx->stream>>>(
       c.data, c.lens, c.nulls, c.elem_len, c.is_string, row_begin, row_count, (uint64_t)(uintptr_t)host_slots, (uint32_t *)d12, dslots);
   ctx->launches++;
@@ -3056,21 +3069,22 @@ int run_filter_block(obgpu_batch *b, int32_t block, const obgpu_filter *f, int64
   if (count == 0) return OBGPU_SUCCESS;
   layout_smem(b, p);
   if ((int)p.smem_total > ctx->max_smem_optin) return OBGPU_NOT_SUPPORTED;
-  TempDev tmp(ctx);
-  CUDA_TRY(ctx, tmp.alloc((size_t)count + 64));
-  uint8_t *d_bytes = (uint8_t *)tmp.p + 64;
+  Scratch tmp(ctx);
+  const size_t o_status = tmp.take(64, 64), o_bytes = tmp.take((size_t)count, 64);
+  CUDA_TRY(ctx, tmp.alloc());
+  uint8_t *d_bytes = tmp.at<uint8_t>(o_bytes);
   CUDA_TRY(ctx, cudaMemsetAsync(tmp.p, 0, 64, ctx->stream));
   p.image = b->d_image;
   p.blk_off = b->d_blk_off;
   p.blk_size = b->d_blk_size;
   p.bm_word_off = b->d_bm_word_off;
   p.n_blocks = b->n_blocks;
-  p.status = (int32_t *)tmp.p;
+  p.status = tmp.at<int32_t>(o_status);
   obgpu_filter_block_kernel<<<1, kThreads, p.smem_total, ctx->stream>>>(p, block, start, count, d_bytes);
   CUDA_TRY(ctx, cudaGetLastError());
   ctx->launches++;
   int32_t *hs = (int32_t *)ctx->h_pinned;
-  CUDA_TRY(ctx, cudaMemcpyAsync(hs, tmp.p, 4, cudaMemcpyDeviceToHost, ctx->stream));
+  CUDA_TRY(ctx, cudaMemcpyAsync(hs, p.status, 4, cudaMemcpyDeviceToHost, ctx->stream));
   CUDA_TRY(ctx, cudaMemcpyAsync(result_bitmap, d_bytes, (size_t)count, cudaMemcpyDeviceToHost, ctx->stream));
   CUDA_TRY(ctx, cudaStreamSynchronize(ctx->stream));
   return check_status(ctx, *hs);
@@ -3095,14 +3109,14 @@ int run_project_block(obgpu_batch *b, int32_t block, int32_t col, const int32_t 
   const size_t el = want_string ? 8 : (size_t)elem_len;
   const int64_t total = vec_offset + row_cap;
   const size_t null_words32 = (size_t)((total + 63) / 64) * 2;
-  size_t off = 256;
-  const size_t o_rid = off; off += ((size_t)row_cap * 4 + 255) & ~(size_t)255;
-  const size_t o_nulls = off; off += (null_words32 * 4 + 255) & ~(size_t)255;
-  const size_t o_data = off; off += ((size_t)total * el + 255) & ~(size_t)255;
-  const size_t o_lens = off; off += want_string ? (((size_t)total * 4 + 255) & ~(size_t)255) : 0;
-  TempDev tmp(ctx);
-  CUDA_TRY(ctx, tmp.alloc(off));
-  uint8_t *a = (uint8_t *)tmp.p;
+  Scratch tmp(ctx);
+  tmp.take(256);   // status, has_null
+  const size_t o_rid = tmp.take((size_t)row_cap * 4);
+  const size_t o_nulls = tmp.take(null_words32 * 4);
+  const size_t o_data = tmp.take((size_t)total * el);
+  const size_t o_lens = want_string ? tmp.take((size_t)total * 4) : 0;
+  CUDA_TRY(ctx, tmp.alloc());
+  uint8_t *a = tmp.p;
   CUDA_TRY(ctx, cudaMemsetAsync(a, 0, o_data, ctx->stream));  // status, has_null, row ids, nulls
   CUDA_TRY(ctx, cudaMemcpyAsync(a + o_rid, row_ids, (size_t)row_cap * 4, cudaMemcpyHostToDevice, ctx->stream));
   // the caller's vector keeps whatever it held in NULL slots / outside the window: seed the device
@@ -3173,10 +3187,11 @@ int obgpu_bitmap_to_row_ids(obgpu_ctx *ctx, const uint8_t *bitmap, int64_t bitma
   const int64_t span = to - *from;
   if (span == 0) { *row_count = 0; return OBGPU_SUCCESS; }
   const int64_t out_n = std::min(limit, span);
-  TempDev tmp(ctx);
-  const size_t o_bytes = 64, o_ids = o_bytes + (((size_t)span + 255) & ~(size_t)255);
-  CUDA_TRY(ctx, tmp.alloc(o_ids + (size_t)out_n * 4));
-  uint8_t *a = (uint8_t *)tmp.p;
+  Scratch tmp(ctx);
+  tmp.take(64, 64);   // count
+  const size_t o_bytes = tmp.take((size_t)span, 64), o_ids = tmp.take((size_t)out_n * 4, 64);
+  CUDA_TRY(ctx, tmp.alloc());
+  uint8_t *a = tmp.p;
   CUDA_TRY(ctx, cudaMemcpyAsync(a + o_bytes, bitmap + *from, (size_t)span, cudaMemcpyHostToDevice, ctx->stream));
   // device bitmap is re-based to *from: ids are (i + *from) - id_offset
   obgpu_bitmap_row_ids_kernel<<<1, kThreads, 0, ctx->stream>>>(a + o_bytes, 0, span, limit, id_offset - *from,

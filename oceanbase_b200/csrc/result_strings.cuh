@@ -66,16 +66,15 @@ __global__ void __launch_bounds__(256) gather_kernel(const uint8_t *__restrict__
   for (int32_t i = lane; i < len; i += 32) dst[i] = src[i];
 }
 
-// device buffer of a pass over n entries: status word, source offsets, lengths, byte offsets (n + 1), prefix chunk totals
+// device buffer of a pass over n entries, reserved in s: status word, source offsets, lengths, byte offsets (n + 1), prefix chunk totals
 struct Layout {
-  size_t o_src, o_len, o_off, o_chunk, total;
-  explicit Layout(int64_t n) {
-    auto al = [](size_t x) { return (x + 255) & ~(size_t)255; };
-    o_src = 256;
-    o_len = o_src + al((size_t)n * 8);
-    o_off = o_len + al((size_t)n * 4);
-    o_chunk = o_off + al(((size_t)n + 1) * 8);
-    total = o_chunk + al(((size_t)(n / kPrefixChunk) + 3) * 8);
+  size_t o_src, o_len, o_off, o_chunk;
+  Layout(Scratch &s, int64_t n) {
+    s.take(256);
+    o_src = s.take((size_t)n * 8);
+    o_len = s.take((size_t)n * 4);
+    o_off = s.take(((size_t)n + 1) * 8);
+    o_chunk = s.take(((size_t)(n / kPrefixChunk) + 3) * 8);
   }
 };
 
@@ -103,16 +102,14 @@ int gather_to_host(obgpu_ctx *ctx, const uint8_t *d_image, const uint64_t *d_src
   *heap_bytes = total;
   if (total > heap_cap || (total > 0 && !host_heap)) return OBGPU_BUF_NOT_ENOUGH;
   if (total == 0) return OBGPU_SUCCESS;
-  uint8_t *d_heap = nullptr;
-  CUDA_TRY(ctx, cudaMallocAsync((void **)&d_heap, (size_t)total + 16, ctx->stream));
-  resstr::gather_kernel<<<(unsigned)((n * 32 + 255) / 256), 256, 0, ctx->stream>>>(d_image, d_src_off, d_lens, n, d_off, d_heap, resstr::Cols{}, 0,
+  Scratch heap(ctx);
+  CUDA_TRY(ctx, heap.alloc((size_t)total + 16));
+  resstr::gather_kernel<<<(unsigned)((n * 32 + 255) / 256), 256, 0, ctx->stream>>>(d_image, d_src_off, d_lens, n, d_off, heap.p, resstr::Cols{}, 0,
                                                                                    n, nullptr);
   ctx->launches++;
-  cudaError_t e = cudaGetLastError();
-  if (e == cudaSuccess) e = cudaMemcpyAsync(host_heap, d_heap, (size_t)total, cudaMemcpyDeviceToHost, ctx->stream);
-  if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->stream);
-  cudaFreeAsync(d_heap, ctx->stream);
-  if (e != cudaSuccess) { ctx->err = cudaGetErrorString(e); return OBGPU_ERR_SYS; }
+  CUDA_TRY(ctx, cudaGetLastError());
+  CUDA_TRY(ctx, cudaMemcpyAsync(host_heap, heap.p, (size_t)total, cudaMemcpyDeviceToHost, ctx->stream));
+  CUDA_TRY(ctx, cudaStreamSynchronize(ctx->stream));
   return OBGPU_SUCCESS;
 }
 
@@ -172,10 +169,10 @@ int obgpu_result_fetch_strings(obgpu_result *r, int32_t i, int64_t row_begin, in
   *heap_bytes = 0;
   if (row_count == 0) return OBGPU_SUCCESS;
   const int64_t n = row_count;
-  const resstr::Layout L(n);
-  TempDev tmp(ctx);
-  CUDA_TRY(ctx, tmp.alloc(L.total));
-  uint8_t *t = (uint8_t *)tmp.p;
+  Scratch tmp(ctx);
+  const resstr::Layout L(tmp, n);
+  CUDA_TRY(ctx, tmp.alloc());
+  uint8_t *t = tmp.p;
   ret = launch_src_off(r, tab, row_begin, n, n, t, L);
   if (ret != OBGPU_SUCCESS) return ret;
   ret = gather_to_host(ctx, r->batch->d_image, (const uint64_t *)(t + L.o_src), (const int32_t *)(t + L.o_len), n, host_heap, heap_cap, host_off,
@@ -202,9 +199,10 @@ int obgpu_result_string_bytes(obgpu_result *r, int32_t n, const int32_t *cols, i
   const int64_t m = (int64_t)n * row_count;
   std::fill(r->str_col_off, r->str_col_off + n + 1, 0);
   if (m > 0) {
-    const resstr::Layout L(m);
-    CUDA_TRY(ctx, cudaMallocAsync(&r->d_str, L.total, ctx->stream));
-    uint8_t *t = (uint8_t *)r->d_str;
+    Scratch str(ctx);
+    const resstr::Layout L(str, m);
+    CUDA_TRY(ctx, str.alloc());
+    uint8_t *t = str.p;
     ret = launch_src_off(r, tab, row_begin, row_count, m, t, L);
     if (ret != OBGPU_SUCCESS) return ret;
     prefix_lens(ctx, (const int32_t *)(t + L.o_len), m, t, L.o_off, L.o_chunk);
@@ -217,6 +215,7 @@ int obgpu_result_string_bytes(obgpu_result *r, int32_t n, const int32_t *cols, i
     CUDA_TRY(ctx, cudaStreamSynchronize(ctx->stream));
     ret = check_status(ctx, st);
     if (ret != OBGPU_SUCCESS) return ret;
+    r->d_str = str.release();
   }
   for (int32_t j = 0; j < n; ++j) {
     bytes[j] = r->str_col_off[j + 1] - r->str_col_off[j];
@@ -247,14 +246,15 @@ int obgpu_result_fetch_string_heap(obgpu_result *r, int32_t n, const int32_t *co
     want_ptrs = want_ptrs || (host_ptrs && host_ptrs[j]);
   }
   cudaSetDevice(ctx->device);
-  const resstr::Layout L(m);
+  Scratch str(ctx);   // only sized: r->d_str has this layout
+  const resstr::Layout L(str, m);
   const uint8_t *t = (const uint8_t *)r->d_str;
   const int64_t total = r->str_col_off[n] - r->str_col_off[0];
-  const size_t heap_room = (size_t)((total + 16 + 7) & ~7ll);   // the pointer table follows the heap, 8-byte aligned
-  TempDev tmp(ctx);
-  CUDA_TRY(ctx, tmp.alloc(heap_room + (want_ptrs ? (size_t)m * 8 : 0)));
-  uint8_t *d_heap = (uint8_t *)tmp.p;
-  uint64_t *d_ptrs = want_ptrs ? (uint64_t *)(d_heap + heap_room) : nullptr;
+  Scratch tmp(ctx);   // the heap, then the pointer table
+  const size_t o_heap = tmp.take((size_t)total + 16, 8), o_ptrs = want_ptrs ? tmp.take((size_t)m * 8, 8) : 0;
+  CUDA_TRY(ctx, tmp.alloc());
+  uint8_t *d_heap = tmp.at<uint8_t>(o_heap);
+  uint64_t *d_ptrs = want_ptrs ? tmp.at<uint64_t>(o_ptrs) : nullptr;
   resstr::gather_kernel<<<(unsigned)((m * 32 + 255) / 256), 256, 0, ctx->stream>>>(
       r->batch->d_image, (const uint64_t *)(t + L.o_src), (const int32_t *)(t + L.o_len), m, (const int64_t *)(t + L.o_off), d_heap, tab,
       row_begin, row_count, d_ptrs);
@@ -301,12 +301,11 @@ int obgpu_project_strings(obgpu_batch *b, int32_t block, int32_t col, const int3
     ptrs[(size_t)k] = (uint64_t)b->offsets[(size_t)block] + cell;   // offset inside the batch's device image
   }
   const int64_t n = row_cap;
-  auto al = [](size_t x) { return (x + 255) & ~(size_t)255; };
-  const size_t o_src = 0, o_len = al((size_t)n * 8), o_off = o_len + al((size_t)n * 4), o_chunk = o_off + al(((size_t)n + 1) * 8);
-  const size_t total = o_chunk + al(((size_t)(n / kPrefixChunk) + 3) * 8);
-  TempDev tmp(ctx);
-  CUDA_TRY(ctx, tmp.alloc(total));
-  uint8_t *t = (uint8_t *)tmp.p;
+  Scratch tmp(ctx);
+  const size_t o_src = tmp.take((size_t)n * 8), o_len = tmp.take((size_t)n * 4), o_off = tmp.take(((size_t)n + 1) * 8);
+  const size_t o_chunk = tmp.take(((size_t)(n / kPrefixChunk) + 3) * 8);
+  CUDA_TRY(ctx, tmp.alloc());
+  uint8_t *t = tmp.p;
   CUDA_TRY(ctx, cudaMemcpyAsync(t + o_src, ptrs.data(), (size_t)n * 8, cudaMemcpyHostToDevice, ctx->stream));
   CUDA_TRY(ctx, cudaMemcpyAsync(t + o_len, lens.data(), (size_t)n * 4, cudaMemcpyHostToDevice, ctx->stream));
   return gather_to_host(ctx, b->d_image, (const uint64_t *)(t + o_src), (const int32_t *)(t + o_len), n, host_heap, heap_cap, host_off, heap_bytes, t,

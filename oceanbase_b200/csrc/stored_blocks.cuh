@@ -225,12 +225,12 @@ static const char *launch_decode(obgpu_ctx *ctx, int32_t compressor, bool blocks
   return malformed;
 }
 
-// The image an open reads on the device. A host image is uploaded to a temporary buffer (tmp, which the caller frees on the ctx
-// stream once the open is enqueued); a device image is read in place and must be 16-byte aligned, else `misaligned` is the error.
-// On failure nothing is left to free.
+// The image an open reads on the device. A host image is uploaded to `copy`, freed on the ctx stream once the open is enqueued;
+// a device image is read in place and must be 16-byte aligned, else `misaligned` is the error.
 struct DeviceImage {
   const uint8_t *d = nullptr;
-  void *tmp = nullptr;
+  Scratch copy;
+  explicit DeviceImage(obgpu_ctx *ctx) : copy(ctx) {}
 };
 static int stage_image(obgpu_ctx *ctx, const void *image, int64_t image_size, int32_t image_on_device, const char *misaligned,
                        DeviceImage &img) {
@@ -242,18 +242,9 @@ static int stage_image(obgpu_ctx *ctx, const void *image, int64_t image_size, in
     img.d = (const uint8_t *)image;
     return OBGPU_SUCCESS;
   }
-  void *tmp = nullptr;
-  if (cudaMallocAsync(&tmp, (size_t)image_size, ctx->stream) != cudaSuccess) {
-    ctx->err = "image copy";
-    return OBGPU_ALLOCATE_MEMORY_FAILED;
-  }
-  if (cudaMemcpyAsync(tmp, image, (size_t)image_size, cudaMemcpyHostToDevice, ctx->stream) != cudaSuccess) {
-    cudaFreeAsync(tmp, ctx->stream);
-    ctx->err = "image copy";
-    return OBGPU_ERR_SYS;
-  }
-  img.d = (const uint8_t *)tmp;
-  img.tmp = tmp;
+  CUDA_TRY(ctx, img.copy.alloc((size_t)image_size));
+  CUDA_TRY(ctx, cudaMemcpyAsync(img.copy.p, image, (size_t)image_size, cudaMemcpyHostToDevice, ctx->stream));
+  img.d = img.copy.p;
   return OBGPU_SUCCESS;
 }
 
@@ -261,80 +252,80 @@ static int stage_image(obgpu_ctx *ctx, const void *image, int64_t image_size, in
 // The one routine behind obgpu_batch_open_macro_blocks and obgpu_batch_open_compressed.
 static int open_stored_blocks(obgpu_ctx *ctx, const uint8_t *d_image, int64_t image_size, const int64_t *d_src, const int64_t *d_zsize,
                               int32_t n, int32_t compressor, obgpu_batch **out) {
-  int ret = OBGPU_SUCCESS;
-  void *d_work = nullptr, *d_tab = nullptr, *d_out = nullptr;
-  auto fail = [&](int code, const char *what) { ctx->err = what; ret = code; };
   std::vector<int64_t> src((size_t)n), zsize((size_t)n), dsize((size_t)n), dst((size_t)n);
   std::vector<int32_t> kind((size_t)n);
-  do {
-    // [dsize i64 x n][kind i32 x n][status i32]
-    if (cudaMallocAsync(&d_work, (size_t)n * 12 + 64, ctx->stream) != cudaSuccess) { fail(OBGPU_ALLOCATE_MEMORY_FAILED, "stored-block survey tables"); break; }
-    int64_t *d_dsize = (int64_t *)d_work;
-    int32_t *d_kind = (int32_t *)(d_dsize + n), *d_status = d_kind + n;
-    cudaMemsetAsync(d_status, 0, 4, ctx->stream);
-    sb::obgpu_stored_survey_kernel<<<(unsigned)((n + 127) / 128), 128, 0, ctx->stream>>>(d_image, d_src, d_zsize, n, compressor, d_dsize,
-                                                                                          d_kind, d_status);
+  Scratch work(ctx);   // survey tables
+  const size_t o_dsize = work.take((size_t)n * 8, 4), o_kind = work.take((size_t)n * 4, 4), o_status = work.take(64, 4);
+  CUDA_TRY(ctx, work.alloc());
+  int64_t *d_dsize = work.at<int64_t>(o_dsize);
+  int32_t *d_kind = work.at<int32_t>(o_kind), *d_status = work.at<int32_t>(o_status);
+  CUDA_TRY(ctx, cudaMemsetAsync(d_status, 0, 4, ctx->stream));
+  sb::obgpu_stored_survey_kernel<<<(unsigned)((n + 127) / 128), 128, 0, ctx->stream>>>(d_image, d_src, d_zsize, n, compressor, d_dsize,
+                                                                                        d_kind, d_status);
+  ctx->launches++;
+  int32_t st = 0;
+  CUDA_TRY(ctx, cudaMemcpyAsync(dsize.data(), d_dsize, (size_t)n * 8, cudaMemcpyDeviceToHost, ctx->stream));
+  CUDA_TRY(ctx, cudaMemcpyAsync(kind.data(), d_kind, (size_t)n * 4, cudaMemcpyDeviceToHost, ctx->stream));
+  CUDA_TRY(ctx, cudaMemcpyAsync(&st, d_status, 4, cudaMemcpyDeviceToHost, ctx->stream));
+  CUDA_TRY(ctx, cudaMemcpyAsync(src.data(), d_src, (size_t)n * 8, cudaMemcpyDeviceToHost, ctx->stream));
+  CUDA_TRY(ctx, cudaMemcpyAsync(zsize.data(), d_zsize, (size_t)n * 8, cudaMemcpyDeviceToHost, ctx->stream));
+  CUDA_TRY(ctx, cudaStreamSynchronize(ctx->stream));
+  if (st != sb::kStOk) {
+    ctx->err = "micro-block header of a stored block is invalid";
+    return OBGPU_INVALID_DATA;
+  }
+  // slots + the two work lists: raw -> realign copy, compressed -> decoder
+  const int64_t out_bytes = (int64_t)slot_layout(dsize.data(), n, dst.data());
+  std::vector<int64_t> raw_tab, lz_tab;   // raw: [src][size][dst], compressed: [src][zsize][dst][dsize]
+  std::vector<int32_t> raw_idx, lz_idx;
+  for (int32_t i = 0; i < n; ++i) (kind[(size_t)i] ? lz_idx : raw_idx).push_back(i);
+  const size_t nr = raw_idx.size(), nz = lz_idx.size();
+  raw_tab.resize(nr * 3);
+  lz_tab.resize(nz * 4);
+  for (size_t k = 0; k < nr; ++k) {
+    const int32_t i = raw_idx[k];
+    raw_tab[k] = src[(size_t)i]; raw_tab[nr + k] = zsize[(size_t)i]; raw_tab[2 * nr + k] = dst[(size_t)i];
+  }
+  for (size_t k = 0; k < nz; ++k) {
+    const int32_t i = lz_idx[k];
+    lz_tab[k] = src[(size_t)i]; lz_tab[nz + k] = zsize[(size_t)i]; lz_tab[2 * nz + k] = dst[(size_t)i]; lz_tab[3 * nz + k] = dsize[(size_t)i];
+  }
+  Scratch decoded(ctx);   // the batch's image once it opens
+  CUDA_TRY(ctx, decoded.alloc((size_t)out_bytes + 64));
+  uint8_t *d_out = decoded.p;
+  CUDA_TRY(ctx, cudaMemsetAsync(d_out + out_bytes, 0, 64, ctx->stream));
+  Scratch tab(ctx);   // [raw work list][compressed work list][per-block status]
+  const size_t o_raw = tab.take(nr * 24, 8), o_lz = tab.take(nz * 32, 8), o_blk_status = tab.take(nz * 4 + 64, 4);
+  CUDA_TRY(ctx, tab.alloc());
+  int64_t *d_raw = tab.at<int64_t>(o_raw), *d_lz = tab.at<int64_t>(o_lz);
+  int32_t *d_blk_status = tab.at<int32_t>(o_blk_status);
+  if (nr) CUDA_TRY(ctx, cudaMemcpyAsync(d_raw, raw_tab.data(), nr * 24, cudaMemcpyHostToDevice, ctx->stream));
+  if (nz) CUDA_TRY(ctx, cudaMemcpyAsync(d_lz, lz_tab.data(), nz * 32, cudaMemcpyHostToDevice, ctx->stream));
+  CUDA_TRY(ctx, cudaMemsetAsync(d_status, 0, 4, ctx->stream));
+  if (nr) {
+    sb::obgpu_macro_realign_kernel<<<(unsigned)nr, sb::kCopyThreads, 0, ctx->stream>>>(d_image, image_size, d_raw, d_raw + nr, d_raw + 2 * nr,
+                                                                                       d_out);
     ctx->launches++;
-    int32_t st = 0;
-    if (cudaMemcpyAsync(dsize.data(), d_dsize, (size_t)n * 8, cudaMemcpyDeviceToHost, ctx->stream) != cudaSuccess ||
-        cudaMemcpyAsync(kind.data(), d_kind, (size_t)n * 4, cudaMemcpyDeviceToHost, ctx->stream) != cudaSuccess ||
-        cudaMemcpyAsync(&st, d_status, 4, cudaMemcpyDeviceToHost, ctx->stream) != cudaSuccess ||
-        cudaMemcpyAsync(src.data(), d_src, (size_t)n * 8, cudaMemcpyDeviceToHost, ctx->stream) != cudaSuccess ||
-        cudaMemcpyAsync(zsize.data(), d_zsize, (size_t)n * 8, cudaMemcpyDeviceToHost, ctx->stream) != cudaSuccess ||
-        cudaStreamSynchronize(ctx->stream) != cudaSuccess) { fail(OBGPU_ERR_SYS, "stored-block survey"); break; }
-    if (st != sb::kStOk) { fail(OBGPU_INVALID_DATA, "micro-block header of a stored block is invalid"); break; }
-    // slots + the two work lists: raw -> realign copy, compressed -> decoder
-    const int64_t out_bytes = (int64_t)slot_layout(dsize.data(), n, dst.data());
-    std::vector<int64_t> raw_tab, lz_tab;   // raw: [src][size][dst], compressed: [src][zsize][dst][dsize]
-    std::vector<int32_t> raw_idx, lz_idx;
-    for (int32_t i = 0; i < n; ++i) (kind[(size_t)i] ? lz_idx : raw_idx).push_back(i);
-    const size_t nr = raw_idx.size(), nz = lz_idx.size();
-    raw_tab.resize(nr * 3);
-    lz_tab.resize(nz * 4);
-    for (size_t k = 0; k < nr; ++k) {
-      const int32_t i = raw_idx[k];
-      raw_tab[k] = src[(size_t)i]; raw_tab[nr + k] = zsize[(size_t)i]; raw_tab[2 * nr + k] = dst[(size_t)i];
-    }
-    for (size_t k = 0; k < nz; ++k) {
-      const int32_t i = lz_idx[k];
-      lz_tab[k] = src[(size_t)i]; lz_tab[nz + k] = zsize[(size_t)i]; lz_tab[2 * nz + k] = dst[(size_t)i]; lz_tab[3 * nz + k] = dsize[(size_t)i];
-    }
-    if (cudaMallocAsync(&d_out, (size_t)out_bytes + 64, ctx->stream) != cudaSuccess) { fail(OBGPU_ALLOCATE_MEMORY_FAILED, "decoded image"); break; }
-    cudaMemsetAsync((uint8_t *)d_out + out_bytes, 0, 64, ctx->stream);
-    const size_t tab_bytes = (nr * 3 + nz * 4) * 8 + nz * 4 + 64;
-    if (cudaMallocAsync(&d_tab, tab_bytes, ctx->stream) != cudaSuccess) { fail(OBGPU_ALLOCATE_MEMORY_FAILED, "stored-block tables"); break; }
-    int64_t *d_raw = (int64_t *)d_tab, *d_lz = d_raw + nr * 3;
-    int32_t *d_blk_status = (int32_t *)(d_lz + nz * 4);
-    if (nr) cudaMemcpyAsync(d_raw, raw_tab.data(), nr * 24, cudaMemcpyHostToDevice, ctx->stream);
-    if (nz) cudaMemcpyAsync(d_lz, lz_tab.data(), nz * 32, cudaMemcpyHostToDevice, ctx->stream);
-    cudaMemsetAsync(d_status, 0, 4, ctx->stream);
-    if (nr) {
-      sb::obgpu_macro_realign_kernel<<<(unsigned)nr, sb::kCopyThreads, 0, ctx->stream>>>(d_image, image_size, d_raw, d_raw + nr, d_raw + 2 * nr,
-                                                                                         (uint8_t *)d_out);
-      ctx->launches++;
-    }
-    const char *malformed = nullptr;
-    if (nz)
-      malformed = launch_decode(ctx, compressor, true, d_image, d_lz, d_lz + nz, (uint8_t *)d_out, d_lz + 2 * nz, d_lz + 3 * nz, (int32_t)nz,
-                                d_blk_status, d_status);
-    // the host tables were copy sources: synchronise before they go out of scope
-    if (cudaGetLastError() != cudaSuccess || cudaMemcpyAsync(&st, d_status, 4, cudaMemcpyDeviceToHost, ctx->stream) != cudaSuccess ||
-        cudaStreamSynchronize(ctx->stream) != cudaSuccess) { fail(OBGPU_ERR_SYS, "stored-block decode"); break; }
-    if (st != sb::kStOk) {
-      fail(OBGPU_INVALID_DATA, st == sb::kStBadChecksum ? "checksum of a compressed micro-block does not match" : malformed);
-      break;
-    }
-    obgpu_batch *b = nullptr;
-    ret = obgpu_batch_open(ctx, d_out, out_bytes, dst.data(), dsize.data(), n, 1, nullptr, &b);
-    if (ret != OBGPU_SUCCESS) break;
-    b->own_image = true;   // the decoded image lives and dies with the batch
-    d_out = nullptr;
-    *out = b;
-  } while (0);
-  if (d_work) cudaFreeAsync(d_work, ctx->stream);
-  if (d_tab) cudaFreeAsync(d_tab, ctx->stream);
-  if (d_out) cudaFreeAsync(d_out, ctx->stream);
-  return ret;
+  }
+  const char *malformed = nullptr;
+  if (nz)
+    malformed = launch_decode(ctx, compressor, true, d_image, d_lz, d_lz + nz, d_out, d_lz + 2 * nz, d_lz + 3 * nz, (int32_t)nz,
+                              d_blk_status, d_status);
+  // the host tables were copy sources: synchronise before they go out of scope
+  CUDA_TRY(ctx, cudaGetLastError());
+  CUDA_TRY(ctx, cudaMemcpyAsync(&st, d_status, 4, cudaMemcpyDeviceToHost, ctx->stream));
+  CUDA_TRY(ctx, cudaStreamSynchronize(ctx->stream));
+  if (st != sb::kStOk) {
+    ctx->err = st == sb::kStBadChecksum ? "checksum of a compressed micro-block does not match" : malformed;
+    return OBGPU_INVALID_DATA;
+  }
+  obgpu_batch *b = nullptr;
+  const int ret = obgpu_batch_open(ctx, d_out, out_bytes, dst.data(), dsize.data(), n, 1, nullptr, &b);
+  if (ret != OBGPU_SUCCESS) return ret;
+  b->own_image = true;   // the decoded image lives and dies with the batch
+  decoded.release();
+  *out = b;
+  return OBGPU_SUCCESS;
 }
 
 // n independent payloads of one codec in device memory (obgpu_lz4_decompress, obgpu_zstd_decompress, obgpu_zlib_decompress)
@@ -344,32 +335,30 @@ static int decompress_streams(obgpu_ctx *ctx, const void *d_in, const int64_t *i
   for (int32_t i = 0; i < n; ++i)
     if (in_off[i] < 0 || in_len[i] < 0 || out_off[i] < 0 || out_len[i] < 0) return OBGPU_INVALID_ARGUMENT;
   cudaSetDevice(ctx->device);
-  void *d_tab = nullptr;
-  int ret = OBGPU_SUCCESS;
   std::vector<int64_t> tab((size_t)n * 4);
   memcpy(tab.data(), in_off, (size_t)n * 8);
   memcpy(tab.data() + n, in_len, (size_t)n * 8);
   memcpy(tab.data() + 2 * (size_t)n, out_off, (size_t)n * 8);
   memcpy(tab.data() + 3 * (size_t)n, out_len, (size_t)n * 8);
-  do {
-    if (cudaMallocAsync(&d_tab, (size_t)n * 36 + 64, ctx->stream) != cudaSuccess) { ctx->err = "stream tables"; ret = OBGPU_ALLOCATE_MEMORY_FAILED; break; }
-    int64_t *d = (int64_t *)d_tab;
-    int32_t *d_st = (int32_t *)(d + 4 * (size_t)n), *d_any = d_st + n;
-    cudaMemcpyAsync(d, tab.data(), (size_t)n * 32, cudaMemcpyHostToDevice, ctx->stream);
-    cudaMemsetAsync(d_any, 0, 4, ctx->stream);
-    const char *malformed = launch_decode(ctx, compressor, false, (const uint8_t *)d_in, d, d + n, (uint8_t *)d_out, d + 2 * n, d + 3 * n, n,
-                                          d_st, d_any);
-    int32_t any = 0;
-    if (cudaGetLastError() != cudaSuccess || cudaMemcpyAsync(status, d_st, (size_t)n * 4, cudaMemcpyDeviceToHost, ctx->stream) != cudaSuccess ||
-        cudaMemcpyAsync(&any, d_any, 4, cudaMemcpyDeviceToHost, ctx->stream) != cudaSuccess ||
-        cudaStreamSynchronize(ctx->stream) != cudaSuccess) { ctx->err = "stream decode"; ret = OBGPU_ERR_SYS; break; }
-    if (any != sb::kStOk) {
-      ctx->err = malformed;
-      ret = OBGPU_INVALID_DATA;
-    }
-  } while (0);
-  if (d_tab) cudaFreeAsync(d_tab, ctx->stream);
-  return ret;
+  Scratch t(ctx);   // [in_off][in_len][out_off][out_len][per-stream status][any status]
+  const size_t o_tab = t.take((size_t)n * 32, 4), o_st = t.take((size_t)n * 4, 4), o_any = t.take(64, 4);
+  CUDA_TRY(ctx, t.alloc());
+  int64_t *d = t.at<int64_t>(o_tab);
+  int32_t *d_st = t.at<int32_t>(o_st), *d_any = t.at<int32_t>(o_any);
+  CUDA_TRY(ctx, cudaMemcpyAsync(d, tab.data(), (size_t)n * 32, cudaMemcpyHostToDevice, ctx->stream));
+  CUDA_TRY(ctx, cudaMemsetAsync(d_any, 0, 4, ctx->stream));
+  const char *malformed = launch_decode(ctx, compressor, false, (const uint8_t *)d_in, d, d + n, (uint8_t *)d_out, d + 2 * n, d + 3 * n, n,
+                                        d_st, d_any);
+  int32_t any = 0;
+  CUDA_TRY(ctx, cudaGetLastError());
+  CUDA_TRY(ctx, cudaMemcpyAsync(status, d_st, (size_t)n * 4, cudaMemcpyDeviceToHost, ctx->stream));
+  CUDA_TRY(ctx, cudaMemcpyAsync(&any, d_any, 4, cudaMemcpyDeviceToHost, ctx->stream));
+  CUDA_TRY(ctx, cudaStreamSynchronize(ctx->stream));
+  if (any != sb::kStOk) {
+    ctx->err = malformed;
+    return OBGPU_INVALID_DATA;
+  }
+  return OBGPU_SUCCESS;
 }
 
 extern "C" {
@@ -387,24 +376,16 @@ int obgpu_batch_open_compressed(obgpu_ctx *ctx, const void *image, int64_t image
       return OBGPU_INVALID_ARGUMENT;
     }
   cudaSetDevice(ctx->device);
-  DeviceImage img;
-  int ret = stage_image(ctx, image, image_size, image_on_device, "a device-resident image must be 16-byte aligned", img);
+  DeviceImage img(ctx);
+  const int ret = stage_image(ctx, image, image_size, image_on_device, "a device-resident image must be 16-byte aligned", img);
   if (ret != OBGPU_SUCCESS) return ret;
-  void *d_tabs = nullptr;
-  do {
-    if (cudaMallocAsync(&d_tabs, (size_t)n_blocks * 16, ctx->stream) != cudaSuccess) { ctx->err = "block tables"; ret = OBGPU_ALLOCATE_MEMORY_FAILED; break; }
-    int64_t *d_src = (int64_t *)d_tabs, *d_zs = d_src + n_blocks;
-    if (cudaMemcpyAsync(d_src, offsets, (size_t)n_blocks * 8, cudaMemcpyHostToDevice, ctx->stream) != cudaSuccess ||
-        cudaMemcpyAsync(d_zs, sizes, (size_t)n_blocks * 8, cudaMemcpyHostToDevice, ctx->stream) != cudaSuccess) {
-      ctx->err = "block tables";
-      ret = OBGPU_ERR_SYS;
-      break;
-    }
-    ret = open_stored_blocks(ctx, img.d, image_size, d_src, d_zs, n_blocks, compressor_type, out);
-  } while (0);
-  if (d_tabs) cudaFreeAsync(d_tabs, ctx->stream);
-  if (img.tmp) cudaFreeAsync(img.tmp, ctx->stream);
-  return ret;
+  Scratch tabs(ctx);   // [src][zsize]
+  const size_t o_src = tabs.take((size_t)n_blocks * 8, 8), o_zs = tabs.take((size_t)n_blocks * 8, 8);
+  CUDA_TRY(ctx, tabs.alloc());
+  int64_t *d_src = tabs.at<int64_t>(o_src), *d_zs = tabs.at<int64_t>(o_zs);
+  CUDA_TRY(ctx, cudaMemcpyAsync(d_src, offsets, (size_t)n_blocks * 8, cudaMemcpyHostToDevice, ctx->stream));
+  CUDA_TRY(ctx, cudaMemcpyAsync(d_zs, sizes, (size_t)n_blocks * 8, cudaMemcpyHostToDevice, ctx->stream));
+  return open_stored_blocks(ctx, img.d, image_size, d_src, d_zs, n_blocks, compressor_type, out);
 }
 
 int obgpu_batch_device_image(const obgpu_batch *batch, const void **image, int64_t *image_size) {

@@ -398,70 +398,59 @@ extern "C" int obgpu_compress_blocks(obgpu_ctx *ctx, const void *d_image, const 
   cudaSetDevice(ctx->device);
   const int64_t n = n_blocks;
   const int n_chunks = (int)((n + kPrefixChunk - 1) / kPrefixChunk);
-  int ret = OBGPU_SUCCESS;
-  void *d_work = nullptr, *d_stage = nullptr, *d_seqs = nullptr;
-  auto fail = [&](int code, const char *what) { ctx->err = what; ret = code; };
-  do {
-    // [Work][stage_off i64 x (n + 1)][dst_off i64 x (n + 1)][chunk totals u64 x n_chunks][cnt u32 x n][stored u32 x n]
-    const size_t bytes = 64 + (size_t)(n + 1) * 16 + (size_t)n_chunks * 8 + (size_t)n * 8;
-    if (cudaMallocAsync(&d_work, bytes, ctx->stream) != cudaSuccess) { fail(OBGPU_ALLOCATE_MEMORY_FAILED, "compress tables"); break; }
-    sc::Work *w = (sc::Work *)d_work;
-    int64_t *stage_off = (int64_t *)((uint8_t *)d_work + 64), *dst_off = stage_off + (n + 1);
-    unsigned long long *chunk_tot = (unsigned long long *)(dst_off + (n + 1));
-    uint32_t *cnt = (uint32_t *)(chunk_tot + n_chunks), *stored = cnt + n;
-    cudaMemsetAsync(w, 0, sizeof(sc::Work), ctx->stream);
-    const unsigned grid = (unsigned)((n + 255) / 256);
-    sc::obgpu_compress_survey_kernel<<<grid, 256, 0, ctx->stream>>>((const uint8_t *)d_image, d_offsets, d_sizes, n_blocks, align, cnt, w);
-    ctx->launches++;
-    sc::Work h{};
-    if (cudaMemcpyAsync(&h, w, sizeof(h), cudaMemcpyDeviceToHost, ctx->stream) != cudaSuccess ||
-        cudaStreamSynchronize(ctx->stream) != cudaSuccess) { fail(OBGPU_ERR_SYS, "compress survey"); break; }
-    if (h.verdict & sc::kBadArg) { fail(OBGPU_INVALID_ARGUMENT, "block offsets must be non-negative multiples of 16"); break; }
-    if (h.verdict & sc::kBadData) { fail(OBGPU_INVALID_DATA, "a block to compress is not a plain, well-framed micro-block"); break; }
-    if (h.verdict & sc::kTooLarge) { fail(OBGPU_NOT_SUPPORTED, "a block to compress is larger than 0x7f000000 bytes"); break; }
-    if (!d_out) {
-      *out_size = (int64_t)h.cap;
-      break;
-    }
-    if (out_cap < (int64_t)h.cap) { fail(OBGPU_BUF_NOT_ENOUGH, "output capacity below the sum of the aligned block sizes"); break; }
-    // staging slots for the compressed payloads
-    obgpu_prefix_local_kernel<<<n_chunks, 256, 0, ctx->stream>>>(cnt, n_blocks, stage_off, chunk_tot);
-    obgpu_prefix_fix_kernel<<<n_chunks + 1, 256, 0, ctx->stream>>>(n_blocks, n_chunks, stage_off, chunk_tot);
-    ctx->launches += 2;
-    const bool packs = compressor != OBGPU_COMPRESSOR_NONE;
-    if (packs && cudaMallocAsync(&d_stage, (size_t)h.stage + 16, ctx->stream) != cudaSuccess) { fail(OBGPU_ALLOCATE_MEMORY_FAILED, "compress staging"); break; }
-    const int ctas = (int)std::min<int64_t>(n, std::max(ctx->sm_count, 1));
-    if (compressor == OBGPU_COMPRESSOR_ZSTD_1_3_8 &&
-        cudaMallocAsync(&d_seqs, (size_t)ctas * (obz::kZstdBlock / 4) * sizeof(obz::Seq), ctx->stream) != cudaSuccess) {
-      fail(OBGPU_ALLOCATE_MEMORY_FAILED, "compress sequence lists");
-      break;
-    }
-    decltype(&sc::obgpu_compress_match_kernel<OBGPU_COMPRESSOR_NONE>) match;
-    switch (compressor) {
-      case OBGPU_COMPRESSOR_LZ4: case OBGPU_COMPRESSOR_LZ4_1_9_1: match = sc::obgpu_compress_match_kernel<OBGPU_COMPRESSOR_LZ4>; break;
-      case OBGPU_COMPRESSOR_ZSTD_1_3_8: match = sc::obgpu_compress_match_kernel<OBGPU_COMPRESSOR_ZSTD_1_3_8>; break;
-      default: match = sc::obgpu_compress_match_kernel<OBGPU_COMPRESSOR_NONE>; break;
-    }
-    const int smem = packs ? (int)sizeof(sc::MatchSmem) : 0;
-    if (packs && cudaFuncSetAttribute((const void *)match, cudaFuncAttributeMaxDynamicSharedMemorySize, smem) != cudaSuccess) {
-      fail(OBGPU_ERR_SYS, "compress match kernel shared memory");
-      break;
-    }
-    match<<<(unsigned)ctas, 32, smem, ctx->stream>>>((const uint8_t *)d_image, d_offsets, d_sizes, n_blocks, stage_off, (uint8_t *)d_stage,
-                                                     (obz::Seq *)d_seqs, stored, w);
-    sc::obgpu_compress_align_kernel<<<grid, 256, 0, ctx->stream>>>(stored, n_blocks, (uint32_t)align, cnt);
-    obgpu_prefix_local_kernel<<<n_chunks, 256, 0, ctx->stream>>>(cnt, n_blocks, dst_off, chunk_tot);
-    obgpu_prefix_fix_kernel<<<n_chunks + 1, 256, 0, ctx->stream>>>(n_blocks, n_chunks, dst_off, chunk_tot);
-    sc::obgpu_compress_frame_kernel<<<(unsigned)n, sc::kFrameThreads, 0, ctx->stream>>>(
-        (const uint8_t *)d_image, d_offsets, d_sizes, stage_off, (const uint8_t *)d_stage, stored, dst_off, align, (uint8_t *)d_out,
-        d_out_offsets, d_out_sizes, w);
-    ctx->launches += 5;
-    if (cudaGetLastError() != cudaSuccess || cudaMemcpyAsync(&h, w, sizeof(h), cudaMemcpyDeviceToHost, ctx->stream) != cudaSuccess ||
-        cudaStreamSynchronize(ctx->stream) != cudaSuccess) { fail(OBGPU_ERR_SYS, "device compress"); break; }
-    *out_size = (int64_t)h.end;
-  } while (0);
-  if (d_work) cudaFreeAsync(d_work, ctx->stream);
-  if (d_stage) cudaFreeAsync(d_stage, ctx->stream);
-  if (d_seqs) cudaFreeAsync(d_seqs, ctx->stream);
-  return ret;
+  // [Work][stage_off i64 x (n + 1)][dst_off i64 x (n + 1)][chunk totals u64 x n_chunks][cnt u32 x n][stored u32 x n]
+  Scratch work(ctx);
+  const size_t o_w = work.take(64, 8), o_stage_off = work.take((size_t)(n + 1) * 8, 8), o_dst_off = work.take((size_t)(n + 1) * 8, 8);
+  const size_t o_chunk = work.take((size_t)n_chunks * 8, 8), o_cnt = work.take((size_t)n * 4, 4), o_stored = work.take((size_t)n * 4, 4);
+  CUDA_TRY(ctx, work.alloc());
+  sc::Work *w = work.at<sc::Work>(o_w);
+  int64_t *stage_off = work.at<int64_t>(o_stage_off), *dst_off = work.at<int64_t>(o_dst_off);
+  unsigned long long *chunk_tot = work.at<unsigned long long>(o_chunk);
+  uint32_t *cnt = work.at<uint32_t>(o_cnt), *stored = work.at<uint32_t>(o_stored);
+  CUDA_TRY(ctx, cudaMemsetAsync(w, 0, sizeof(sc::Work), ctx->stream));
+  const unsigned grid = (unsigned)((n + 255) / 256);
+  sc::obgpu_compress_survey_kernel<<<grid, 256, 0, ctx->stream>>>((const uint8_t *)d_image, d_offsets, d_sizes, n_blocks, align, cnt, w);
+  ctx->launches++;
+  sc::Work h{};
+  CUDA_TRY(ctx, cudaMemcpyAsync(&h, w, sizeof(h), cudaMemcpyDeviceToHost, ctx->stream));
+  CUDA_TRY(ctx, cudaStreamSynchronize(ctx->stream));
+  if (h.verdict & sc::kBadArg) { ctx->err = "block offsets must be non-negative multiples of 16"; return OBGPU_INVALID_ARGUMENT; }
+  if (h.verdict & sc::kBadData) { ctx->err = "a block to compress is not a plain, well-framed micro-block"; return OBGPU_INVALID_DATA; }
+  if (h.verdict & sc::kTooLarge) { ctx->err = "a block to compress is larger than 0x7f000000 bytes"; return OBGPU_NOT_SUPPORTED; }
+  if (!d_out) {
+    *out_size = (int64_t)h.cap;
+    return OBGPU_SUCCESS;
+  }
+  if (out_cap < (int64_t)h.cap) { ctx->err = "output capacity below the sum of the aligned block sizes"; return OBGPU_BUF_NOT_ENOUGH; }
+  // staging slots for the compressed payloads
+  obgpu_prefix_local_kernel<<<n_chunks, 256, 0, ctx->stream>>>(cnt, n_blocks, stage_off, chunk_tot);
+  obgpu_prefix_fix_kernel<<<n_chunks + 1, 256, 0, ctx->stream>>>(n_blocks, n_chunks, stage_off, chunk_tot);
+  ctx->launches += 2;
+  const bool packs = compressor != OBGPU_COMPRESSOR_NONE;
+  Scratch stage(ctx), seqs(ctx);
+  if (packs) CUDA_TRY(ctx, stage.alloc((size_t)h.stage + 16));
+  const int ctas = (int)std::min<int64_t>(n, std::max(ctx->sm_count, 1));
+  if (compressor == OBGPU_COMPRESSOR_ZSTD_1_3_8) CUDA_TRY(ctx, seqs.alloc((size_t)ctas * (obz::kZstdBlock / 4) * sizeof(obz::Seq)));
+  decltype(&sc::obgpu_compress_match_kernel<OBGPU_COMPRESSOR_NONE>) match;
+  switch (compressor) {
+    case OBGPU_COMPRESSOR_LZ4: case OBGPU_COMPRESSOR_LZ4_1_9_1: match = sc::obgpu_compress_match_kernel<OBGPU_COMPRESSOR_LZ4>; break;
+    case OBGPU_COMPRESSOR_ZSTD_1_3_8: match = sc::obgpu_compress_match_kernel<OBGPU_COMPRESSOR_ZSTD_1_3_8>; break;
+    default: match = sc::obgpu_compress_match_kernel<OBGPU_COMPRESSOR_NONE>; break;
+  }
+  const int smem = packs ? (int)sizeof(sc::MatchSmem) : 0;
+  if (packs) CUDA_TRY(ctx, cudaFuncSetAttribute((const void *)match, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+  match<<<(unsigned)ctas, 32, smem, ctx->stream>>>((const uint8_t *)d_image, d_offsets, d_sizes, n_blocks, stage_off, stage.p,
+                                                   seqs.at<obz::Seq>(0), stored, w);
+  sc::obgpu_compress_align_kernel<<<grid, 256, 0, ctx->stream>>>(stored, n_blocks, (uint32_t)align, cnt);
+  obgpu_prefix_local_kernel<<<n_chunks, 256, 0, ctx->stream>>>(cnt, n_blocks, dst_off, chunk_tot);
+  obgpu_prefix_fix_kernel<<<n_chunks + 1, 256, 0, ctx->stream>>>(n_blocks, n_chunks, dst_off, chunk_tot);
+  sc::obgpu_compress_frame_kernel<<<(unsigned)n, sc::kFrameThreads, 0, ctx->stream>>>(
+      (const uint8_t *)d_image, d_offsets, d_sizes, stage_off, stage.p, stored, dst_off, align, (uint8_t *)d_out,
+      d_out_offsets, d_out_sizes, w);
+  ctx->launches += 5;
+  CUDA_TRY(ctx, cudaGetLastError());
+  CUDA_TRY(ctx, cudaMemcpyAsync(&h, w, sizeof(h), cudaMemcpyDeviceToHost, ctx->stream));
+  CUDA_TRY(ctx, cudaStreamSynchronize(ctx->stream));
+  *out_size = (int64_t)h.end;
+  return OBGPU_SUCCESS;
 }
