@@ -207,6 +207,29 @@ int obgpu_encode_columns_ex(obgpu_ctx *ctx, const obgpu_encode_col *cols, const 
 int obgpu_merge_result_encode_ex(obgpu_merge_result *res, const int32_t *result_cols, const int32_t *obj_types,
                                  const int32_t *encodings, int32_t n_cols, int32_t rowkey_col_cnt, int64_t rows_per_block,
                                  int32_t align, obgpu_encoded **out);
+/* The same for a table whose row store is CS_ENCODING_ROW_STORE (column groups of a column-store table):
+ *   storage/blocksstable/cs_encoding/ob_micro_block_cs_encoder.cpp:1394-1488   ObMicroBlockCSEncoder::build_block (CS layout:
+ *                                                   all-column header, column headers, column metas + streams, stream offsets)
+ *   cs_encoding/ob_micro_block_cs_encoder.cpp:2289-2375   choose_encoder_for_integer_ (OBGPU_ENC_CS_AUTO, per micro-block)
+ *   cs_encoding/ob_integer_column_encoder.cpp:177-314     ObIntegerColumnEncoder (base, NULL replacement or NULL bitmap, estimate)
+ *   cs_encoding/ob_int_dict_column_encoder.cpp:262-279    ObIntDictColumnEncoder (sorted dictionary stream, estimate)
+ *   cs_encoding/ob_dict_column_encoder.cpp:144-189        ObDictColumnEncoder::try_const_encoding_ref_ / do_store_dict_ref_
+ *   cs_encoding/ob_stream_encoding_struct.cpp:101-190     ObIntegerStreamMeta
+ * encodings[i]: OBGPU_ENC_CS_INTEGER / CS_INT_DICT / CS_AUTO; NULL: every column CS_INTEGER. Same handle as the PAX
+ * encoder: obgpu_encoded_get_info / fetch / device_image / column_checksums / obgpu_compress_blocks work unchanged. The
+ * blocks equal obgpu_writer_encode_table byte for byte for the same rows with the same per-column encodings while the
+ * writer's CS stream mode is 1 (obgpu_writer_set_cs_stream_encoding, RAW streams, its default): the device always writes
+ * RAW integer streams, whatever that process-wide mode is. No block is left to the host writer (n_host_blocks is 0).
+ * byte_packing_only is ignored (the CS writer does not read it). OBGPU_NOT_SUPPORTED before any launch: a PAX encoding,
+ * OBGPU_ENC_CS_STRING / CS_STR_DICT, a string obj_type, more than 64 columns, or a rows_per_block whose block does not fit
+ * one CTA's shared memory (CS_INT_DICT / CS_AUTO columns need more of it). Bad pointers and sizes: OBGPU_INVALID_ARGUMENT,
+ * as for obgpu_encode_columns_ex. */
+int obgpu_encode_columns_cs(obgpu_ctx *ctx, const obgpu_encode_col *cols, const int32_t *encodings, int32_t n_cols,
+                            int32_t rowkey_col_cnt, int64_t total_rows, int64_t rows_per_block, int32_t align,
+                            obgpu_encoded **out);
+int obgpu_merge_result_encode_cs(obgpu_merge_result *res, const int32_t *result_cols, const int32_t *obj_types,
+                                 const int32_t *encodings, int32_t n_cols, int32_t rowkey_col_cnt, int64_t rows_per_block,
+                                 int32_t align, obgpu_encoded **out);
 typedef struct obgpu_encoded_info {
   int64_t image_size;    /* bytes of the image (aligned block slots)          */
   int64_t total_rows;

@@ -178,10 +178,12 @@ int ObGpuPartitionMajorMerger::write_column_groups(const std::vector<ObGpuColumn
   std::vector<obgpu_encoded *> enc(groups.size(), nullptr);
   for (size_t g = 0; OB_SUCCESS == ret && g < groups.size(); ++g) {
     const ObGpuColumnGroup &cg = groups[g];
-    if (cg.cols_.empty() || cg.cols_.size() != cg.obj_types_.size() || (!cg.encodings_.empty() && cg.encodings_.size() != cg.cols_.size()))
+    if (cg.cols_.empty() || cg.cols_.size() != cg.obj_types_.size() || (!cg.encodings_.empty() && cg.encodings_.size() != cg.cols_.size()) ||
+        (cg.row_store_type_ != OB_GPU_ENCODING_ROW_STORE && cg.row_store_type_ != OB_GPU_CS_ENCODING_ROW_STORE))
       ret = OB_INVALID_ARGUMENT;
-    else ret = obgpu_merge_result_encode_ex(result_, cg.cols_.data(), cg.obj_types_.data(), cg.encodings_.empty() ? nullptr : cg.encodings_.data(),
-                                            (int32_t)cg.cols_.size(), cg.rowkey_col_cnt_, rows_per_block, align, &enc[g]);
+    else ret = (cg.row_store_type_ == OB_GPU_CS_ENCODING_ROW_STORE ? obgpu_merge_result_encode_cs : obgpu_merge_result_encode_ex)(
+        result_, cg.cols_.data(), cg.obj_types_.data(), cg.encodings_.empty() ? nullptr : cg.encodings_.data(), (int32_t)cg.cols_.size(),
+        cg.rowkey_col_cnt_, rows_per_block, align, &enc[g]);
   }
   for (size_t g = 0; OB_SUCCESS == ret && g < groups.size(); ++g) {
     const ObGpuColumnGroup &cg = groups[g];

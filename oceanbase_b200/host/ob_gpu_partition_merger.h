@@ -50,13 +50,21 @@ struct ObGpuMergedRows {
   std::vector<std::vector<int64_t>> offsets_;
 };
 
+// common::ObRowStoreType (deps/oblib/src/common/ob_store_format.h:31-40) of the micro-blocks a column group is written as
+enum ObGpuRowStoreType : int32_t { OB_GPU_ENCODING_ROW_STORE = 1, OB_GPU_CS_ENCODING_ROW_STORE = 3 };
+
 // One column group of a column-oriented merge (ObStorageColumnGroupSchema): which columns of the merged row it stores, in
 // row order of the group. -1 = the rowkey, -2, -3 ... = the following rowkey columns, >= 0 = payload column index.
 struct ObGpuColumnGroup {
   std::vector<int32_t> cols_;
   std::vector<int32_t> obj_types_;   // OBGPU_OBJ_* of every column (integer classes)
   int32_t rowkey_col_cnt_ = 0;       // > 0 for the group that carries the rowkey (all-column / rowkey group)
-  std::vector<int32_t> encodings_;   // OBGPU_ENC_RAW / OBGPU_ENC_AUTO of every column; empty: every column RAW
+  // OB_GPU_ENCODING_ROW_STORE: PAX blocks (obgpu_merge_result_encode_ex); OB_GPU_CS_ENCODING_ROW_STORE: CS blocks
+  // (obgpu_merge_result_encode_cs), which the device always writes whole (host_encoded_blocks_ stays 0)
+  int32_t row_store_type_ = OB_GPU_ENCODING_ROW_STORE;
+  // PAX: OBGPU_ENC_RAW / OBGPU_ENC_AUTO of every column, empty: every column RAW; CS: OBGPU_ENC_CS_INTEGER / CS_INT_DICT /
+  // CS_AUTO of every column, empty: every column CS_INTEGER
+  std::vector<int32_t> encodings_;
   // positions in cols_ of the columns the skip index aggregates (ObSkipIndexColMeta, MIN / MAX / NULL_COUNT); empty: no rows
   std::vector<int32_t> skip_index_cols_;
 };
@@ -95,7 +103,9 @@ public:
   // ObWriteHelper::project / append, column_store/ob_column_oriented_merger.cpp:722-745, ob_co_merge_writer.cpp:67-117,345):
   // the merged stream -- produced once by merge_partition -- is replayed into the writer of every column group. Here a
   // writer is the device encoder (obgpu_merge_result_encode): the rows never leave the device as rows, each group comes back
-  // as reference-format micro-blocks (each column RAW or AUTO, ObGpuColumnGroup::encodings_) + its column checksums.
+  // as reference-format micro-blocks + its column checksums: PAX blocks (each column RAW or AUTO) or, for a group whose
+  // row_store_type_ is OB_GPU_CS_ENCODING_ROW_STORE, CS blocks (each column CS_INTEGER, CS_INT_DICT or CS_AUTO), per
+  // ObGpuColumnGroup::encodings_.
   // rows_per_block cuts the blocks.
   // compressor (ObCompressorType: OBGPU_COMPRESSOR_LZ4 / LZ4_1_9_1 / ZSTD_1_3_8): every group comes back in STORED form
   // (ObMicroBlockCompressor): the device's blocks compressed on the device (obgpu_compress_blocks) before the fetch, the
