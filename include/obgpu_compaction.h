@@ -218,8 +218,8 @@ int obgpu_merge_result_encode_ex(obgpu_merge_result *res, const int32_t *result_
  * encodings[i]: OBGPU_ENC_CS_INTEGER / CS_INT_DICT / CS_AUTO; NULL: every column CS_INTEGER. Same handle as the PAX
  * encoder: obgpu_encoded_get_info / fetch / device_image / column_checksums / obgpu_compress_blocks work unchanged. The
  * blocks equal obgpu_writer_encode_table byte for byte for the same rows with the same per-column encodings while the
- * writer's CS stream mode is 1 (obgpu_writer_set_cs_stream_encoding, RAW streams, its default): the device always writes
- * RAW integer streams, whatever that process-wide mode is. No block is left to the host writer (n_host_blocks is 0).
+ * writer's CS stream mode is 1 (obgpu_writer_set_cs_stream_encoding, RAW streams, its default): these two always write
+ * RAW integer streams, whatever that process-wide mode is (the _ex forms below take the mode). No block is left to the host writer (n_host_blocks is 0).
  * byte_packing_only is ignored (the CS writer does not read it). OBGPU_NOT_SUPPORTED before any launch: a PAX encoding,
  * OBGPU_ENC_CS_STRING / CS_STR_DICT, a string obj_type, more than 64 columns, or a rows_per_block whose block does not fit
  * one CTA's shared memory (CS_INT_DICT / CS_AUTO columns need more of it). Bad pointers and sizes: OBGPU_INVALID_ARGUMENT,
@@ -230,6 +230,26 @@ int obgpu_encode_columns_cs(obgpu_ctx *ctx, const obgpu_encode_col *cols, const 
 int obgpu_merge_result_encode_cs(obgpu_merge_result *res, const int32_t *result_cols, const int32_t *obj_types,
                                  const int32_t *encodings, int32_t n_cols, int32_t rowkey_col_cnt, int64_t rows_per_block,
                                  int32_t align, obgpu_encoded **out);
+/* The same with the integer streams encoded under `stream_mode`, which has the meaning of obgpu_writer_set_cs_stream_encoding's
+ * mode (the two functions above are stream_mode 1):
+ *   cs_encoding/ob_integer_stream_encoder.h:224-400   ObIntegerStreamEncoder::inner_encode / choose_stream_codec /
+ *                                                     dectect_candidate_codec (mode 0: the candidate that encodes a prefix sample
+ *                                                     smallest; modes 2..6, 8: that codec; RAW wherever the codec is larger)
+ *   deps/oblib/src/lib/codec/                         ob_simd_fixed_pfor.h, ob_delta_zigzag_pfor.h, ob_double_delta_zigzag_pfor.h,
+ *                                                     ob_xor_fixed_pfor.h, ob_delta_zigzag_rle.h, ob_double_delta_zigzag_rle.h
+ *   0 detect per stream, 1 RAW, 2..6 / 8 that ObIntegerStream::EncodingType. The CS_INTEGER value stream, the CS_INT_DICT
+ * dictionary stream and its ref stream (plain or const form) take the codec; the stream-offsets stream stays RAW. The blocks equal
+ * obgpu_writer_encode_table byte for byte for the same rows and per-column encodings after
+ * obgpu_writer_set_cs_stream_encoding(stream_mode). The device never reads that process-wide writer mode: the mode is this
+ * argument. OBGPU_ENC_CS_AUTO's choice does not depend on the mode. Same handle and the same refusals as above; a stream_mode
+ * below 0, above 8 or 7 (UNIVERSAL_COMPRESS) is OBGPU_INVALID_ARGUMENT before any launch. Modes other than 1 need a little more
+ * shared memory per CTA, so their largest rows_per_block is slightly smaller. */
+int obgpu_encode_columns_cs_ex(obgpu_ctx *ctx, const obgpu_encode_col *cols, const int32_t *encodings, int32_t n_cols,
+                               int32_t rowkey_col_cnt, int64_t total_rows, int64_t rows_per_block, int32_t align,
+                               int32_t stream_mode, obgpu_encoded **out);
+int obgpu_merge_result_encode_cs_ex(obgpu_merge_result *res, const int32_t *result_cols, const int32_t *obj_types,
+                                    const int32_t *encodings, int32_t n_cols, int32_t rowkey_col_cnt, int64_t rows_per_block,
+                                    int32_t align, int32_t stream_mode, obgpu_encoded **out);
 typedef struct obgpu_encoded_info {
   int64_t image_size;    /* bytes of the image (aligned block slots)          */
   int64_t total_rows;

@@ -406,18 +406,31 @@ def _encodings(encodings, n):
     return e
 
 
+def _stream_mode(stream_mode: int, cs: bool) -> int:
+    if stream_mode != 1 and not cs:
+        raise ValueError("stream_mode selects the integer stream codecs of CS blocks: it needs cs=True")
+    return stream_mode
+
+
 def encode_columns(ctx, cols, total_rows: int, rows_per_block: int, rowkey_cnt: int = 0, align: int = 128, keep=None,
-                   encodings=None, cs: bool = False) -> Encoded:
+                   encodings=None, cs: bool = False, stream_mode: int = 1) -> Encoded:
     """cols: (device pointer of the int64 value images, device pointer of the NULL bytes or None, OBJ_* type, byte_packing_only).
     encodings: None (every column RAW) or per column capi.ENC_RAW / capi.ENC_AUTO.
     cs=True: CS_ENCODING_ROW_STORE blocks (obgpu_encode_columns_cs); encodings None (every column CS_INTEGER) or per column
-    capi.ENC_CS_INTEGER / ENC_CS_INT_DICT / ENC_CS_AUTO."""
+    capi.ENC_CS_INTEGER / ENC_CS_INT_DICT / ENC_CS_AUTO.
+    stream_mode (cs=True only): the integer stream codecs, as obgpu_writer_set_cs_stream_encoding takes them: 1 RAW (the
+    default), 0 detect per stream, 2..6 / 8 that codec (obgpu_encode_columns_cs_ex)."""
     h = C.c_void_p()
     arr = _encode_cols(cols)
     enc = _encodings(encodings, len(cols))
-    name = "obgpu_encode_columns_cs" if cs else "obgpu_encode_columns_ex"
-    check(getattr(lib, name)(ctx._h, arr, None if enc is None else enc.ctypes.data, len(cols), rowkey_cnt, total_rows,
-                             rows_per_block, align, C.byref(h)), name, ctx._h)
+    mode = _stream_mode(stream_mode, cs)
+    args = (ctx._h, arr, None if enc is None else enc.ctypes.data, len(cols), rowkey_cnt, total_rows, rows_per_block, align)
+    if cs:
+        name = "obgpu_encode_columns_cs_ex"
+        args += (mode,)
+    else:
+        name = "obgpu_encode_columns_ex"
+    check(getattr(lib, name)(*args, C.byref(h)), name, ctx._h)
     return Encoded(ctx, h, len(cols), keep)
 
 
@@ -452,36 +465,44 @@ def column_checksums(ctx, cols, total_rows: int) -> np.ndarray:
 
 
 def encode_merge_result(res: MergeResult, result_cols: Sequence[int], obj_types: Sequence[int], rows_per_block: int,
-                        rowkey_cnt: int = 1, align: int = 128, encodings=None, cs: bool = False) -> Encoded:
+                        rowkey_cnt: int = 1, align: int = 128, encodings=None, cs: bool = False, stream_mode: int = 1) -> Encoded:
     """One column group of the merged stream (-1: the rowkey, -2 ...: further rowkey columns, >= 0 payload columns).
     encodings: None (every column RAW) or per column capi.ENC_RAW / capi.ENC_AUTO.
-    cs=True: CS_ENCODING_ROW_STORE blocks (obgpu_merge_result_encode_cs), encodings as encode_columns takes them with cs=True."""
+    cs=True: CS_ENCODING_ROW_STORE blocks (obgpu_merge_result_encode_cs_ex), encodings and stream_mode as encode_columns takes
+    them with cs=True."""
     rc = np.ascontiguousarray(result_cols, dtype=np.int32)
     ot = np.ascontiguousarray(obj_types, dtype=np.int32)
     enc = _encodings(encodings, len(rc))
+    mode = _stream_mode(stream_mode, cs)
     h = C.c_void_p()
-    name = "obgpu_merge_result_encode_cs" if cs else "obgpu_merge_result_encode_ex"
-    check(getattr(lib, name)(res._h, rc.ctypes.data, ot.ctypes.data, None if enc is None else enc.ctypes.data, len(rc),
-                             rowkey_cnt, rows_per_block, align, C.byref(h)), name, res.ctx._h)
+    args = (res._h, rc.ctypes.data, ot.ctypes.data, None if enc is None else enc.ctypes.data, len(rc), rowkey_cnt, rows_per_block, align)
+    if cs:
+        name = "obgpu_merge_result_encode_cs_ex"
+        args += (mode,)
+    else:
+        name = "obgpu_merge_result_encode_ex"
+    check(getattr(lib, name)(*args, C.byref(h)), name, res.ctx._h)
     return Encoded(res.ctx, h, len(rc), res)
 
 
 def co_merge_write(res: MergeResult, column_groups: Sequence[Sequence[int]], obj_types: Dict[int, int], rows_per_block: int,
-                   align: int = 128, encodings: Optional[Dict[int, int]] = None, cs: bool = False) -> List[Encoded]:
+                   align: int = 128, encodings: Optional[Dict[int, int]] = None, cs: bool = False,
+                   stream_mode: int = 1) -> List[Encoded]:
     """Column-oriented merge, writer side (ObCOMergeLogReplayer::replay_merge_log -> ObCOMergeWriter -> ObWriteHelper::project /
     append, column_store/ob_column_oriented_merger.cpp:722-745, ob_co_merge_writer.cpp:67-117): the merged stream is produced
     ONCE and replayed into the writer of every column group; here every group is one obgpu_merge_result_encode over the columns
     the group projects. A group that holds the rowkey (-1 first) is written with rowkey_cnt 1, a pure column group with 0.
     encodings: like obj_types, per result column capi.ENC_RAW / capi.ENC_AUTO; None: every column RAW.
     cs=True: every group is written as CS_ENCODING_ROW_STORE blocks, encodings per column capi.ENC_CS_INTEGER / ENC_CS_INT_DICT /
-    ENC_CS_AUTO (None: every column CS_INTEGER)."""
+    ENC_CS_AUTO (None: every column CS_INTEGER), stream_mode as encode_columns takes it."""
+    _stream_mode(stream_mode, cs)
     out = []
     for cg in column_groups:
         cg = list(cg)
         rk = 1 if cg and cg[0] == -1 else 0
         enc = None if encodings is None else [encodings[c] for c in cg]
         out.append(encode_merge_result(res, cg, [obj_types[c] for c in cg], rows_per_block, rowkey_cnt=rk, align=align,
-                                       encodings=enc, cs=cs))
+                                       encodings=enc, cs=cs, stream_mode=stream_mode))
     return out
 
 

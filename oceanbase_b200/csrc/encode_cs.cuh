@@ -1,6 +1,7 @@
 // Phase B for tables whose row store is CS_ENCODING_ROW_STORE: merged integer columns -> CS micro-blocks, byte for byte the blocks
-// the host writer (sstable_writer.cpp: BlockBuilder::build_cs, choose_cs_auto_encoding, put_dict_ref_stream) writes with RAW
-// integer streams (obgpu_writer_set_cs_stream_encoding(1), its default). One kernel, one CTA per micro-block, on the phases of the
+// the host writer (sstable_writer.cpp: BlockBuilder::build_cs, choose_cs_auto_encoding, put_dict_ref_stream, emit_int_stream) writes
+// at the same CS stream mode (obgpu_writer_set_cs_stream_encoding): mode 1 RAW integer streams, the other modes the stream codecs of
+// stream_encode.cuh (the CODEC instantiations). One kernel, one CTA per micro-block, on the phases of the
 // PAX encoder (encode_kernels.cuh): ticket + decoupled look-back, stats pass with the column checksum folded in, block-wide stable
 // sort, parallel crc32c, one TMA store of the aligned slot.
 //
@@ -40,11 +41,11 @@ __device__ __forceinline__ uint32_t vi_len(unsigned long long v) {   // serializ
 }
 __device__ __forceinline__ uint32_t cs_bit_size(unsigned long long v) { return v == 0 ? 1u : 64u - (uint32_t)__clzll((long long)v); }
 
-// INTEGER_STREAM_META_V2, attr, IS_RAW, width tag, [vi64 base], [vi64 NULL replacement], pfor_packing_type_ 1, at byte `at`
+// INTEGER_STREAM_META_V2, attr, codec type, width tag, [vi64 base], [vi64 NULL replacement], pfor_packing_type_ 1, at byte `at`
 __device__ void put_stream_meta(uint32_t *img32, uint32_t at, uint32_t attr, uint32_t width, unsigned long long base,
-                                unsigned long long nullv) {
+                                unsigned long long nullv, uint32_t type = obf::IS_RAW) {
   const uint32_t tag = width == 1u ? 0u : width == 2u ? 1u : width == 4u ? 2u : 3u;
-  put_bytes(img32, at, 4u, 1u | (attr << 8) | ((uint32_t)obf::IS_RAW << 16) | (tag << 24));
+  put_bytes(img32, at, 4u, 1u | (attr << 8) | (type << 16) | (tag << 24));
   at += 4u;
   for (int k = 0; k < 2; ++k) {
     if (!(attr & (1u << k))) continue;
@@ -132,7 +133,50 @@ __device__ bool cs_auto_pick(const ColSpec &cs, const AutoCol &A, uint32_t nrows
   return dict_est < int_est * 70 / 100 || (dict_est < int_est && d < n * 50 / 100);
 }
 
-template <bool SORT>
+// The streams of a CS_INT_DICT column with d > 0 distinct values (A: the analysis on the write's key): the dictionary's base,
+// width and meta, and the ref stream, plain or in the const form (put_dict_ref_stream: the constant ties to the smallest sorted
+// ref, NULL only when strictly more frequent).
+__device__ __forceinline__ void cs_dict_layout(const ColSpec &cs, const AutoCol &A, uint32_t nrows, uint32_t nn, CsCol &L) {
+  const uint32_t d = A.d;
+  const unsigned long long f = cs.is_signed ? kSign : 0ull, vmin = A.kmin ^ f, vmax = A.kmax ^ f;
+  const bool use_base = cs.is_signed && (long long)vmin < 0;
+  L.base = use_base ? vmin : 0ull;
+  L.width = (uint8_t)bpis(vmax - L.base);
+  L.sattr = use_base ? (uint8_t)obf::IS_USE_BASE : 0;
+  L.meta = (uint8_t)(5u + (use_base ? vi_len(L.base) : 0u));
+  const uint32_t max_ref = nn ? d : d - 1u, max_cnt = max(A.fmax, nn), exc = nrows - max_cnt;
+  L.cform = exc == 0 || (exc <= 64u && exc < nrows * 10u / 100u);
+  L.exc = exc;
+  if (L.cform) {
+    L.rcnt = 2u + 2u * exc;
+    L.rwidth = (uint8_t)bpis(exc == 0 ? A.ref_w : max(max(exc, A.row_w), max_ref));
+  } else {
+    L.rcnt = nrows;
+    L.rwidth = (uint8_t)bpis(max_ref);
+  }
+}
+
+// The const-form ref stream [exceptions][constant cw][exception rows][exception refs] into cref, from the sorted refs in s.a.
+// Every thread calls it.
+__device__ void cs_const_refs(const AutoScratch &s, uint32_t nrows, uint32_t cw, uint32_t exc, uint32_t *cref) {
+  if (threadIdx.x == 0) { cref[0] = exc; cref[1] = cw; }
+  if (exc) {
+    for (uint32_t r = threadIdx.x; r < nrows; r += kThreads) s.hs[r] = s.a[r] != cw ? 1u : 0u;
+    __syncthreads();
+    blk_scan(s.hs, nrows, s.red);
+    for (uint32_t r = threadIdx.x; r < nrows; r += kThreads) {
+      if (s.a[r] == cw) continue;
+      const uint32_t k = s.hs[r] - 1u;
+      cref[2u + k] = r;
+      cref[2u + exc + k] = s.a[r];
+    }
+  }
+  __syncthreads();
+}
+
+// SORT: some column may store a dictionary (the sort scratch); CODEC: the integer streams take the stream codecs of
+// p.stream_mode (stream_encode.cuh) through a sizing phase between the analysis and the plan. <SORT, false> writes RAW streams.
+template <bool SORT, bool CODEC>
 __global__ void __launch_bounds__(kThreads) obgpu_encode_cs_kernel(const __grid_constant__ Params p) {
   extern __shared__ __align__(128) uint8_t smem[];
   uint32_t *img32 = reinterpret_cast<uint32_t *>(smem);              // block image, p.slot_cap bytes
@@ -158,6 +202,18 @@ __global__ void __launch_bounds__(kThreads) obgpu_encode_cs_kernel(const __grid_
     scr.b = scr.a + R;
     scr.hp = scr.b + R;
     scr.red = s_ared;
+  }
+  // CODEC: [n_cols] CsCodec, [kWarps][kHistBins] histograms, [chunks] chunk sizes, [kCrefMax] const-form refs behind the rest
+  StreamScratch sts{};
+  __shared__ uint32_t s_sred[CODEC ? kWarps : 1];
+  if constexpr (CODEC) {
+    uintptr_t q = SORT ? reinterpret_cast<uintptr_t>(scr.hp + p.rows_per_block + 1) : reinterpret_cast<uintptr_t>(s_cs + p.n_cols);
+    q = (q + 15u) & ~(uintptr_t)15u;
+    sts.cod = reinterpret_cast<CsCodec *>(q);
+    sts.hist = reinterpret_cast<uint32_t *>(sts.cod + p.n_cols);
+    sts.cref = sts.hist + kWarps * kHistBins;
+    sts.csz = sts.cref + kCrefMax;
+    sts.red = s_sred;
   }
   __shared__ uint32_t s_red[kWarps];
   __shared__ int s_blk;
@@ -241,8 +297,41 @@ __global__ void __launch_bounds__(kThreads) obgpu_encode_cs_kernel(const __grid_
           dict = s_pick != 0;
         }
         if (dict && !(cs.is_auto && same_key)) analyze_column(wk, row0, nrows, nn, p.sort_cap, scr, s_auto[c]);
+        if constexpr (CODEC) {   // the dictionary streams, while the column's sort on the write's key is in the scratch
+          if (dict && s_auto[c].d > 0) {
+            CsCol L{};
+            cs_dict_layout(cs, s_auto[c], nrows, nn, L);
+            uint32_t b0, b1;
+            const uint32_t t0 = choose_codec(p.stream_mode, DictVals{scr.sk, scr.hp, cs.is_signed ? kSign : 0ull, L.base}, s_auto[c].d,
+                                             L.width, sts, &b0);
+            if (L.cform) cs_const_refs(scr, nrows, s_auto[c].ref_w, L.exc, sts.cref);
+            const uint32_t t1 = choose_codec(p.stream_mode, RefVals{L.cform ? sts.cref : scr.a}, L.rcnt, L.rwidth, sts, &b1);
+            if (tid == 0) sts.cod[c] = CsCodec{{b0, b1}, {(uint8_t)t0, (uint8_t)t1}, {0, 0}};
+          }
+        }
       }
       if (tid == 0) s_cs[c].type = dict ? (uint8_t)obf::CS_INT_DICT : (uint8_t)obf::CS_INTEGER;
+    }
+    __syncthreads();
+  }
+
+  if constexpr (CODEC) {   // ---- stream sizing of the CS_INTEGER columns (the dictionary streams were sized in the analysis) ----
+    for (int c = 0; c < nc; ++c) {
+      if (SORT && s_cs[c].type != obf::CS_INTEGER) continue;
+      const ColSpec &cs = p.col[c];
+      uint32_t nn = 0;
+      unsigned long long kmin = ~0ull, kmax = 0;
+      for (int w = 0; w < kWarps; ++w) {
+        nn += s_wnull[w * nc + c];
+        kmin = min(kmin, s_wmin[w * nc + c]);
+        kmax = max(kmax, s_wmax[w * nc + c]);
+      }
+      const CsIntPlan ip = cs_int_plan(cs.is_signed, cs.store_size, kmin, kmax, nn < nrows, nn > 0);
+      const IntVals iv{cs.vals + row0, cs.nulls ? cs.nulls + row0 : nullptr, cs.is_signed ? ~0ull : cs.store_mask, ip.base,
+                       ip.replace ? ip.nullv - ip.base : 0ull};
+      uint32_t b0;
+      const uint32_t t0 = choose_codec(p.stream_mode, iv, nrows, bpis(ip.range), sts, &b0);
+      if (tid == 0) sts.cod[c] = CsCodec{{b0, 0u}, {(uint8_t)t0, (uint8_t)ST_RAW}, {0, 0}};
     }
     __syncthreads();
   }
@@ -272,32 +361,16 @@ __global__ void __launch_bounds__(kThreads) obgpu_encode_cs_kernel(const __grid_
           L.sattr = (uint8_t)((ip.use_base ? obf::IS_USE_BASE : 0) | (ip.replace ? obf::IS_REPLACE_NULL_VALUE : 0));
           L.attrs = ip.bitmap ? (uint8_t)obf::CS_HAS_NULL_OR_NOP_BITMAP : 0;
           L.meta = (uint8_t)(5u + (ip.use_base ? vi_len(ip.base) : 0u) + (ip.replace ? vi_len(ip.nullv) : 0u));
-          bytes = (ip.bitmap ? (nrows + 7u) / 8u : 0u) + L.meta + L.width * nrows;
+          bytes = (ip.bitmap ? (nrows + 7u) / 8u : 0u) + L.meta + (CODEC ? sts.cod[c].bytes[0] : L.width * nrows);
           ns = 1;
         } else if (SORT) {
           const AutoCol &A = s_auto[c];
           const uint32_t d = A.d;
           bytes = 10u;   // ObDictEncodingMeta
           if (d > 0) {
-            const unsigned long long f = cs.is_signed ? kSign : 0ull, vmin = A.kmin ^ f, vmax = A.kmax ^ f;
-            const bool use_base = cs.is_signed && (long long)vmin < 0;
-            L.base = use_base ? vmin : 0ull;
-            L.width = (uint8_t)bpis(vmax - L.base);
-            L.sattr = use_base ? (uint8_t)obf::IS_USE_BASE : 0;
-            L.meta = (uint8_t)(5u + (use_base ? vi_len(L.base) : 0u));
-            L.s0 = 10u + L.meta + L.width * d;
-            // put_dict_ref_stream: the constant ties to the smallest sorted ref, NULL only when strictly more frequent
-            const uint32_t max_ref = nn ? d : d - 1u, max_cnt = max(A.fmax, nn), exc = nrows - max_cnt;
-            L.cform = exc == 0 || (exc <= 64u && exc < nrows * 10u / 100u);
-            L.exc = exc;
-            if (L.cform) {
-              L.rcnt = 2u + 2u * exc;
-              L.rwidth = (uint8_t)bpis(exc == 0 ? A.ref_w : max(max(exc, A.row_w), max_ref));
-            } else {
-              L.rcnt = nrows;
-              L.rwidth = (uint8_t)bpis(max_ref);
-            }
-            bytes = L.s0 + 5u + L.rwidth * L.rcnt;
+            cs_dict_layout(cs, A, nrows, nn, L);
+            L.s0 = 10u + L.meta + (CODEC ? sts.cod[c].bytes[0] : L.width * d);
+            bytes = L.s0 + 5u + (CODEC ? sts.cod[c].bytes[1] : L.rwidth * L.rcnt);
             ns = 2;
           }
         }
@@ -360,17 +433,21 @@ __global__ void __launch_bounds__(kThreads) obgpu_encode_cs_kernel(const __grid_
     if (L.type == obf::CS_INTEGER) {
       const bool bitmap = L.attrs != 0;
       const uint32_t mo = o + (bitmap ? (nrows + 7u) / 8u : 0u), v0 = mo + L.meta, w = L.width;
-      if (tid == 0) put_stream_meta(img32, mo, L.sattr, w, L.base, L.nullv);
+      const uint32_t type = CODEC ? sts.cod[c].type[0] : (uint32_t)ST_RAW;
+      const bool raw = type == ST_RAW;
+      if (tid == 0) put_stream_meta(img32, mo, L.sattr, w, L.base, L.nullv, type);
       const unsigned long long nv = (L.sattr & obf::IS_REPLACE_NULL_VALUE) ? L.nullv - L.base : 0ull;
       for (uint32_t r = (uint32_t)tid; r < nrows; r += kThreads) {
         if (nl && nl[r] != 0) {
           if (bitmap) or_bits(img32, (o + r / 8u) * 8u + 7u - (r & 7u), 1u, 1ull);   // MSB first
-          put_bytes(img32, v0 + r * w, w, nv);
+          if (raw) put_bytes(img32, v0 + r * w, w, nv);
           continue;
         }
         const unsigned long long x = (unsigned long long)cs.vals[row0 + r];
-        put_bytes(img32, v0 + r * w, w, (cs.is_signed ? x : x & cs.store_mask) - L.base);
+        if (raw) put_bytes(img32, v0 + r * w, w, (cs.is_signed ? x : x & cs.store_mask) - L.base);
       }
+      if constexpr (CODEC)
+        if (!raw) codec_stream(type, IntVals{cs.vals + row0, nl, cs.is_signed ? ~0ull : cs.store_mask, L.base, nv}, nrows, w, sts, img32, v0);
       continue;
     }
     if constexpr (SORT) {   // INT_DICT
@@ -388,12 +465,22 @@ __global__ void __launch_bounds__(kThreads) obgpu_encode_cs_kernel(const __grid_
       sort_column(wk, row0, nrows, nn, p.sort_cap, scr);
       const unsigned long long f = cs.is_signed ? kSign : 0ull;
       const uint32_t w = L.width, rw = L.rwidth, r0 = o + L.s0 + 5u, cw = s_auto[c].ref_w, exc = L.exc;
+      const uint32_t t0 = CODEC ? sts.cod[c].type[0] : (uint32_t)ST_RAW, t1 = CODEC ? sts.cod[c].type[1] : (uint32_t)ST_RAW;
       if (tid == 0) {
-        put_stream_meta(img32, o + 10u, L.sattr, w, L.base, 0ull);
-        put_stream_meta(img32, o + L.s0, 0u, rw, 0ull, 0ull);
+        put_stream_meta(img32, o + 10u, L.sattr, w, L.base, 0ull, t0);
+        put_stream_meta(img32, o + L.s0, 0u, rw, 0ull, 0ull, t1);
       }
-      for (uint32_t v = (uint32_t)tid; v < d; v += kThreads) put_bytes(img32, o + 10u + L.meta + v * w, w, (scr.sk[scr.hp[v]] ^ f) - L.base);
-      if (!L.cform) {
+      if (t0 == ST_RAW) {
+        for (uint32_t v = (uint32_t)tid; v < d; v += kThreads) put_bytes(img32, o + 10u + L.meta + v * w, w, (scr.sk[scr.hp[v]] ^ f) - L.base);
+      } else if constexpr (CODEC) {
+        codec_stream(t0, DictVals{scr.sk, scr.hp, f, L.base}, d, w, sts, img32, o + 10u + L.meta);
+      }
+      if (t1 != ST_RAW) {
+        if constexpr (CODEC) {
+          if (L.cform) cs_const_refs(scr, nrows, cw, exc, sts.cref);
+          codec_stream(t1, RefVals{L.cform ? sts.cref : scr.a}, L.rcnt, rw, sts, img32, r0);
+        }
+      } else if (!L.cform) {
         for (uint32_t r = (uint32_t)tid; r < nrows; r += kThreads) put_bytes(img32, r0 + r * rw, rw, scr.a[r]);
       } else {   // [exceptions][const ref][exception rows][exception refs]
         if (tid == 0) {
@@ -427,13 +514,16 @@ __global__ void __launch_bounds__(kThreads) obgpu_encode_cs_kernel(const __grid_
 }  // namespace enc
 
 static bool cs_encoding_ok(int32_t e) { return e == OBGPU_ENC_CS_INTEGER || e == OBGPU_ENC_CS_INT_DICT || e == OBGPU_ENC_CS_AUTO; }
+// obgpu_writer_set_cs_stream_encoding's modes: 0 detect, 1 RAW, 2..8 one codec except 7 (UNIVERSAL_COMPRESS)
+static bool cs_stream_mode_ok(int32_t m) { return m >= 0 && m <= 8 && m != 7; }
 
 extern "C" {
 
-int obgpu_encode_columns_cs(obgpu_ctx *ctx, const obgpu_encode_col *cols, const int32_t *encodings, int32_t n_cols, int32_t rowkey_col_cnt,
-                            int64_t total_rows, int64_t rows_per_block, int32_t align, obgpu_encoded **out) {
+int obgpu_encode_columns_cs_ex(obgpu_ctx *ctx, const obgpu_encode_col *cols, const int32_t *encodings, int32_t n_cols,
+                               int32_t rowkey_col_cnt, int64_t total_rows, int64_t rows_per_block, int32_t align, int32_t stream_mode,
+                               obgpu_encoded **out) {
   if (!ctx || !cols || !out || n_cols <= 0 || rowkey_col_cnt < 0 || rowkey_col_cnt > n_cols || total_rows <= 0 || rows_per_block <= 0 ||
-      rows_per_block > (1 << 22) || align < 16 || align > 4096 || (align & (align - 1)) != 0)
+      rows_per_block > (1 << 22) || align < 16 || align > 4096 || (align & (align - 1)) != 0 || !cs_stream_mode_ok(stream_mode))
     return OBGPU_INVALID_ARGUMENT;
   if (n_cols > enc::kMaxCols) return OBGPU_NOT_SUPPORTED;
   const int64_t n_blocks64 = (total_rows + rows_per_block - 1) / rows_per_block;
@@ -465,16 +555,30 @@ int obgpu_encode_columns_cs(obgpu_ctx *ctx, const obgpu_encode_col *cols, const 
   while ((int64_t)sort_cap < R) sort_cap <<= 1;
   // INT_DICT / AUTO: the AutoCol records and the sort scratch (keys, rows, scan: sort_cap each; refs, first occurrences: R each; R + 1 heads)
   if (n_sort) smem += 32 + (size_t)n_cols * sizeof(enc::AutoCol) + (size_t)sort_cap * 16 + (size_t)R * 12 + 4;
+  // stream codecs: the CsCodec records, the chunk histograms, the const-form refs and the chunk sizes of the longest stream
+  const bool codec = stream_mode != enc::ST_RAW;
+  if (codec)
+    smem += 16 + (size_t)n_cols * sizeof(enc::CsCodec) + 4 * (size_t)(enc::kWarps * enc::kHistBins + enc::kCrefMax) +
+            4 * (size_t)((std::max<int64_t>(R, enc::kCrefMax) + 127) / 128);
   if ((int64_t)smem > (int64_t)ctx->max_smem_optin - 8192) return OBGPU_NOT_SUPPORTED;   // block image does not fit one CTA's shared memory
   p.rowkey_cnt = rowkey_col_cnt;
-  // the sorting instantiation only when some column may store a dictionary: CS_INTEGER-only calls keep the lean kernel
-  return enc_launch(ctx, p, n_blocks64, total_rows, rows_per_block, align, slot_cap, sort_cap, smem,
-                    n_sort ? enc::obgpu_encode_cs_kernel<true> : enc::obgpu_encode_cs_kernel<false>, out);
+  p.stream_mode = stream_mode;
+  // the sorting instantiations only when some column may store a dictionary: CS_INTEGER-only calls keep the lean kernel; RAW
+  // streams (mode 1) keep the kernels without the stream codecs
+  void (*kernel)(enc::Params) = n_sort ? (codec ? enc::obgpu_encode_cs_kernel<true, true> : enc::obgpu_encode_cs_kernel<true, false>)
+                                       : (codec ? enc::obgpu_encode_cs_kernel<false, true> : enc::obgpu_encode_cs_kernel<false, false>);
+  return enc_launch(ctx, p, n_blocks64, total_rows, rows_per_block, align, slot_cap, sort_cap, smem, kernel, out);
 }
 
-int obgpu_merge_result_encode_cs(obgpu_merge_result *res, const int32_t *result_cols, const int32_t *obj_types, const int32_t *encodings,
-                                 int32_t n_cols, int32_t rowkey_col_cnt, int64_t rows_per_block, int32_t align, obgpu_encoded **out) {
-  if (!res || !result_cols || !obj_types || n_cols <= 0 || !out) return OBGPU_INVALID_ARGUMENT;
+int obgpu_encode_columns_cs(obgpu_ctx *ctx, const obgpu_encode_col *cols, const int32_t *encodings, int32_t n_cols, int32_t rowkey_col_cnt,
+                            int64_t total_rows, int64_t rows_per_block, int32_t align, obgpu_encoded **out) {
+  return obgpu_encode_columns_cs_ex(ctx, cols, encodings, n_cols, rowkey_col_cnt, total_rows, rows_per_block, align, enc::ST_RAW, out);
+}
+
+int obgpu_merge_result_encode_cs_ex(obgpu_merge_result *res, const int32_t *result_cols, const int32_t *obj_types,
+                                    const int32_t *encodings, int32_t n_cols, int32_t rowkey_col_cnt, int64_t rows_per_block,
+                                    int32_t align, int32_t stream_mode, obgpu_encoded **out) {
+  if (!res || !result_cols || !obj_types || n_cols <= 0 || !out || !cs_stream_mode_ok(stream_mode)) return OBGPU_INVALID_ARGUMENT;
   if (n_cols > enc::kMaxCols) return OBGPU_NOT_SUPPORTED;
   for (int c = 0; encodings && c < n_cols; ++c)
     if (!cs_encoding_ok(encodings[c])) return OBGPU_NOT_SUPPORTED;
@@ -482,7 +586,13 @@ int obgpu_merge_result_encode_cs(obgpu_merge_result *res, const int32_t *result_
   int64_t rows = 0;
   const int rc = merge_result_cols(res, result_cols, obj_types, n_cols, cols, rows);
   if (rc != OBGPU_SUCCESS) return rc;
-  return obgpu_encode_columns_cs(res->ctx, cols.data(), encodings, n_cols, rowkey_col_cnt, rows, rows_per_block, align, out);
+  return obgpu_encode_columns_cs_ex(res->ctx, cols.data(), encodings, n_cols, rowkey_col_cnt, rows, rows_per_block, align, stream_mode, out);
+}
+
+int obgpu_merge_result_encode_cs(obgpu_merge_result *res, const int32_t *result_cols, const int32_t *obj_types, const int32_t *encodings,
+                                 int32_t n_cols, int32_t rowkey_col_cnt, int64_t rows_per_block, int32_t align, obgpu_encoded **out) {
+  return obgpu_merge_result_encode_cs_ex(res, result_cols, obj_types, encodings, n_cols, rowkey_col_cnt, rows_per_block, align, enc::ST_RAW,
+                                         out);
 }
 
 }  // extern "C"

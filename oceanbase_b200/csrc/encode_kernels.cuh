@@ -57,6 +57,7 @@ struct Params {
   unsigned long long *totals;        // [0] image bytes, [1] host blocks
   int32_t *ticket;
   const uint32_t *xpow32;            // x^(32 k) mod P, reflected (x^0 = 0x80000000)
+  int32_t stream_mode;               // CS encoder with stream codecs: the integer stream mode (0 detect, 2..8 that codec)
 };
 
 __device__ __forceinline__ uint32_t gf2_mulmod(uint32_t a, uint32_t b) {

@@ -3269,6 +3269,7 @@ int obgpu_project_datums(obgpu_batch *batch, int32_t block, int32_t col, const i
 #include "merge_exchange.cuh"
 #include "merge_streamed.cuh"
 #include "encode_kernels.cuh"   // phase B: merged columns -> SSTable bytes + column checksums
+#include "stream_encode.cuh"   // integer stream codecs of CS blocks on the device
 #include "encode_cs.cuh"       // phase B for CS tables: merged integer columns -> CS_ENCODING_ROW_STORE micro-blocks
 #include "stored_blocks.cuh"    // stored (raw, LZ4- or zstd-compressed) micro-blocks -> page batch, decoded on the device
 #include "stored_compress.cuh"  // plain micro-blocks -> stored (LZ4- or zstd-compressed) form, compressed on the device

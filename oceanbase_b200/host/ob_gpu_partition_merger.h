@@ -65,6 +65,9 @@ struct ObGpuColumnGroup {
   // PAX: OBGPU_ENC_RAW / OBGPU_ENC_AUTO of every column, empty: every column RAW; CS: OBGPU_ENC_CS_INTEGER / CS_INT_DICT /
   // CS_AUTO of every column, empty: every column CS_INTEGER
   std::vector<int32_t> encodings_;
+  // CS only: the integer stream codecs (obgpu_merge_result_encode_cs_ex, obgpu_writer_set_cs_stream_encoding's modes): 1 RAW,
+  // 0 detect per stream, 2..6 / 8 that codec. A PAX group takes 1 only.
+  int32_t cs_stream_mode_ = 1;
   // positions in cols_ of the columns the skip index aggregates (ObSkipIndexColMeta, MIN / MAX / NULL_COUNT); empty: no rows
   std::vector<int32_t> skip_index_cols_;
 };
