@@ -356,6 +356,8 @@ static int fill_batch(obgpu_ctx *ctx, obgpu_batch *b, const void *image, int64_t
   return OBGPU_SUCCESS;
 }
 
+static void batch_codes_free(obgpu_batch *b);   // batch_codes.cuh
+
 extern "C" {
 
 int obgpu_batch_open(obgpu_ctx *ctx, const void *image, int64_t image_size, const int64_t *offsets,
@@ -392,6 +394,7 @@ void obgpu_batch_close(obgpu_batch *b) {
   if (b->d_agg_off) cudaFreeAsync(b->d_agg_off, b->ctx->stream);
   if (b->d_xf) cudaFreeAsync(b->d_xf, b->ctx->stream);
   if (b->own_image && b->d_image) cudaFreeAsync((void *)b->d_image, b->ctx->stream);
+  batch_codes_free(b);
   delete b;
 }
 

@@ -182,6 +182,7 @@ int obgpu_pipeline_scan(obgpu_pipeline *p, const obgpu_host_scan_spec *s, obgpu_
                                        (const uint8_t *)s->image + lo, &batch)   // the pinned host image IS the device image
                     : obgpu_batch_open(ctx, (const uint8_t *)s->image + lo, hi - lo, offs.data(), s->sizes + b0, b1 - b0, 0, nullptr, &batch);
       if (ret != OBGPU_SUCCESS) { fail(ret); return; }
+      batch->codes_allowed = false;   // scanned once: batch string codes would cost more than they save
       if (s->agg_rows && s->agg_off) {   // offsets keep their table-wide base: the entry rebases them
         ret = obgpu_batch_set_agg_rows(batch, s->agg_rows, s->agg_off + b0);
         if (ret != OBGPU_SUCCESS) { fail(ret); return; }

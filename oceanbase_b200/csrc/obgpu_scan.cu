@@ -156,6 +156,14 @@ struct ScanParams {
   int32_t pc_rec, pp_rec;
   uint8_t used_sc[kMaxUsedCols], used_elem_len[kMaxUsedCols];
   uint64_t used_int_mask[kMaxUsedCols];
+  // batch string codes (batch_codes.cuh) in the record count kernel: filter column i < kCodedCols with bit i of pf_coded set stages
+  // its refs and its block's codes (at pf_codes[i] in a region slot) instead of its region; a leaf on it tests bit code[ref] of
+  // code_bits + slot * code_words, the leaf evaluated once per scan over the column's distinct strings
+  int32_t pf_coded, code_words;
+  uint32_t pf_codes[4];
+  const uint16_t *codes[4];          // [sum of r8(dict_count)] codes of every block's dictionary entries
+  const uint32_t *code_off16[4];     // [n_blocks] first code of a block, in 16-byte units
+  const uint32_t *code_bits;
 };
 
 // =================================================================================================
@@ -1791,6 +1799,7 @@ struct obgpu_ctx {
   static constexpr int kProfRing = 256;
   cudaEvent_t ev0[kProfRing] = {nullptr}, ev1[kProfRing] = {nullptr};
   int64_t prof_count = 0;
+  int32_t last_pc_bytes = 0, last_count_ctas = 0;   // small-block count kernel of the last scan (obgpu_ctx_count_layout)
 };
 
 // Device scratch of one host call: slices reserved with take(), then one cudaMallocAsync of their total on the ctx stream.
@@ -1814,6 +1823,20 @@ struct Scratch {
   cudaError_t alloc(size_t n) { take(n, 1); return alloc(); }   // an arena of one slice
   template <class T> T *at(size_t off) const { return reinterpret_cast<T *>(p + off); }
   void *release() { void *q = p; p = nullptr; return q; }
+};
+
+// Batch-wide integer codes of a string dictionary column (batch_codes.cuh): every block's dictionary entry -> the code of its
+// string among the column's distinct strings, and the code table (image byte offset << 16 | length per code).
+struct StrCodes {
+  int32_t state = 0;            // 0: not built, 1: built, < 0: the column keeps the region path (OBGPU_CODES_* reason)
+  int32_t n_codes = 0;
+  uint32_t refs_span = 0;       // widest refs range of a block (bytes, 16-byte aligned)
+  uint32_t codes_span = 0;      // widest code slice of a block (bytes)
+  float build_ms = 0.f;
+  void *d_mem = nullptr;        // one allocation: [code_off16: n_blocks][code table: n_codes][codes]
+  const uint32_t *d_off16 = nullptr;
+  const uint64_t *d_table = nullptr;
+  const uint16_t *d_codes = nullptr;
 };
 
 struct obgpu_batch {
@@ -1851,6 +1874,9 @@ struct obgpu_batch {
   // CS stream codecs: blocks restated as RAW at open (stream_codecs.cuh); nullptr when nothing had to be decoded
   obcs::XformRec *d_xf = nullptr;
   std::vector<uint8_t> col_mat;        // per store index: 1 when some block rebuilt the column's strings at open (mat_codecs.cuh)
+  // batch string codes (batch_codes.cuh): per store index, built on the first scan with an EQ / NE / IN leaf on the column
+  std::vector<struct StrCodes> str_codes;
+  bool codes_allowed = true;           // false: batches scanned once (the host pipeline) never build codes
 };
 
 // Whether a scan of the batch may take the small-block pipelined kernels (scan_small.cuh): fill_batch builds stage records
@@ -2027,6 +2053,7 @@ int obgpu_ctx_kernel_times(obgpu_ctx *ctx, float *ms, int32_t cap, int32_t *n) {
 }  // extern "C"
 
 #include "batch_open.cuh"   // page-batch open: header checks, open-time rewrites of the image, decode plans
+#include "batch_codes.cuh"  // batch-wide codes of dictionary string columns, built on first use
 
 // ---- building the kernel parameter block ---------------------------------------------------------
 static int used_index(ScanParams &p, int32_t col) {
@@ -2322,7 +2349,7 @@ static void layout_smem_scan(const obgpu_batch *b, ScanParams &p, int max_smem) 
 
 
 // Small-block pipelined kernels (scan_small.cuh): which of them this scan can use, and their per-warp layouts.
-static void layout_pipe(const obgpu_batch *b, ScanParams &p, int max_smem) {
+static void layout_pipe(obgpu_batch *b, ScanParams &p, int max_smem) {
   p.pipe_count = p.pipe_project = 0;
   p.pc_rec = p.pp_rec = 0;
   if (!pipe_wanted(b->max_rows)) return;
@@ -2372,8 +2399,33 @@ static void layout_pipe(const obgpu_batch *b, ScanParams &p, int max_smem) {
         if (rec) rec = p.used_sc[nd.used_idx] == 5 ? (nd.op == OP_EQ || nd.op == OP_NE || nd.op == OP_IN) : nd.range_ok != 0;
       }
       p.pc_rec = rec ? 1 : 0;
+      // batch string codes: a string filter column among the first four (every leaf on it is an EQ / NE / IN: records) stages its
+      // refs and its block's code slice instead of its region, when its codes exist or can be built now
+      uint32_t coded_off = off;
+      p.pf_coded = 0;
+      const char *ce = getenv("OBGPU_STR_CODES");   // testing knob: 0 keeps every string leaf on its per-block dictionary
+      if (rec && b->codes_allowed && !(ce && atoi(ce) == 0)) {
+        uint32_t at = 0;
+        for (int i = 0; i < nf; ++i) {
+          const StrCodes *sc = i < 4 && p.used_sc[i] == 5 ? &batch_codes(b, p.used_col[i]) : nullptr;
+          p.pf_off[i] = at;
+          if (sc && sc->state == 1) {
+            p.pf_coded |= 1 << i;
+            p.pf_span[i] = r16(sc->refs_span);
+            p.pf_codes[i] = kCountHdrBytes + at + p.pf_span[i];
+            p.codes[i] = sc->d_codes;
+            p.code_off16[i] = sc->d_off16;
+            p.code_words = std::max<int32_t>(p.code_words, (sc->n_codes + 31) / 32);
+            at += p.pf_span[i] + r16(sc->codes_span);
+          } else {
+            p.pf_span[i] = r16(b->col_span[(size_t)p.used_col[i]]);
+            at += p.pf_span[i];
+          }
+        }
+        coded_off = at;
+      }
       p.pc_meta_bytes = kMetaPlans + (uint32_t)nf * (rec ? kCountEnt<true> : kCountEnt<false>);
-      p.pc_region_bytes = kCountHdrBytes + off;
+      p.pc_region_bytes = kCountHdrBytes + coded_off;
       uint32_t w = 0;
       p.pc_meta = w;   w += 3u * p.pc_meta_bytes;
       p.pc_region = w; w += 2u * p.pc_region_bytes;
@@ -2649,6 +2701,8 @@ static int scan_common(obgpu_batch *b, const obgpu_scan_spec *spec, const obgpu_
   const bool use_skip = b->d_agg != nullptr && p.n_nodes > 0;
   const size_t o_blk_const = use_skip ? arena.take((size_t)n) : 0;
   const size_t o_leaf_const = use_skip ? arena.take((size_t)n * (size_t)p.n_nodes) : 0;
+  const bool coded = p.pipe_count && p.pc_rec && p.pf_coded && !ext_bm;
+  const size_t o_code_bits = coded ? arena.take((size_t)p.n_slots * (size_t)p.code_words * 4) : 0;
   size_t o_data[kMaxProj], o_lens[kMaxProj];
   for (int c = 0; c < spec->n_proj; ++c) {
     const int t = b->col_types[(size_t)spec->proj_cols[c]];
@@ -2683,6 +2737,8 @@ static int scan_common(obgpu_batch *b, const obgpu_scan_spec *spec, const obgpu_
   p.bitmap_words = (uint32_t *)(a + o_bm);
   p.row_ids = spec->want_row_ids ? (int32_t *)(a + o_rid) : nullptr;
   p.out_cap = r->cap;
+  p.code_bits = coded ? (const uint32_t *)(a + o_code_bits) : nullptr;
+  if (!coded) p.pf_coded = 0;
   for (int c = 0; c < spec->n_proj; ++c) {
     r->cols[c].data = a + o_data[c];
     r->cols[c].lens = r->cols[c].is_string ? (int32_t *)(a + o_lens[c]) : nullptr;
@@ -2723,9 +2779,24 @@ static int scan_common(obgpu_batch *b, const obgpu_scan_spec *spec, const obgpu_
       int occ = 1;
       const auto kern = p.pc_rec ? obgpu_count_pipe_kernel<true> : obgpu_count_pipe_kernel<false>;
       cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, kThreads, smem);
+      ctx->last_pc_bytes = (int32_t)p.pc_bytes;
+      ctx->last_count_ctas = occ;
       const int grid = std::min((n + kWarps - 1) / kWarps, std::max(1, occ) * ctx->sm_count);
+      if (p.pc_rec && p.pf_coded) {
+        // the leaves on coded columns, once over each column's distinct strings
+        const int n_leaves = p.n_nodes == 1 ? 1 : p.n_nodes - 1;
+        for (int i = 0; i < n_leaves; ++i) {
+          const FilterNodeDev &nd = p.nodes[i];
+          if (!((p.pf_coded >> nd.used_idx) & 1)) continue;
+          const StrCodes &sc = b->str_codes[(size_t)p.used_col[nd.used_idx]];
+          obgpu_code_leaf_kernel<<<(p.code_words * 32 + 255) / 256, 256, 0, ctx->stream>>>(p, i, sc.d_table, sc.n_codes, p.code_words,
+                                                                                          const_cast<uint32_t *>(p.code_bits) + nd.slot * p.code_words);
+          ctx->launches++;
+        }
+      }
       kern<<<grid, kThreads, smem, ctx->stream>>>(p);
     } else {
+      ctx->last_pc_bytes = ctx->last_count_ctas = 0;
       obgpu_count_kernel<<<(n + kWarps - 1) / kWarps, kThreads, cw_total, ctx->stream>>>(p);
     }
     ctx->launches++;

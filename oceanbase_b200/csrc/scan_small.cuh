@@ -106,6 +106,35 @@ __device__ __forceinline__ uint32_t lean_rows(const D &d, uint32_t sbit, const u
   return and_mode ? (mybm & acc) : (mybm | acc);
 }
 
+__device__ __forceinline__ uint32_t sld16(uint32_t a) {
+  unsigned short v;
+  asm volatile("ld.shared.u16 %0, [%1];" : "=h"(v) : "r"(a));
+  return v;
+}
+
+// Rows of a string K_DICT column with batch codes (batch_codes.cuh) against the leaf's bitset over the column's distinct strings:
+// row verdict = bit code[ref] of the bitset at word wbase of p.code_bits (read through the read-only cache: a few hundred bytes
+// shared by every warp), the block's codes staged at shared address cbase; NULL refs (ref >= dict_count) never match. Lane g collects
+// word g; returns the lane's updated bitmap word.
+template <class D>
+__device__ __forceinline__ uint32_t lean_rows_coded(const ScanParams &p, const D &d, uint32_t sbit, uint32_t cbase, uint32_t wbase, uint32_t mybm,
+                                                    uint32_t myvalid, uint32_t nwords, bool and_mode, int lane) {
+  const uint32_t step = 32u * d.stride, width = d.width, dcount = d.dict_count;
+  uint32_t bit = sbit + d.val_bit + (uint32_t)lane * d.stride, acc = 0;
+  for (uint32_t g = 0; g < nwords; ++g, bit += step) {
+    const uint32_t ref = sbits32(bit, width);
+    bool hit = false;
+    if (ref < dcount) {
+      const uint32_t c = sld16(cbase + ref * 2u);
+      hit = (__ldg(p.code_bits + wbase + (c >> 5)) >> (c & 31u)) & 1u;
+    }
+    const uint32_t w = __ballot_sync(0xffffffffu, hit);
+    if ((uint32_t)lane == g) acc = w;
+  }
+  acc &= myvalid;
+  return and_mode ? (mybm & acc) : (mybm | acc);
+}
+
 // Sorted fixed-width integer dictionary and a range leaf: the matching refs are [a, e) = [#entries below the range,
 // #entries not above it) (the reference binary-searches the bounds, ob_dict_decoder.cpp:967-988,1085-1176).
 template <class D>
@@ -425,6 +454,8 @@ __global__ void __launch_bounds__(kThreads) obgpu_count_pipe_kernel(const __grid
     uint8_t *m = meta0 + (uint32_t)ms * p.pc_meta_bytes;
     if (p.blk_const != nullptr) verdict = p.blk_const[b];
     issue_meta<REC, false, kEnt>(p, b, smem_u32(m), nf, [&](int i) { return p.used_col[i]; }, lane);
+    // a coded column's first code of the block, in the meta slot's otherwise unused sel_offset bytes (4 per column)
+    if (REC && lane < 4 && ((p.pf_coded >> lane) & 1)) cp_async4(smem_u32(m) + kMetaSel + 4u * (uint32_t)lane, p.code_off16[lane] + b);
   };
   // region slot: [int32 delta[kPipeMaxFilterCols] | declined mask | verdict] (64 bytes) then the regions at p.pf_off[i]
   auto regions = [&](int b, int ms, int rsl) {
@@ -434,10 +465,23 @@ __global__ void __launch_bounds__(kThreads) obgpu_count_pipe_kernel(const __grid
     uint64_t *bar = bars + rsl;
     const BlockRec &rec = *reinterpret_cast<const BlockRec *>(m);
     int32_t *hdr = reinterpret_cast<int32_t *>(rs);
-    uint32_t r[4] = {0, 0, 0, 0};
+    uint32_t r[4] = {0, 0, 0, 0}, cb = 0;
     bool bad = false;
     if (lane < nf && rec.rows != 0 && verdict == 0) {
-      bad = staged_ranges<REC, true>(rec, m + kMetaPlans + (uint32_t)lane * kEnt, p.pf_span[lane], r) == 0;
+      if (REC && ((p.pf_coded >> lane) & 1)) {
+        // coded column: its refs (the first projection range, or the second when the END offsets come first) and its code slice
+        const StageRec &sr = *reinterpret_cast<const StageRec *>(m + kMetaPlans + (uint32_t)lane * kEnt);
+        const bool alt = sr.lo[1] != sr.hi[1] && (sr.val_bit >> 3) >= sr.dict_payload;
+        r[0] = (uint32_t)(alt ? sr.lo[1] : sr.lo[0]) * 16u;
+        r[1] = (uint32_t)(alt ? sr.hi[1] : sr.hi[0]) * 16u;
+        cb = (((uint32_t)sr.dict_count + 7u) >> 3) * 16u;
+        bad = r[1] - r[0] > p.pf_span[lane] || r[1] > ((rec.size + 15u) & ~15u) + 32u;
+        if (bad) r[0] = r[1] = cb = 0;
+        // issued before the slot's expect_tx (the slot's phase cannot complete before that arrival): the address dies here
+        if (cb != 0) tma_bulk_g2s(rs + p.pf_codes[lane], p.codes[lane] + (size_t)*reinterpret_cast<const uint32_t *>(m + kMetaSel + 4u * lane) * 8u, cb, bar);
+      } else {
+        bad = staged_ranges<REC, true>(rec, m + kMetaPlans + (uint32_t)lane * kEnt, p.pf_span[lane], r) == 0;
+      }
       hdr[lane] = (int32_t)(kCountHdrBytes + p.pf_off[lane]) - (int32_t)r[0];
     }
     const uint32_t badmask = __ballot_sync(0xffffffffu, bad);
@@ -446,7 +490,7 @@ __global__ void __launch_bounds__(kThreads) obgpu_count_pipe_kernel(const __grid
       hdr[kPipeMaxFilterCols + 1] = (int32_t)verdict;
     }
     // one bulk copy (TMA) per filter column, all completing on the slot's mbarrier
-    const uint32_t total = warp_sum_u32(r[1] - r[0]);
+    const uint32_t total = warp_sum_u32(r[1] - r[0] + cb);
     if (lane == 0) mbar_expect_tx(bar, total);
     __syncwarp();
     if (r[1] > r[0]) tma_bulk_g2s(rs + kCountHdrBytes + p.pf_off[lane], p.image + rec.off + r[0], r[1] - r[0], bar);
@@ -490,7 +534,10 @@ __global__ void __launch_bounds__(kThreads) obgpu_count_pipe_kernel(const __grid
         if (p.leaf_const != nullptr && p.leaf_const[(int64_t)blk * p.n_nodes + i] != 0) continue;
         const auto &d = desc_of(p, ents[nd.used_idx], nd.used_idx);
         // with records every leaf is lean (layout_pipe)
-        if (REC || (d.kind == K_DICT && nd.slot >= 0 && nd.op != OP_FALSE && nd.op != OP_TRUE && d.width <= 32u)) {
+        if (REC && ((p.pf_coded >> nd.used_idx) & 1)) {
+          mybm = lean_rows_coded(p, d, (smem_u32(rs) + (uint32_t)hdr[nd.used_idx]) * 8u, smem_u32(rs) + p.pf_codes[nd.used_idx],
+                                 (uint32_t)(nd.slot * p.code_words), mybm, myvalid, nwords, and_mode, lane);
+        } else if (REC || (d.kind == K_DICT && nd.slot >= 0 && nd.op != OP_FALSE && nd.op != OP_TRUE && d.width <= 32u)) {
           mybm = lean_leaf(p, nd, d, (smem_u32(rs) + (uint32_t)hdr[nd.used_idx]) * 8u, rs + hdr[nd.used_idx],
                            bitsets + nd.slot * p.bitset_words, bm, mybm, myvalid, nwords, and_mode, c.b, t, lane);
         } else {
