@@ -162,17 +162,23 @@ void obgpu_batch_close(obgpu_batch *batch);
 int obgpu_batch_block_info(const obgpu_batch *batch, int32_t block, int64_t *row_count,
                            int32_t *column_count);
 int obgpu_batch_total_rows(const obgpu_batch *batch, int64_t *total_rows);
-/* Batch string codes of store column col: the first scan that puts an EQ / NE / IN leaf on a dictionary-coded VARCHAR / CHAR
- * column (and runs the small-block count kernel on stage records) numbers the column's distinct strings once for the batch;
- * later scans evaluate the leaf over those strings instead of over every block's dictionary. state: 0 not built, 1 built
- * (n_codes distinct strings, built in build_ms of device time, paid by that first scan), or one of OBGPU_CODES_* (the column
- * keeps the per-block dictionary path). Batches opened by the host scan pipeline are scanned once and build none. */
-#define OBGPU_CODES_NOT_CODABLE (-1) /* not a dictionary string column on every block, or the image is past 2^37 bytes */
-#define OBGPU_CODES_OVER_CAP (-2)    /* more than 65536 distinct strings */
+/* Batch codes of store column col -- string and integer columns alike, despite the call's name: the first scan that puts a record
+ * leaf on a dictionary-coded column (an EQ / NE / IN leaf on a VARCHAR / CHAR column, an EQ / NE / LT / LE / GT / GE / BT leaf on
+ * a fixed-width integer one) and runs the small-block count kernel on stage records numbers the column's distinct values once for
+ * the batch; later scans evaluate the leaf over those values instead of over every block's dictionary. state: 0 not built, 1 built
+ * (n_codes distinct values, built in build_ms of device time, paid by that first scan), or one of OBGPU_CODES_* (the column
+ * keeps the per-block dictionary path). Batches opened by the host scan pipeline are scanned once and build none;
+ * OBGPU_STR_CODES=0 in the environment turns string and integer codes off. */
+#define OBGPU_CODES_NOT_CODABLE (-1) /* not a dictionary string or integer column on every block, or the image is past 2^37 bytes */
+#define OBGPU_CODES_OVER_CAP (-2)    /* more than 65536 distinct values */
 #define OBGPU_CODES_NO_MEMORY (-3)   /* the codes would not leave 1 GiB of device memory free */
 int obgpu_batch_string_codes(const obgpu_batch *batch, int32_t col, int32_t *state, int32_t *n_codes, float *build_ms);
-/* The small-block count kernel of the ctx's last scan: shared memory per warp and resident CTAs per SM (0 when it did not run). */
-int obgpu_ctx_count_layout(const obgpu_ctx *ctx, int32_t *pc_bytes, int32_t *ctas_per_sm);
+/* The small-block count kernel of the ctx's last scan: shared memory per warp, resident CTAs per SM and (kernel may be NULL) which
+ * instantiation ran, one of OBGPU_COUNT_PIPE_* (all 0 when it did not run). */
+#define OBGPU_COUNT_PIPE_PLANS 1   /* decode plans */
+#define OBGPU_COUNT_PIPE_RECORDS 2 /* stage records, every leaf lean */
+#define OBGPU_COUNT_PIPE_CODED 3   /* stage records, every filter column on batch codes: coded row passes only */
+int obgpu_ctx_count_layout(const obgpu_ctx *ctx, int32_t *pc_bytes, int32_t *ctas_per_sm, int32_t *kernel);
 /* Disk-format bytes into the block cache: n_macro_blocks macro blocks of macro_block_size bytes each (ObMacroBlock,
  * blocksstable/ob_macro_block.cpp:455-520: ObMacroBlockCommonHeader, ObSSTableMacroBlockHeader, micro-blocks back to back) are
  * validated and walked ON THE DEVICE (ObMacroBlockCommonHeader::check_integrity ob_macro_block_common_header.cpp:54-69,

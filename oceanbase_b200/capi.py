@@ -190,8 +190,9 @@ def declared_signatures():
         "obgpu_batch_close": (None, [vp]),
         "obgpu_batch_block_info": (C.c_int, [vp, i32, P(i64), P(i32)]),
         "obgpu_batch_total_rows": (C.c_int, [vp, P(i64)]),
+        # batch codes of string and integer columns alike (include/obgpu_scan.h)
         "obgpu_batch_string_codes": (C.c_int, [vp, i32, P(i32), P(i32), P(C.c_float)]),
-        "obgpu_ctx_count_layout": (C.c_int, [vp, P(i32), P(i32)]),
+        "obgpu_ctx_count_layout": (C.c_int, [vp, P(i32), P(i32), P(i32)]),
         "obgpu_scan": (C.c_int, [vp, P(ScanSpec), P(vp)]),
         "obgpu_result_free": (None, [vp]),
         "obgpu_result_info_get": (C.c_int, [vp, P(ResultInfo)]),

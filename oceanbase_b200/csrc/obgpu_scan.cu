@@ -153,12 +153,12 @@ struct ScanParams {
   // stage records instead of plans in the meta slots (pc_rec: count, pp_rec: project), and what they need from the column type
   // (about 256 bytes at the end of the block; every kernel taking ScanParams carries them, well inside the parameter space)
   const StageRec *stage;      // [n_blocks][max_cols]
-  int32_t pc_rec, pp_rec;
+  int32_t pc_rec, pp_rec, pc_all_coded;   // pc_all_coded: every filter column of the record count kernel has batch codes
   uint8_t used_sc[kMaxUsedCols], used_elem_len[kMaxUsedCols];
   uint64_t used_int_mask[kMaxUsedCols];
-  // batch string codes (batch_codes.cuh) in the record count kernel: filter column i < kCodedCols with bit i of pf_coded set stages
-  // its refs and its block's codes (at pf_codes[i] in a region slot) instead of its region; a leaf on it tests bit code[ref] of
-  // code_bits + slot * code_words, the leaf evaluated once per scan over the column's distinct strings
+  // batch codes (batch_codes.cuh) in the record count kernel: filter column i < 4 with bit i of pf_coded set stages its refs and
+  // its block's codes (at pf_codes[i] in a region slot) instead of its region; a leaf on it tests bit code[ref] of
+  // code_bits + slot * code_words, the leaf evaluated once per scan over the column's distinct values
   int32_t pf_coded, code_words;
   uint32_t pf_codes[4];
   const uint16_t *codes[4];          // [sum of r8(dict_count)] codes of every block's dictionary entries
@@ -279,8 +279,8 @@ __device__ __forceinline__ uint32_t warp_select_group(uint32_t wd, uint32_t ng, 
 // =================================================================================================
 // Predicate evaluation
 // =================================================================================================
-__device__ __forceinline__ bool int_pred(const ScanParams &p, const FilterNodeDev &nd, const ColDesc &d,
-                                         uint64_t v) {
+template <class D>
+__device__ __forceinline__ bool int_pred(const ScanParams &p, const FilterNodeDev &nd, const D &d, uint64_t v) {
   const int64_t a = cmp_image(d, v);
   if (nd.range_ok) return (((uint64_t)a - nd.lo) <= nd.span) != (nd.negate != 0);
   const bool sgn = d.sc == 1;
@@ -1799,7 +1799,8 @@ struct obgpu_ctx {
   static constexpr int kProfRing = 256;
   cudaEvent_t ev0[kProfRing] = {nullptr}, ev1[kProfRing] = {nullptr};
   int64_t prof_count = 0;
-  int32_t last_pc_bytes = 0, last_count_ctas = 0;   // small-block count kernel of the last scan (obgpu_ctx_count_layout)
+  // small-block count kernel of the last scan (obgpu_ctx_count_layout): per-warp shared memory, CTAs per SM, OBGPU_COUNT_PIPE_*
+  int32_t last_pc_bytes = 0, last_count_ctas = 0, last_count_kernel = 0;
 };
 
 // Device scratch of one host call: slices reserved with take(), then one cudaMallocAsync of their total on the ctx stream.
@@ -1825,9 +1826,9 @@ struct Scratch {
   void *release() { void *q = p; p = nullptr; return q; }
 };
 
-// Batch-wide integer codes of a string dictionary column (batch_codes.cuh): every block's dictionary entry -> the code of its
-// string among the column's distinct strings, and the code table (image byte offset << 16 | length per code).
-struct StrCodes {
+// Batch-wide codes of a dictionary column (batch_codes.cuh): every block's dictionary entry -> the code of its value among the
+// column's distinct values, and the code table (string: image byte offset, length and tag per code; integer: the value).
+struct ColCodes {
   int32_t state = 0;            // 0: not built, 1: built, < 0: the column keeps the region path (OBGPU_CODES_* reason)
   int32_t n_codes = 0;
   uint32_t refs_span = 0;       // widest refs range of a block (bytes, 16-byte aligned)
@@ -1874,8 +1875,8 @@ struct obgpu_batch {
   // CS stream codecs: blocks restated as RAW at open (stream_codecs.cuh); nullptr when nothing had to be decoded
   obcs::XformRec *d_xf = nullptr;
   std::vector<uint8_t> col_mat;        // per store index: 1 when some block rebuilt the column's strings at open (mat_codecs.cuh)
-  // batch string codes (batch_codes.cuh): per store index, built on the first scan with an EQ / NE / IN leaf on the column
-  std::vector<struct StrCodes> str_codes;
+  // batch codes (batch_codes.cuh): per store index, built on the first scan with a record leaf on the column
+  std::vector<struct ColCodes> col_codes;
   bool codes_allowed = true;           // false: batches scanned once (the host pipeline) never build codes
 };
 
@@ -1978,7 +1979,9 @@ int obgpu_ctx_create(int device, obgpu_ctx **out) {
   };
   const bool ok = opt_in((const void *)obgpu_count_kernel) && opt_in((const void *)obgpu_project_kernel<false>) && opt_in((const void *)obgpu_project_kernel<true>) &&
                   opt_in((const void *)obgpu_filter_block_kernel) && opt_in((const void *)obgpu_project_block_kernel) &&
-                  opt_in((const void *)obgpu_count_pipe_kernel<false>) && opt_in((const void *)obgpu_count_pipe_kernel<true>) &&
+                  opt_in((const void *)static_cast<void (*)(ScanParams)>(obgpu_count_pipe_kernel<false>)) &&
+                  opt_in((const void *)static_cast<void (*)(ScanParams)>(obgpu_count_pipe_kernel<true>)) &&
+                  opt_in((const void *)static_cast<void (*)(ScanParams, CodedLeaves)>(obgpu_count_pipe_kernel<true>)) &&
                   opt_in((const void *)obgpu_project_pipe_kernel<false>) && opt_in((const void *)obgpu_project_pipe_kernel<true>);
   cudaGetLastError();  // do not leave a stale (non-sticky) error for later launch checks
   if (!ok) {
@@ -2053,7 +2056,7 @@ int obgpu_ctx_kernel_times(obgpu_ctx *ctx, float *ms, int32_t cap, int32_t *n) {
 }  // extern "C"
 
 #include "batch_open.cuh"   // page-batch open: header checks, open-time rewrites of the image, decode plans
-#include "batch_codes.cuh"  // batch-wide codes of dictionary string columns, built on first use
+#include "batch_codes.cuh"  // batch-wide codes of dictionary string and integer columns, built on first use
 
 // ---- building the kernel parameter block ---------------------------------------------------------
 static int used_index(ScanParams &p, int32_t col) {
@@ -2351,7 +2354,7 @@ static void layout_smem_scan(const obgpu_batch *b, ScanParams &p, int max_smem) 
 // Small-block pipelined kernels (scan_small.cuh): which of them this scan can use, and their per-warp layouts.
 static void layout_pipe(obgpu_batch *b, ScanParams &p, int max_smem) {
   p.pipe_count = p.pipe_project = 0;
-  p.pc_rec = p.pp_rec = 0;
+  p.pc_rec = p.pp_rec = p.pc_all_coded = 0;
   if (!pipe_wanted(b->max_rows)) return;
   auto r16 = [](uint32_t v) { return (v + 15u) & ~15u; };
   // n column areas back to back in a region slot: column i (block column col(i)) at off[i], with its widest span in the batch rounded
@@ -2399,15 +2402,16 @@ static void layout_pipe(obgpu_batch *b, ScanParams &p, int max_smem) {
         if (rec) rec = p.used_sc[nd.used_idx] == 5 ? (nd.op == OP_EQ || nd.op == OP_NE || nd.op == OP_IN) : nd.range_ok != 0;
       }
       p.pc_rec = rec ? 1 : 0;
-      // batch string codes: a string filter column among the first four (every leaf on it is an EQ / NE / IN: records) stages its
-      // refs and its block's code slice instead of its region, when its codes exist or can be built now
+      // batch codes: a filter column among the first four (with records every leaf on it is a record leaf: an EQ / NE / IN on a
+      // string, a range on an integer) stages its refs and its block's code slice instead of its region, when its codes exist or can
+      // be built now
       uint32_t coded_off = off;
       p.pf_coded = 0;
-      const char *ce = getenv("OBGPU_STR_CODES");   // testing knob: 0 keeps every string leaf on its per-block dictionary
+      const char *ce = getenv("OBGPU_STR_CODES");   // testing knob: 0 keeps every leaf on its per-block dictionary
       if (rec && b->codes_allowed && !(ce && atoi(ce) == 0)) {
         uint32_t at = 0;
         for (int i = 0; i < nf; ++i) {
-          const StrCodes *sc = i < 4 && p.used_sc[i] == 5 ? &batch_codes(b, p.used_col[i]) : nullptr;
+          const ColCodes *sc = i < 4 ? &batch_codes(b, p.used_col[i]) : nullptr;
           p.pf_off[i] = at;
           if (sc && sc->state == 1) {
             p.pf_coded |= 1 << i;
@@ -2424,13 +2428,17 @@ static void layout_pipe(obgpu_batch *b, ScanParams &p, int max_smem) {
         }
         coded_off = at;
       }
+      // every filter column coded: the count kernel's CodedLeaves instantiation, which needs no bitmap, survivor or bitset scratch
+      p.pc_all_coded = rec && p.pf_coded == (1 << nf) - 1;
       p.pc_meta_bytes = kMetaPlans + (uint32_t)nf * (rec ? kCountEnt<true> : kCountEnt<false>);
       p.pc_region_bytes = kCountHdrBytes + coded_off;
       uint32_t w = 0;
       p.pc_meta = w;   w += 3u * p.pc_meta_bytes;
       p.pc_region = w; w += 2u * p.pc_region_bytes;
-      p.pc_bm = w;     w += r16(std::max(p.words_cap, 32u) * 4u) + r16(p.rows_cap * 2u);   // spilled bitmap + survivor list
-      p.pc_bitset = w; w += r16((uint32_t)p.n_slots * (uint32_t)p.bitset_words * 4u);
+      p.pc_bm = w;     // spilled bitmap + survivor list
+      if (!p.pc_all_coded) w += r16(std::max(p.words_cap, 32u) * 4u) + r16(p.rows_cap * 2u);
+      p.pc_bitset = w;
+      if (!p.pc_all_coded) w += r16((uint32_t)p.n_slots * (uint32_t)p.bitset_words * 4u);
       p.pc_bar = w;    w += 16u;
       p.pc_bytes = ((w + 127u) & ~127u) + 128u;   // slack: ragged tail words read a few refs past the staged region
       if (p.pc_bytes * (uint32_t)kWarps * 2u <= (uint32_t)max_smem) p.pipe_count = 1;   // at least two CTAs per SM
@@ -2738,7 +2746,7 @@ static int scan_common(obgpu_batch *b, const obgpu_scan_spec *spec, const obgpu_
   p.row_ids = spec->want_row_ids ? (int32_t *)(a + o_rid) : nullptr;
   p.out_cap = r->cap;
   p.code_bits = coded ? (const uint32_t *)(a + o_code_bits) : nullptr;
-  if (!coded) p.pf_coded = 0;
+  if (!coded) p.pf_coded = p.pc_all_coded = 0;
   for (int c = 0; c < spec->n_proj; ++c) {
     r->cols[c].data = a + o_data[c];
     r->cols[c].lens = r->cols[c].is_string ? (int32_t *)(a + o_lens[c]) : nullptr;
@@ -2777,26 +2785,31 @@ static int scan_common(obgpu_batch *b, const obgpu_scan_spec *spec, const obgpu_
     if (p.pipe_count) {
       const int smem = (int)(p.pc_bytes * (uint32_t)kWarps);
       int occ = 1;
-      const auto kern = p.pc_rec ? obgpu_count_pipe_kernel<true> : obgpu_count_pipe_kernel<false>;
+      const void *kern = p.pc_all_coded ? (const void *)static_cast<void (*)(ScanParams, CodedLeaves)>(obgpu_count_pipe_kernel<true>)
+                         : p.pc_rec     ? (const void *)static_cast<void (*)(ScanParams)>(obgpu_count_pipe_kernel<true>)
+                                        : (const void *)static_cast<void (*)(ScanParams)>(obgpu_count_pipe_kernel<false>);
       cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, kThreads, smem);
       ctx->last_pc_bytes = (int32_t)p.pc_bytes;
       ctx->last_count_ctas = occ;
+      ctx->last_count_kernel = p.pc_all_coded ? OBGPU_COUNT_PIPE_CODED : p.pc_rec ? OBGPU_COUNT_PIPE_RECORDS : OBGPU_COUNT_PIPE_PLANS;
       const int grid = std::min((n + kWarps - 1) / kWarps, std::max(1, occ) * ctx->sm_count);
       if (p.pc_rec && p.pf_coded) {
-        // the leaves on coded columns, once over each column's distinct strings
+        // the leaves on coded columns, once over each column's distinct values
         const int n_leaves = p.n_nodes == 1 ? 1 : p.n_nodes - 1;
         for (int i = 0; i < n_leaves; ++i) {
           const FilterNodeDev &nd = p.nodes[i];
           if (!((p.pf_coded >> nd.used_idx) & 1)) continue;
-          const StrCodes &sc = b->str_codes[(size_t)p.used_col[nd.used_idx]];
+          const ColCodes &sc = b->col_codes[(size_t)p.used_col[nd.used_idx]];
           obgpu_code_leaf_kernel<<<(p.code_words * 32 + 255) / 256, 256, 0, ctx->stream>>>(p, i, sc.d_table, sc.n_codes, p.code_words,
                                                                                           const_cast<uint32_t *>(p.code_bits) + nd.slot * p.code_words);
           ctx->launches++;
         }
       }
-      kern<<<grid, kThreads, smem, ctx->stream>>>(p);
+      if (p.pc_all_coded) obgpu_count_pipe_kernel<true><<<grid, kThreads, smem, ctx->stream>>>(p, CodedLeaves{});
+      else if (p.pc_rec) obgpu_count_pipe_kernel<true><<<grid, kThreads, smem, ctx->stream>>>(p);
+      else obgpu_count_pipe_kernel<false><<<grid, kThreads, smem, ctx->stream>>>(p);
     } else {
-      ctx->last_pc_bytes = ctx->last_count_ctas = 0;
+      ctx->last_pc_bytes = ctx->last_count_ctas = ctx->last_count_kernel = 0;
       obgpu_count_kernel<<<(n + kWarps - 1) / kWarps, kThreads, cw_total, ctx->stream>>>(p);
     }
     ctx->launches++;

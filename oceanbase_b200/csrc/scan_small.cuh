@@ -369,6 +369,13 @@ __device__ __forceinline__ int staged_ranges(const BlockRec &rec, const uint8_t 
   return nr;
 }
 
+// Byte range [lo, hi) of a coded column's refs (batch_codes.cuh) in a block of `rows` rows: 16-byte aligned, with 16 bytes of slack
+// past the last ref for the ragged tail words (as proj_ranges gives a string dictionary's refs)
+__device__ __forceinline__ void coded_refs_range(const StageRec &sr, uint32_t rows, uint32_t &lo, uint32_t &hi) {
+  lo = (sr.val_bit >> 3) & ~15u;
+  hi = (((sr.val_bit + rows * (uint32_t)sr.stride + 7u) >> 3) + 16u + 15u) & ~15u;
+}
+
 // Staged bit addresses of a string dictionary's refs (rbit) and END offsets (ibit) from the slot deltas d0, d1 of its projection
 // ranges: with two ranges they are ordered by block offset (proj_ranges); with one (d0 == d1) both are in it.
 template <class D>
@@ -433,9 +440,12 @@ __device__ __forceinline__ void warp_pipeline(int n_blocks, uint64_t *bars, int 
 // =================================================================================================
 // Count, pipelined. Per warp: meta ring (3 slots: block record + the filter columns' plans, or their stage records when
 // REC), region ring (2 slots: header with the per-column deltas + the filter columns' regions), bitmap words, predicate bitsets.
+// CODED (every filter column has batch codes, REC): a block's work is only the coded row pass of each leaf -- no lean_leaf, no
+// survivor path, no per-block bitset -- and layout_pipe gives the warp no bitmap, survivor or bitset scratch.
 // =================================================================================================
-template <bool REC>
-__global__ void __launch_bounds__(kThreads) obgpu_count_pipe_kernel(const __grid_constant__ ScanParams p) {
+template <bool REC, bool CODED>
+__device__ __forceinline__ void count_pipe(const ScanParams &p) {
+  static_assert(REC || !CODED, "batch codes are staged with stage records");
   constexpr uint32_t kEnt = kCountEnt<REC>;
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   uint8_t *wr = g_smem + (uint32_t)warp * p.pc_bytes;
@@ -468,12 +478,10 @@ __global__ void __launch_bounds__(kThreads) obgpu_count_pipe_kernel(const __grid
     uint32_t r[4] = {0, 0, 0, 0}, cb = 0;
     bool bad = false;
     if (lane < nf && rec.rows != 0 && verdict == 0) {
-      if (REC && ((p.pf_coded >> lane) & 1)) {
-        // coded column: its refs (the first projection range, or the second when the END offsets come first) and its code slice
+      if (REC && (CODED || ((p.pf_coded >> lane) & 1))) {
+        // coded column: its refs and its code slice
         const StageRec &sr = *reinterpret_cast<const StageRec *>(m + kMetaPlans + (uint32_t)lane * kEnt);
-        const bool alt = sr.lo[1] != sr.hi[1] && (sr.val_bit >> 3) >= sr.dict_payload;
-        r[0] = (uint32_t)(alt ? sr.lo[1] : sr.lo[0]) * 16u;
-        r[1] = (uint32_t)(alt ? sr.hi[1] : sr.hi[0]) * 16u;
+        coded_refs_range(sr, rec.rows, r[0], r[1]);
         cb = (((uint32_t)sr.dict_count + 7u) >> 3) * 16u;
         bad = r[1] - r[0] > p.pf_span[lane] || r[1] > ((rec.size + 15u) & ~15u) + 32u;
         if (bad) r[0] = r[1] = cb = 0;
@@ -506,14 +514,29 @@ __global__ void __launch_bounds__(kThreads) obgpu_count_pipe_kernel(const __grid
     const uint32_t nwords = (rows + 31u) >> 5;
     if (count_block_settled(p, blk, rows, gbm, (uint32_t)hdr[kPipeMaxFilterCols + 1], hdr[kPipeMaxFilterCols] != 0, lane)) return;
     const MetaEnt<REC> *ents = reinterpret_cast<const MetaEnt<REC> *>(m + kMetaPlans);
+    const bool and_mode = p.simple_shape == 1;
+    const int n_leaves = p.n_nodes == 1 ? 1 : p.n_nodes - 1;
+    if constexpr (CODED) {
+      const uint32_t myvalid = (uint32_t)lane < nwords ? valid_mask_of(rows, (uint32_t)lane) : 0u;
+      uint32_t mybm = and_mode ? myvalid : 0u;
+      for (int i = 0; i < n_leaves; ++i) {
+        const FilterNodeDev &nd = p.nodes[i];
+        if (p.leaf_const != nullptr && p.leaf_const[(int64_t)blk * p.n_nodes + i] != 0) continue;
+        mybm = lean_rows_coded(p, desc_of(p, ents[nd.used_idx], nd.used_idx), (smem_u32(rs) + (uint32_t)hdr[nd.used_idx]) * 8u,
+                               smem_u32(rs) + p.pf_codes[nd.used_idx], (uint32_t)(nd.slot * p.code_words), mybm, myvalid, nwords, and_mode, lane);
+        if (i + 1 < n_leaves && !__any_sync(0xffffffffu, and_mode ? mybm != 0u : mybm != myvalid)) break;   // early-out
+      }
+      if ((uint32_t)lane < nwords) gbm[lane] = mybm;
+      const uint32_t cnt = warp_sum_u32(__popc(mybm));
+      if (lane == 0) p.counts[blk] = cnt;
+      return;
+    }
     BlockCtx c;
     view_from_rec(rec, nullptr, c.b);
     c.descs = reinterpret_cast<const ColDesc *>(ents);
     c.bitsets = bitsets;
     c.rle_base = nullptr;
     c.rle_slot_bytes = c.rle_starts_bytes = 0;
-    const bool and_mode = p.simple_shape == 1;
-    const int n_leaves = p.n_nodes == 1 ? 1 : p.n_nodes - 1;
     // every filter column is staged: block-relative offsets of a leaf's column resolve into its region
     auto staged_at = [&](const FilterNodeDev &nd, const ColDesc &, BlockCtx &cs) {
       if (nd.op != OP_FALSE && nd.op != OP_TRUE) {
@@ -600,6 +623,18 @@ __global__ void __launch_bounds__(kThreads) obgpu_count_pipe_kernel(const __grid
   };
 
   warp_pipeline<0>(p.n_blocks, bars, lane, meta, regions, work);
+}
+
+template <bool REC>
+__global__ void __launch_bounds__(kThreads) obgpu_count_pipe_kernel(const __grid_constant__ ScanParams p) {
+  count_pipe<REC, false>(p);
+}
+// The all-coded instantiation: the tag keeps the kernel's name (obgpu_count_pipe_kernel<true>, a record-path count kernel) and
+// lets it carry its own register budget -- 10 CTAs of kThreads threads per SM
+struct CodedLeaves {};
+template <bool REC>
+__global__ void __launch_bounds__(kThreads, 10) obgpu_count_pipe_kernel(const __grid_constant__ ScanParams p, CodedLeaves) {
+  count_pipe<REC, true>(p);
 }
 
 // =================================================================================================

@@ -3,7 +3,8 @@
     python tools/scan_kernel_split.py [--part both|kernels|clocks] [--rows N] [--steps K] [--clocks-lib PATH]
 
 kernels: count / prefix / project kernel times per scan from torch.profiler (CUDA activities), in a process of its own; the count
-         kernel's shared memory per warp and CTAs per SM with and without batch string codes, and the one-time build of the codes.
+         kernel's instantiation, shared memory per warp and CTAs per SM with and without batch codes, and each string or integer
+         filter column's code state and the one-time build of its codes.
 clocks:  a library built with -DOBGPU_PIPE_CLOCKS (into a temporary directory, or --clocks-lib) stamps clock64 around each
          pipelined warp iteration of obgpu_count_pipe_kernel / obgpu_project_pipe_kernel (scan_small.cuh) and reports the share
          of a warp's loop spent waiting on its cp.async groups and mbarrier, issuing the next blocks' copies, and working on the
@@ -75,19 +76,20 @@ def part_kernels(args):
     from torch.profiler import profile, ProfilerActivity
     import oceanbase_b200 as ob
     ctx, batch, w, cap, d_image, shape = open_cfg3(args, ob)
-    # the count kernel's per-warp shared memory and CTAs per SM without batch string codes, then the scan that builds them
+    # the count kernel's instantiation, per-warp shared memory and CTAs per SM without batch codes, then the scan that builds them
     lib = ob.capi.lib
     layout = {}
-    pcb, ctas = ctypes.c_int32(), ctypes.c_int32()
-    os.environ["OBGPU_STR_CODES"] = "0"
-    scans(batch, w, cap, 1)
-    lib.obgpu_ctx_count_layout(ctx._h, ctypes.byref(pcb), ctypes.byref(ctas))
-    layout["without_codes"] = {"pc_bytes": pcb.value, "ctas_per_sm": ctas.value}
-    os.environ.pop("OBGPU_STR_CODES")
-    scans(batch, w, cap, 1)
-    lib.obgpu_ctx_count_layout(ctx._h, ctypes.byref(pcb), ctypes.byref(ctas))
-    layout["with_codes"] = {"pc_bytes": pcb.value, "ctas_per_sm": ctas.value}
-    codes = {}
+    pcb, ctas, kern = ctypes.c_int32(), ctypes.c_int32(), ctypes.c_int32()
+    kernels = {0: "not run", 1: "plans", 2: "records", 3: "all coded"}   # OBGPU_COUNT_PIPE_*
+    for key, knob in (("without_codes", "0"), ("with_codes", None)):
+        if knob is None:
+            os.environ.pop("OBGPU_STR_CODES")
+        else:
+            os.environ["OBGPU_STR_CODES"] = knob
+        scans(batch, w, cap, 1)
+        lib.obgpu_ctx_count_layout(ctx._h, ctypes.byref(pcb), ctypes.byref(ctas), ctypes.byref(kern))
+        layout[key] = {"kernel": kernels.get(kern.value, kern.value), "pc_bytes": pcb.value, "ctas_per_sm": ctas.value}
+    codes = {}   # obgpu_batch_string_codes reports string and integer columns alike
     for col in range(16):
         st, nc, bms = ctypes.c_int32(), ctypes.c_int32(), ctypes.c_float()
         if lib.obgpu_batch_string_codes(batch._h, col, ctypes.byref(st), ctypes.byref(nc), ctypes.byref(bms)) == 0 and st.value != 0:
@@ -104,7 +106,7 @@ def part_kernels(args):
             ms[name] = ms.get(name, 0.0) + e.device_time_total / 1e3 / args.steps
     batch.close()
     ctx.close()
-    return {"shape": shape, "count_layout": layout, "string_codes": codes, "kernel_ms_per_scan": {k: round(v, 4) for k, v in sorted(ms.items())},
+    return {"shape": shape, "count_layout": layout, "batch_codes": codes, "kernel_ms_per_scan": {k: round(v, 4) for k, v in sorted(ms.items())},
             "scan_kernels_ms": round(sum(ms.values()), 4), "steps": args.steps}
 
 
