@@ -318,41 +318,43 @@ static int fill_batch(obgpu_ctx *ctx, obgpu_batch *b, const void *image, int64_t
   const size_t rows_bytes = ((size_t)n_blocks * 4 + 63) & ~(size_t)63;
   const size_t rec_bytes = (size_t)n_blocks * sizeof(BlockRec);
   // stage records only where the small-block pipelined kernels can run
-  const bool pipe = pipe_wanted(b->max_rows);
+  const bool pipe = pipe_wanted(b->max_rows, scan_knobs());
   const size_t stage_bytes = pipe ? (size_t)n_blocks * b->max_cols * sizeof(StageRec) : 0;
-  constexpr size_t kSpanRows = 8;
-  CUDA_TRY(ctx, cudaMallocAsync(&dp, plan_bytes + stage_bytes + rows_bytes + rec_bytes + (size_t)b->max_cols * 4 * kSpanRows + 64, ctx->stream));
+  const size_t mc = b->max_cols;
+  CUDA_TRY(ctx, cudaMallocAsync(&dp, plan_bytes + stage_bytes + rows_bytes + rec_bytes + mc * sizeof(ColFacts) + 64, ctx->stream));
   b->d_plans = (ColDesc *)dp;
   b->d_stage = pipe ? (StageRec *)((uint8_t *)dp + plan_bytes) : nullptr;
   b->d_rows = (uint32_t *)((uint8_t *)dp + plan_bytes + stage_bytes);
   b->d_recs = (BlockRec *)((uint8_t *)dp + plan_bytes + stage_bytes + rows_bytes);
-  uint32_t *d_span = (uint32_t *)((uint8_t *)dp + plan_bytes + stage_bytes + rows_bytes + rec_bytes);
-  // per-column reductions of the index kernel: [region span][dictionary size][type min][type max][RLE runs][projection span][materialised]
-  // [stage record gaps: SR_NOT_FILTER | SR_NOT_FLAT]
-  CUDA_TRY(ctx, cudaMemsetAsync(d_span, 0, (size_t)b->max_cols * 4 * kSpanRows, ctx->stream));
-  CUDA_TRY(ctx, cudaMemsetAsync(d_span + 2 * (size_t)b->max_cols, 0xff, (size_t)b->max_cols * 4, ctx->stream));
+  ColFacts *d_facts = (ColFacts *)((uint8_t *)dp + plan_bytes + stage_bytes + rows_bytes + rec_bytes);
+  // per-column reductions of the index kernel, from zero except the type minimum
+  ColFacts init{};
+  init.type_min = 0xffffffffu;
+  std::vector<ColFacts> facts(mc, init);
+  // pageable host memory: both copies are staged synchronously by the runtime before they return
+  CUDA_TRY(ctx, cudaMemcpyAsync(d_facts, facts.data(), mc * sizeof(ColFacts), cudaMemcpyHostToDevice, ctx->stream));
   const int64_t nthreads = (int64_t)n_blocks * b->max_cols;
   obgpu_index_kernel<<<(unsigned)((nthreads + 255) / 256), 256, 0, ctx->stream>>>(
       b->d_image, b->d_blk_off, b->d_blk_size, b->d_bm_word_off, n_blocks, (int)b->max_cols, b->d_plans,
-      b->d_rows, b->d_recs, b->d_stage, d_span);
+      b->d_rows, b->d_recs, b->d_stage, d_facts);
   ctx->launches++;
   CUDA_TRY(ctx, cudaGetLastError());
-  b->col_span.assign((size_t)b->max_cols * kSpanRows, 0);
-  CUDA_TRY(ctx, cudaMemcpyAsync(b->col_span.data(), d_span, (size_t)b->max_cols * 4 * kSpanRows, cudaMemcpyDeviceToHost, ctx->stream));
-  // `stage` is pageable: the copy above is staged synchronously by the runtime before returning
+  CUDA_TRY(ctx, cudaMemcpyAsync(facts.data(), d_facts, mc * sizeof(ColFacts), cudaMemcpyDeviceToHost, ctx->stream));
   CUDA_TRY(ctx, cudaStreamSynchronize(ctx->stream));
-  const size_t mc = b->max_cols;
-  b->col_pspan.assign(b->col_span.begin() + 5 * mc, b->col_span.begin() + 6 * mc);
-  b->col_stage_gaps.assign(b->col_span.begin() + 7 * mc, b->col_span.begin() + 8 * mc);
+  b->col_span.assign(mc, 0);
+  b->col_pspan.assign(mc, 0);
+  b->col_stage_gaps.assign(mc, 0);
   b->col_mat.assign(mc, 0);
-  for (size_t c = 0; c < mc; ++c) b->col_mat[c] = b->col_span[6 * mc + c] ? 1 : 0;
   for (size_t c = 0; c < mc; ++c) {
-    b->col_max_dict[c] = b->col_span[mc + c];
-    const uint32_t tmin = b->col_span[2 * mc + c], tmax = b->col_span[3 * mc + c];
-    b->col_types[c] = tmin == 0xffffffffu ? 0 : (tmin == tmax ? (uint8_t)tmin : 0xff);   // 0xff: the blocks disagree
-    b->col_max_rle[c] = b->col_span[4 * mc + c];
+    const ColFacts &f = facts[c];
+    b->col_span[c] = f.span;
+    b->col_pspan[c] = f.pspan;
+    b->col_stage_gaps[c] = f.stage_gaps;
+    b->col_mat[c] = f.mat ? 1 : 0;
+    b->col_max_dict[c] = f.max_dict;
+    b->col_types[c] = f.type_min == 0xffffffffu ? 0 : (f.type_min == f.type_max ? (uint8_t)f.type_min : 0xff);   // 0xff: the blocks disagree
+    b->col_max_rle[c] = f.max_rle;
   }
-  b->col_span.resize(mc);
   return OBGPU_SUCCESS;
 }
 

@@ -78,6 +78,55 @@ constexpr int kParamHeap = 768;
 // layout of obcs::XformRec (stream_codecs.cuh), declared here for the kernel parameter block
 struct XformRecFwd { uint64_t orig_off; int64_t str_delta; };
 
+// ---- shared-memory layouts (bytes from the dynamic smem base), one per kernel family --------------------------------------
+// Each is filled by one host function, and only for a kernel the scan's plan launches (plan_scan). The order of the fields keeps
+// the 8-byte pairs of parameter words each kernel reads: moving a field changes the kernels' register allocation (-Xptxas -v).
+
+// Warp-private RLE scratch of a projection warp: [run values (u64)][run table at `rle`], `bytes` per warp
+struct WarpRleLayout { uint32_t rle, bytes; };
+
+// single-block kernels: [block][bitsets][rle tables][descs]
+struct BlockLayout { uint32_t bitset, rle, desc, total; };
+
+// obgpu_count_kernel, per warp: descs | bm | bitsets | staging buffer of stage_bytes
+struct alignas(8) CountCtaLayout { uint32_t desc, bm, bitset, stage, stage_bytes, bytes; };
+
+// obgpu_project_kernel: [staged block or packed column regions][scratch = sel | bm | wpre | per-warp rle | plans];
+// obgpu_project_sparse_kernel, per warp: selected-row list | one plan, sparse_warp bytes
+struct ProjCtaLayout {
+  uint32_t scratch;       // offset of the scratch
+  uint32_t total;
+  WarpRleLayout w;
+  uint32_t plans;         // inside the scratch, like sel, bm, wpre and wscr
+  int32_t compact;        // stages only the projected columns' regions (packed)
+  int32_t sparse_split;   // selectivity hint <= 1/16: sparse blocks go to the warp-per-block kernel
+  int32_t no_stage;       // blocks do not fit shared memory: every block is decoded from global memory
+  int32_t tiles;          // blocks walked by one CTA (1, or 8 with the sparse split)
+  uint32_t sel, bm, wpre, wscr;
+  uint32_t sparse_warp;
+};
+
+// obgpu_count_pipe_kernel (scan_small.cuh), per warp: 3 meta slots | 2 region slots | bm + survivors | bitsets | barriers
+struct alignas(8) CountPipeLayout {
+  // batch codes (batch_codes.cuh) in the record kernels: filter column i < 4 with bit i of `coded` set stages its refs and its
+  // block's codes (at code_at[i] in a region slot) instead of its region; a leaf on it tests bit code[ref] of
+  // ScanParams::code_bits + slot * code_words, the leaf evaluated once per scan over the column's distinct values
+  int32_t coded, code_words;
+  uint32_t code_at[4];
+  int32_t n;                          // filter columns = used columns [0, n)
+  uint32_t off[8], span[8];           // offset / capacity of a filter column's region inside a region slot
+  uint32_t meta_bytes, region_bytes;  // bytes per meta / region slot
+  uint32_t meta, region, bm, bitset, bar, bytes;
+};
+
+// obgpu_project_pipe_kernel (scan_small.cuh), per warp: 3 meta slots | 2 region slots | sel | warp scratch | barriers
+struct ProjPipeLayout {
+  uint32_t bytes;
+  uint32_t off[kMaxProj], span[kMaxProj];   // offset / capacity of a column's ranges in a region slot
+  uint32_t meta_bytes, region_bytes, hdr_bytes, bm_bytes;
+  uint32_t meta, region, sel, wscr, bar;
+  WarpRleLayout w;
+};
 
 struct ScanParams {
   const uint8_t *image;
@@ -123,48 +172,27 @@ struct ScanParams {
   const uint8_t *leaf_const;
   // blocks of a batch whose CS streams were restated as RAW at open (stream_codecs.cuh): where each block came from
   const struct XformRecFwd *xf;
-  // ---- shared-memory layout (bytes from the dynamic smem base) -------------------------------------
-  // single-block kernels: [block][bitsets][rle tables][descs]
-  // project kernel:       [staged block or column regions][bitsets][scratch = sel|bm|wpre|per-warp rle|plans]
-  uint32_t stage_bytes;       // project kernel: bytes of the staged block or column regions
-  uint32_t smem_bitset;
-  uint32_t smem_rle, smem_desc;            // single-block kernels
-  uint32_t smem_scratch, scratch_bytes;    // project kernel
-  uint32_t cw_desc, cw_bm, cw_bitset, cw_stage, cw_stage_bytes, cw_bytes;  // count kernel, per-warp: descs | bm | bitsets | stage
-  uint32_t pw_rle, pw_bytes;            // project kernel, per-warp region at off_desc: run values (u64) | RLE run table
-  uint32_t off_plans;                   // project kernel: the block's n_proj decode plans (ColDesc), prefetched
-  int32_t compact;                      // project kernel stages only the projected columns' regions (packed)
-  int32_t sparse_split;                 // selectivity hint <= 1/16: sparse blocks go to the warp-per-block kernel
-  int32_t no_stage;                     // blocks do not fit shared memory: every block is decoded from global memory
-  int32_t proj_tiles;                   // blocks walked by one CTA of the project kernel (1, or 8 with the sparse split)
-  uint32_t off_sel, off_bm, off_wpre, off_desc;  // inside one scratch
-  uint32_t smem_total;
-  // ---- small-block pipelined kernels (scan_small.cuh): warp per block, cp.async rings ----------------------------
-  int32_t pipe_count, pipe_project;         // which of the two kernels this scan uses
-  int32_t pf_n;                             // filter columns = used columns [0, pf_n)
-  uint32_t pf_off[8], pf_span[8];           // count: offset / capacity of a filter column's region inside a region slot
-  uint32_t pc_meta_bytes, pc_region_bytes;  // count: bytes per meta / region slot
-  uint32_t pc_meta, pc_region, pc_bm, pc_bitset, pc_bar, pc_bytes;   // count: per-warp layout
-  uint32_t pp_off[kMaxProj], pp_span[kMaxProj];              // project: offset / capacity of a column's ranges in a region slot
-  uint32_t pp_meta_bytes, pp_region_bytes, pp_hdr_bytes, pp_bm_bytes;
-  uint32_t pp_meta, pp_region, pp_sel, pp_wscr, pp_bar, pp_bytes;    // project: per-warp layout
-  uint32_t rle_slot_bytes;    // bytes per run-table slot: mask[words_cap] (u32) + pre[words_cap] (u16)
+  // ---- shared-memory layouts -------------------------------------------------------------------------------------
+  // facts every layout shares (assign_rle_slots)
   uint32_t rows_cap, words_cap;
-  // stage records instead of plans in the meta slots (pc_rec: count, pp_rec: project), and what they need from the column type
+  uint32_t rle_slot_bytes;    // bytes per run-table slot: mask[words_cap] (u32) + pre[words_cap] (u16)
+  BlockLayout blk;            // single-block kernels
+  CountCtaLayout cw;          // obgpu_count_kernel
+  ProjCtaLayout cp;           // obgpu_project_kernel, obgpu_project_sparse_kernel
+  CountPipeLayout pc;         // obgpu_count_pipe_kernel: warp per block, cp.async rings
+  ProjPipeLayout pp;          // obgpu_project_pipe_kernel
+  // stage records instead of plans in the meta slots of the pipelined kernels, and what they need from the column type
   // (about 256 bytes at the end of the block; every kernel taking ScanParams carries them, well inside the parameter space)
   const StageRec *stage;      // [n_blocks][max_cols]
-  int32_t pc_rec, pp_rec, pc_all_coded;   // pc_all_coded: every filter column of the record count kernel has batch codes
   uint8_t used_sc[kMaxUsedCols], used_elem_len[kMaxUsedCols];
   uint64_t used_int_mask[kMaxUsedCols];
-  // batch codes (batch_codes.cuh) in the record count kernel: filter column i < 4 with bit i of pf_coded set stages its refs and
-  // its block's codes (at pf_codes[i] in a region slot) instead of its region; a leaf on it tests bit code[ref] of
-  // code_bits + slot * code_words, the leaf evaluated once per scan over the column's distinct values
-  int32_t pf_coded, code_words;
-  uint32_t pf_codes[4];
+  // batch codes of the coded filter columns (CountPipeLayout::coded)
   const uint16_t *codes[4];          // [sum of r8(dict_count)] codes of every block's dictionary entries
   const uint32_t *code_off16[4];     // [n_blocks] first code of a block, in 16-byte units
   const uint32_t *code_bits;
 };
+// every scan kernel takes the block by value (__grid_constant__): keep it from growing
+static_assert(sizeof(ScanParams) <= 3840, "ScanParams grew");
 
 // =================================================================================================
 // PTX helpers: mbarrier + TMA bulk copy, acquire/release descriptor access
@@ -1039,10 +1067,10 @@ __device__ __forceinline__ void project_str_col(const ScanParams &p, const Block
 
 // One projected column of one block decoded by ONE WARP from the staged image (c.b.s / c.sbit already point at the
 // column's staged bytes): RLE columns get their run table (and, for 8-byte integers, their run values) in the warp's
-// private scratch `wscr` first. Shared by the CTA-per-block and the warp-per-block projection kernels.
+// private scratch `wscr` (run table at wscr + wrle) first. Shared by the CTA-per-block and the warp-per-block projection kernels.
 __device__ __forceinline__ void project_column_staged(const ScanParams &p, BlockCtx &c, ColDesc *wdesc, int pc, const uint16_t *sel,
                                                       uint32_t cnt, int64_t base, uint64_t blk_addr, bool all_rows, uint32_t rows,
-                                                      uint8_t *wscr, const Team &t) {
+                                                      uint8_t *wscr, uint32_t wrle, const Team &t) {
   const int lane = t.lane;
   const ColDesc &d = *wdesc;
   if (!d.ok) {
@@ -1055,8 +1083,8 @@ __device__ __forceinline__ void project_column_staged(const ScanParams &p, Block
       return;
     }
     if (lane == 0) wdesc->rle_slot = 0;
-    rle_table_build(c.b.s, d, rows, reinterpret_cast<uint32_t *>(wscr + p.pw_rle),
-                    reinterpret_cast<uint16_t *>(wscr + p.pw_rle + c.rle_starts_bytes), t);
+    rle_table_build(c.b.s, d, rows, reinterpret_cast<uint32_t *>(wscr + wrle),
+                    reinterpret_cast<uint16_t *>(wscr + wrle + c.rle_starts_bytes), t);
     const uint32_t n = d.rle_count;
     if (d.sc != 5 && d.elem_len == 8) {
       // integer RLE column: decode each RUN once (value of run k), rows then only look up their run
@@ -1148,13 +1176,27 @@ __device__ __forceinline__ uint32_t stage_rec_of(const ColDesc &d, const BlockVi
   return no;
 }
 
+// What the index kernel reduces over a batch's blocks for one column (atomicMax unless noted)
+struct ColFacts {
+  uint32_t span;         // bytes of the column's region (count kernel staging buffer, project kernel column staging);
+                         // 0xffffffff: no single region (CS string bytes), whole-block staging only
+  uint32_t max_dict;     // dictionary size + 2 of dictionary-coded columns (predicate bitset words)
+  uint32_t type_min;     // ObObjType, atomicMin (starts at 0xffffffff): equal to type_max when the blocks agree
+  uint32_t type_max;
+  uint32_t max_rle;      // largest RLE run count (sizes the run tables)
+  uint32_t pspan;        // bytes a projection of the column stages (scan_small.cuh: VARCHAR dictionaries without their string bytes)
+  uint32_t mat;          // 1: strings that exist only in this batch's copy of some block (mat_codecs.cuh)
+  uint32_t stage_gaps;   // SR_NOT_FILTER / SR_NOT_FLAT if some block's stage record cannot serve that path (atomicOr)
+};
+
 __global__ void __launch_bounds__(256) obgpu_index_kernel(const uint8_t *image, const uint64_t *blk_off,
                                                           const uint32_t *blk_size, const int64_t *bm_word_off,
                                                           int n_blocks, int max_cols, ColDesc *plans, uint32_t *rows,
-                                                          BlockRec *recs, StageRec *stage, uint32_t *col_span) {
+                                                          BlockRec *recs, StageRec *stage, ColFacts *facts) {
   const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= (int64_t)n_blocks * max_cols) return;
   const int block = (int)(i / max_cols), col = (int)(i % max_cols);
+  ColFacts &f = facts[col];
   BlockView b;
   parse_block(image + blk_off[block], blk_size[block], b);
   ColDesc d{};
@@ -1167,7 +1209,7 @@ __global__ void __launch_bounds__(256) obgpu_index_kernel(const uint8_t *image, 
     const uint32_t no = stage_rec_of(d, b, sr);
     stage[i] = sr;
     // the bits are set by the first blocks that lack them: later blocks read them instead of queueing on one address
-    uint32_t *gaps = &col_span[7 * max_cols + col];
+    uint32_t *gaps = &f.stage_gaps;
     if (b.ok && (*(volatile uint32_t *)gaps & no) != no) atomicOr(gaps, no);
   }
   if (col == 0) {
@@ -1188,28 +1230,22 @@ __global__ void __launch_bounds__(256) obgpu_index_kernel(const uint8_t *image, 
     recs[block] = r;
   }
   if (d.ok) {
-    // bytes of the column's region (count kernel staging buffer, project kernel column staging)
     uint32_t lo, hi;
-    if (col_region(d, b, lo, hi)) atomicMax(&col_span[col], hi - lo);
-    else atomicMax(&col_span[col], 0xffffffffu);   // no single region (CS string bytes): whole-block staging only
-    // dictionary size (predicate bitset words) of dictionary-coded columns: col_span[max_cols + col]
-    if (is_dict_kind(d)) atomicMax(&col_span[max_cols + col], d.dict_count + 2u);
-    // bytes a projection of the column stages (scan_small.cuh: VARCHAR dictionaries without their string bytes)
-    atomicMax(&col_span[5 * max_cols + col], proj_ranges_bytes(d, b));
-    // strings that exist only in this batch's copy of the block (HEX_PACKING / STRING_DIFF / STRING_PREFIX, mat_codecs.cuh)
-    if (d.kind == K_CSSTR && !b.is_cs) atomicMax(&col_span[6 * max_cols + col], 1u);
+    atomicMax(&f.span, col_region(d, b, lo, hi) ? hi - lo : 0xffffffffu);
+    if (is_dict_kind(d)) atomicMax(&f.max_dict, d.dict_count + 2u);
+    atomicMax(&f.pspan, proj_ranges_bytes(d, b));
+    // HEX_PACKING / STRING_DIFF / STRING_PREFIX
+    if (d.kind == K_CSSTR && !b.is_cs) atomicMax(&f.mat, 1u);
   }
   if (b.ok && (uint32_t)col < b.column_count) {
-    // per-column facts the host keeps for a batch: ObObjType (min / max over the blocks: equal when the blocks
-    // agree) and the largest RLE run count (sizes the run tables)
     const uint8_t *s = image + blk_off[block];
     const uint32_t t = b.is_cs ? s[b.header_size + 12u + 4u * (uint32_t)col + 3u] : s[b.header_size + 16u * (uint32_t)col + 3u];
-    atomicMin(&col_span[2 * max_cols + col], t);
-    atomicMax(&col_span[3 * max_cols + col], t);
+    atomicMin(&f.type_min, t);
+    atomicMax(&f.type_max, t);
     if (!b.is_cs && s[b.header_size + 16u * (uint32_t)col + 1u] == COL_RLE) {
       const uint32_t off = ld32(s, b.header_size + 16u * (uint32_t)col + 8u);
       if (off <= b.size && b.meta_off <= b.size - off && b.meta_off + off + 10u <= b.size)
-        atomicMax(&col_span[4 * max_cols + col], (uint32_t)ld_bytes(s, b.meta_off + off + 2u, 4));
+        atomicMax(&f.max_rle, (uint32_t)ld_bytes(s, b.meta_off + off + 2u, 4));
     }
   }
 }
@@ -1224,10 +1260,10 @@ __global__ void __launch_bounds__(kThreads) obgpu_count_kernel(const __grid_cons
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const int block = blockIdx.x * kWarps + warp;
   if (block >= p.n_blocks) return;
-  uint8_t *wr = g_smem + (uint32_t)warp * p.cw_bytes;
-  ColDesc *descs = reinterpret_cast<ColDesc *>(wr + p.cw_desc);
-  uint32_t *bm = reinterpret_cast<uint32_t *>(wr + p.cw_bm);
-  uint32_t *bitsets = reinterpret_cast<uint32_t *>(wr + p.cw_bitset);
+  uint8_t *wr = g_smem + (uint32_t)warp * p.cw.bytes;
+  ColDesc *descs = reinterpret_cast<ColDesc *>(wr + p.cw.desc);
+  uint32_t *bm = reinterpret_cast<uint32_t *>(wr + p.cw.bm);
+  uint32_t *bitsets = reinterpret_cast<uint32_t *>(wr + p.cw.bitset);
   const Team t = warp_team(lane);
 
   const BlockRec rec = p.recs[block];
@@ -1265,16 +1301,16 @@ __global__ void __launch_bounds__(kThreads) obgpu_count_kernel(const __grid_cons
   }
   uint32_t cnt = 0;
   if (p.simple_shape != 0) {
-    uint8_t *stage = wr + p.cw_stage;
+    uint8_t *stage = wr + p.cw.stage;
     int staged_idx = -1;  // used-column index currently held by the staging buffer
     BlockCtx cs = c;
     cnt = leaf_list_over_words(p, c, cs, block, bm, gbm, rows, nwords, t, [&](const FilterNodeDev &nd, const ColDesc &d, BlockCtx &cs) {
       // stage the leaf column's region (ext bits, values / refs, run arrays, dictionary): every lane pulls 16-byte
       // pieces, 4 loads in flight per lane; all later reads hit shared memory
       if (staged_idx == nd.used_idx) return true;
-      if (p.cw_stage_bytes == 0 || nd.op == OP_FALSE || nd.op == OP_TRUE) return false;
+      if (p.cw.stage_bytes == 0 || nd.op == OP_FALSE || nd.op == OP_TRUE) return false;
       uint32_t lo, hi;
-      if (!col_region(d, c.b, lo, hi) || hi - lo > p.cw_stage_bytes || hi <= lo) {
+      if (!col_region(d, c.b, lo, hi) || hi - lo > p.cw.stage_bytes || hi <= lo) {
         staged_idx = -1;
         return false;
       }
@@ -1395,16 +1431,16 @@ __global__ void __launch_bounds__(kThreads) obgpu_project_kernel(const __grid_co
   __shared__ int32_t s_delta[kMaxProj];
 
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  uint8_t *scr = g_smem + p.smem_scratch;
-  uint16_t *sel = reinterpret_cast<uint16_t *>(scr + p.off_sel);
-  uint32_t *bm = reinterpret_cast<uint32_t *>(scr + p.off_bm);
-  uint32_t *wpre = reinterpret_cast<uint32_t *>(scr + p.off_wpre);
+  uint8_t *scr = g_smem + p.cp.scratch;
+  uint16_t *sel = reinterpret_cast<uint16_t *>(scr + p.cp.sel);
+  uint32_t *bm = reinterpret_cast<uint32_t *>(scr + p.cp.bm);
+  uint32_t *wpre = reinterpret_cast<uint32_t *>(scr + p.cp.wpre);
   // One block per CTA normally; with the sparse split most blocks belong to the warp-per-block kernel, so a CTA
-  // walks p.proj_tiles consecutive blocks and only works on the dense ones (far fewer CTAs to launch and retire).
+  // walks p.cp.tiles consecutive blocks and only works on the dense ones (far fewer CTAs to launch and retire).
   // Blocks are visited last-to-first: the count kernel has just walked the batch front to back, so the
   // filter-column bytes of the LAST blocks are the ones still sitting in L2.
   bool used_bar = false;
-  const int ntiles = MULTI ? p.proj_tiles : 1;  // MULTI = false: the loop and its bookkeeping compile away
+  const int ntiles = MULTI ? p.cp.tiles : 1;  // MULTI = false: the loop and its bookkeeping compile away
   for (int it = 0; it < ntiles; ++it) {
     const int lin = (int)blockIdx.x * ntiles + it;
     if (lin >= p.n_blocks) break;
@@ -1431,19 +1467,19 @@ __global__ void __launch_bounds__(kThreads) obgpu_project_kernel(const __grid_co
     // Few selected rows: staging the block would move far more bytes than the cells that are read. Such a
     // block is decoded straight from global memory (generic loads, a handful of sectors per column).
     const bool few = (uint64_t)cnt * 16u <= rows;
-    if (few && p.sparse_split) continue;   // obgpu_project_sparse_kernel owns this block
-    const bool sparse = few || p.no_stage != 0;
+    if (few && p.cp.sparse_split) continue;   // obgpu_project_sparse_kernel owns this block
+    const bool sparse = few || p.cp.no_stage != 0;
     if (tid == 0) {
       if (used_bar) mbar_inval(&s_bar);  // a block handled earlier by this CTA left the barrier initialised
       mbar_init(&s_bar, 1);
       fence_barrier_init();
-      if (!p.compact && !sparse) {
+      if (!p.cp.compact && !sparse) {
         mbar_expect_tx(&s_bar, (size + 15u) & ~15u);
         tma_bulk_g2s(g_smem, p.image + rec.off, (size + 15u) & ~15u, &s_bar);
       }
       s_next = 0;
     }
-    ColDesc *plans_s = reinterpret_cast<ColDesc *>(scr + p.off_plans);
+    ColDesc *plans_s = reinterpret_cast<ColDesc *>(scr + p.cp.plans);
     constexpr int kPieces = (int)(sizeof(ColDesc) / 16);
     const int npieces = p.n_proj * kPieces;
     uint4 pv0{}, pv1{};
@@ -1463,7 +1499,7 @@ __global__ void __launch_bounds__(kThreads) obgpu_project_kernel(const __grid_co
     __syncthreads();  // barrier object, queue and plans initialised before anyone uses them
     BlockCtx c;
     view_from_rec(rec, sparse ? p.image + rec.off : g_smem, c.b);
-    if (p.compact && !sparse) {
+    if (p.cp.compact && !sparse) {
       // Only the projected columns' regions are staged, packed back to back: lane pc of warp 0 issues
       // the bulk copy of column pc; s_delta[pc] = (offset in shared memory) - (offset in the block), so
       // block-relative addressing keeps working once the base is shifted by it.
@@ -1528,9 +1564,9 @@ __global__ void __launch_bounds__(kThreads) obgpu_project_kernel(const __grid_co
     c.sbit = smem_u32(g_smem) * 8u;
     c.bitsets = nullptr;
     // warp-private scratch: [run values][RLE run table]
-    uint8_t *wscr = scr + p.off_desc + (uint32_t)warp * p.pw_bytes;
+    uint8_t *wscr = scr + p.cp.wscr + (uint32_t)warp * p.cp.w.bytes;
     c.descs = plans_s;
-    c.rle_base = wscr + p.pw_rle;
+    c.rle_base = wscr + p.cp.w.rle;
     c.rle_slot_bytes = 0;  // one table per warp: slot 0
     c.rle_starts_bytes = p.words_cap * 4u;
 
@@ -1552,12 +1588,12 @@ __global__ void __launch_bounds__(kThreads) obgpu_project_kernel(const __grid_co
         __syncwarp();
         continue;
       }
-      if (p.compact) {  // rebase onto this column's staged region
+      if (p.cp.compact) {  // rebase onto this column's staged region
         const int32_t delta = s_delta[pc];
         c.b.s = g_smem + delta;
         c.sbit = (smem_u32(g_smem) + (uint32_t)delta) * 8u;
       }
-      project_column_staged(p, c, wdesc, pc, sel, cnt, base, blk_addr, all_rows, rows, wscr, t);
+      project_column_staged(p, c, wdesc, pc, sel, cnt, base, blk_addr, all_rows, rows, wscr, p.cp.w.rle, t);
       __syncwarp();
     }
     used_bar = true;
@@ -1583,10 +1619,9 @@ __global__ void __launch_bounds__(kThreads) obgpu_project_sparse_kernel(const __
     if (lane == 0) atomicOr(p.status, ST_OVERFLOW);
     return;
   }
-  const uint32_t sel_cap = p.rows_cap / 16u + 32u;
-  uint8_t *wr = g_smem + (uint32_t)warp * (((sel_cap * 2u + 15u) & ~15u) + (uint32_t)sizeof(ColDesc));
+  uint8_t *wr = g_smem + (uint32_t)warp * p.cp.sparse_warp;
   uint16_t *sel = reinterpret_cast<uint16_t *>(wr);
-  ColDesc *wdesc = reinterpret_cast<ColDesc *>(wr + ((sel_cap * 2u + 15u) & ~15u));
+  ColDesc *wdesc = reinterpret_cast<ColDesc *>(wr + p.cp.sparse_warp - (uint32_t)sizeof(ColDesc));
   // bitmap words -> ascending selected-row list
   const uint32_t *gbm = p.bitmap_words + rec.bm_word_off;
   const uint32_t nwords = (rows + 31u) >> 5;
@@ -1638,8 +1673,8 @@ __global__ void __launch_bounds__(kThreads) obgpu_filter_block_kernel(const __gr
                                                                       uint8_t *out_bytes) {
   __shared__ __align__(8) uint64_t s_bar;
   const Team t = cta_team();
-  uint32_t *bitsets = reinterpret_cast<uint32_t *>(g_smem + p.smem_bitset);
-  ColDesc *descs = reinterpret_cast<ColDesc *>(g_smem + p.smem_desc);
+  uint32_t *bitsets = reinterpret_cast<uint32_t *>(g_smem + p.blk.bitset);
+  ColDesc *descs = reinterpret_cast<ColDesc *>(g_smem + p.blk.desc);
   if (t.tid == 0) {
     mbar_init(&s_bar, 1);
     fence_barrier_init();
@@ -1650,7 +1685,7 @@ __global__ void __launch_bounds__(kThreads) obgpu_filter_block_kernel(const __gr
   BlockCtx c;
   c.bitsets = bitsets;
   bool corrupt;
-  bool ok = prepare_block(p, 0, size, descs, g_smem + p.smem_rle, t, c, corrupt);
+  bool ok = prepare_block(p, 0, size, descs, g_smem + p.blk.rle, t, c, corrupt);
   if (ok && (start < 0 || start + count > (int64_t)c.b.row_count)) {
     ok = false;
     corrupt = true;
@@ -1677,7 +1712,7 @@ __global__ void __launch_bounds__(kThreads) obgpu_project_block_kernel(
     void *data, int32_t *lens, uint32_t *nulls, int32_t elem_len) {
   __shared__ __align__(8) uint64_t s_bar;
   const Team t = cta_team();
-  ColDesc *descs = reinterpret_cast<ColDesc *>(g_smem + p.smem_desc);
+  ColDesc *descs = reinterpret_cast<ColDesc *>(g_smem + p.blk.desc);
   if (t.tid == 0) {
     mbar_init(&s_bar, 1);
     fence_barrier_init();
@@ -1688,7 +1723,7 @@ __global__ void __launch_bounds__(kThreads) obgpu_project_block_kernel(
   BlockCtx c;
   c.bitsets = nullptr;
   bool corrupt;
-  if (!prepare_block(p, 0, size, descs, g_smem + p.smem_rle, t, c, corrupt)) {
+  if (!prepare_block(p, 0, size, descs, g_smem + p.blk.rle, t, c, corrupt)) {
     if (t.tid == 0) atomicOr(p.status, corrupt ? ST_CORRUPT : ST_UNSUPPORTED);
     return;
   }
@@ -1880,13 +1915,16 @@ struct obgpu_batch {
   bool codes_allowed = true;           // false: batches scanned once (the host pipeline) never build codes
 };
 
-// Whether a scan of the batch may take the small-block pipelined kernels (scan_small.cuh): fill_batch builds stage records
-// for such batches, layout_pipe chooses the kernels
-static bool pipe_wanted(uint32_t max_rows) {
-  bool want = max_rows <= 512;
-  if (const char *e = getenv("OBGPU_PIPE")) want = atoi(e) != 0;   // testing knob: force the path on / off
-  return want;
+// Testing knobs (nullptr: not set), read here only, that force a kernel path so tests reach every path on small inputs: OBGPU_PIPE
+// (small-block pipelined kernels on / off), OBGPU_PROJECT_COMPACT (0: stage whole blocks, 1: only the projected columns' regions),
+// OBGPU_STR_CODES (0: no batch codes) and OBGPU_SPARSE_SPLIT (sparse split on / off)
+struct ScanKnobs { const char *pipe, *project_compact, *str_codes, *sparse_split; };
+static ScanKnobs scan_knobs() {
+  return {getenv("OBGPU_PIPE"), getenv("OBGPU_PROJECT_COMPACT"), getenv("OBGPU_STR_CODES"), getenv("OBGPU_SPARSE_SPLIT")};
 }
+
+// Whether a scan may take the small-block pipelined kernels (scan_small.cuh): fill_batch builds stage records, plan_scan chooses
+static bool pipe_wanted(uint32_t max_rows, const ScanKnobs &k) { return k.pipe ? atoi(k.pipe) != 0 : max_rows <= 512; }
 
 struct ResultCol {
   void *data = nullptr;
@@ -2250,10 +2288,15 @@ static int build_filter(obgpu_ctx *ctx, const obgpu_batch *b, const obgpu_filter
   return OBGPU_SUCCESS;
 }
 
-// run-table slots for used columns that are RLE-coded in some block
+// The kernels of one scan (plan_scan). The pipelined count kernels are numbered as obgpu_ctx_count_layout reports them.
+enum ScanCount { COUNT_NONE = 0, COUNT_PIPE_PLANS = OBGPU_COUNT_PIPE_PLANS, COUNT_PIPE_RECORDS = OBGPU_COUNT_PIPE_RECORDS,
+                 COUNT_PIPE_CODED = OBGPU_COUNT_PIPE_CODED, COUNT_CTA, COUNT_BITMAP };
+enum ScanProj { PROJ_NONE, PROJ_CTA, PROJ_CTA_SPARSE, PROJ_PIPE_PLANS, PROJ_PIPE_RECORDS };
+struct ScanPlan { ScanCount count; ScanProj proj; };
+
+// run-table slots for used columns that are RLE-coded in some block, and the row capacity every layout is sized by
 static void assign_rle_slots(const obgpu_batch *b, ScanParams &p) {
-  p.n_rle_slots = 0;
-  p.rle_runs_cap = 0;
+  p.n_rle_slots = p.rle_runs_cap = 0;
   for (int i = 0; i < kMaxUsedCols; ++i) p.used_rle_slot[i] = -1;
   for (int i = 0; i < p.n_used; ++i) {
     const size_t col = (size_t)p.used_col[i];
@@ -2262,214 +2305,242 @@ static void assign_rle_slots(const obgpu_batch *b, ScanParams &p) {
       p.rle_runs_cap = std::max<int32_t>(p.rle_runs_cap, (int32_t)std::min<uint32_t>(b->col_max_rle[col], 65535u));
     }
   }
-  const uint32_t rows_cap = std::max<uint32_t>(b->max_rows, 32u);
-  p.rows_cap = rows_cap;
-  p.words_cap = (rows_cap + 31u) / 32u;
+  p.rows_cap = std::max<uint32_t>(b->max_rows, 32u);
+  p.words_cap = (p.rows_cap + 31u) / 32u;
   p.rle_slot_bytes = p.n_rle_slots > 0 ? ((p.words_cap * 6u + 15u) & ~15u) : 0u;
 }
+
+static uint32_t r16(uint32_t v) { return (v + 15u) & ~15u; }
+static uint32_t r128(uint32_t v) { return (v + 127u) & ~127u; }
+static uint32_t bitset_bytes(const ScanParams &p) { return r16((uint32_t)p.n_slots * (uint32_t)p.bitset_words * 4u); }
 
 // single-block kernels: [block][bitsets][rle tables][descs]
 static void layout_smem(const obgpu_batch *b, ScanParams &p) {
   assign_rle_slots(b, p);
-  uint32_t off = (b->max_block_bytes + 16u + 127u) & ~127u;
-  p.smem_bitset = off; off += ((uint32_t)p.n_slots * (uint32_t)p.bitset_words * 4u + 15u) & ~15u;
-  p.smem_rle = off;   off += (uint32_t)p.n_rle_slots * p.rle_slot_bytes;
-  p.smem_desc = off;  off += (uint32_t)sizeof(ColDesc) * (uint32_t)std::max(p.n_used, 1);
-  p.smem_total = (off + 15u) & ~15u;
+  uint32_t off = r128(b->max_block_bytes + 16u);
+  p.blk.bitset = off; off += bitset_bytes(p);
+  p.blk.rle = off;    off += (uint32_t)p.n_rle_slots * p.rle_slot_bytes;
+  p.blk.desc = off;   off += (uint32_t)sizeof(ColDesc) * (uint32_t)std::max(p.n_used, 1);
+  p.blk.total = r16(off);
 }
 
-// project kernel: [staged block or packed column regions][bitsets][scratch = sel|bm|wpre|per-warp rle|plans];
-// count kernel: per warp descs | bm | bitsets | staging buffer
-static void layout_smem_scan(const obgpu_batch *b, ScanParams &p, int max_smem) {
-  assign_rle_slots(b, p);
-  p.no_stage = 0;
-  p.stage_bytes = (b->max_block_bytes + 16u + 127u) & ~127u;
-  {
-    // stage only the projected columns when that is clearly less than the whole block (upper bound:
-    // per-column maximum region over the batch's blocks)
-    uint64_t sum = 0;
-    bool known = p.n_proj > 0;
-    for (int i = 0; i < p.n_proj && known; ++i) {
-      const size_t col = (size_t)p.used_col[p.proj_used[i]];
-      if (col >= b->col_span.size() || b->col_span[col] == 0xffffffffu) known = false;   // no single region (CS string bytes)
-      else sum += b->col_span[col];
-    }
-    p.compact = 0;
-    if (known && sum * 4 <= (uint64_t)p.stage_bytes * 3) {
-      p.compact = 1;
-      p.stage_bytes = ((uint32_t)sum + 127u) & ~127u;
-    }
-    if (const char *e = getenv("OBGPU_PROJECT_COMPACT")) {  // testing knob: force either mode
-      const int want = atoi(e);
-      if (want == 0) { p.compact = 0; p.stage_bytes = (b->max_block_bytes + 16u + 127u) & ~127u; }
-      else if (known && want == 1) { p.compact = 1; p.stage_bytes = ((uint32_t)sum + 127u) & ~127u; }
-    }
-  }
-  uint32_t off = p.stage_bytes;
-  p.smem_bitset = off; off += ((uint32_t)p.n_slots * (uint32_t)p.bitset_words * 4u + 15u) & ~15u;
-  uint32_t s = 0;
-  p.off_sel = s;  s += (p.rows_cap * 2u + 15u) & ~15u;
-  p.off_bm = s;   s += (p.words_cap * 4u + 15u) & ~15u;
-  p.off_wpre = s; s += (p.words_cap * 4u + 15u) & ~15u;
-  p.pw_rle = p.n_rle_slots > 0 ? (((uint32_t)p.rle_runs_cap + 2u) * 8u) : 0u;
-  p.pw_bytes = (p.pw_rle + (p.n_rle_slots > 0 ? p.words_cap * 6u : 0u) + 15u) & ~15u;
-  p.off_desc = s; s += p.pw_bytes * (uint32_t)kWarps;
-  p.off_plans = s; s += (uint32_t)sizeof(ColDesc) * (uint32_t)std::max(p.n_proj, 1);
-  p.scratch_bytes = (s + 127u) & ~127u;
-  p.smem_scratch = (off + 127u) & ~127u;
-  p.smem_total = p.smem_scratch + p.scratch_bytes;
-  if ((int)p.smem_total > max_smem && p.stage_bytes > 0) {
-    // the blocks (or the projected column regions) do not fit next to the scratch: no staging at all, and
-    // no per-warp run tables either (the global path looks runs up by binary search)
-    p.no_stage = 1;
-    p.compact = 0;
-    p.stage_bytes = 0;
-    p.smem_bitset = 0;
-    p.pw_rle = p.pw_bytes = 0;
-    uint32_t s2 = p.off_desc;          // sel | bm | wpre stay where they are
-    p.off_plans = s2; s2 += (uint32_t)sizeof(ColDesc) * (uint32_t)std::max(p.n_proj, 1);
-    p.scratch_bytes = (s2 + 127u) & ~127u;
-    p.smem_scratch = ((((uint32_t)p.n_slots * (uint32_t)p.bitset_words * 4u + 15u) & ~15u) + 127u) & ~127u;
-    p.smem_total = p.smem_scratch + p.scratch_bytes;
-  }
-  // count kernel, per warp: descs | bm | bitsets
+// Warp scratch of both projection kernels: run values of an 8-byte integer RLE column, then its run table
+static WarpRleLayout warp_rle(const ScanParams &p) {
+  if (p.n_rle_slots == 0) return {0u, 0u};
+  const uint32_t rle = ((uint32_t)p.rle_runs_cap + 2u) * 8u;
+  return {rle, r16(rle + p.words_cap * 6u)};
+}
+
+// obgpu_count_kernel, per warp: descs | bm | bitsets | staging buffer for one filter column's region at a time (coalesced
+// 16-byte loads); a column whose region exceeds the per-warp budget is read from global memory directly
+static void layout_count_cta(const obgpu_batch *b, ScanParams &p) {
   uint32_t w = 0;
-  p.cw_desc = w;   w += ((uint32_t)sizeof(ColDesc) * (uint32_t)std::max(p.n_used, 1) + 15u) & ~15u;
-  p.cw_bm = w;     w += (p.words_cap * 4u + 15u) & ~15u;
-  p.cw_bitset = w; w += ((uint32_t)p.n_slots * (uint32_t)p.bitset_words * 4u + 15u) & ~15u;
-  // staging buffer for one filter column's region at a time (coalesced 16-byte loads); a column whose
-  // region exceeds the per-warp budget is read from global memory directly
+  p.cw.desc = w;   w += r16((uint32_t)sizeof(ColDesc) * (uint32_t)std::max(p.n_used, 1));
+  p.cw.bm = w;     w += r16(p.words_cap * 4u);
+  p.cw.bitset = w; w += bitset_bytes(p);
   uint32_t span = 0;
   for (int i = 0; i < p.n_used; ++i) {
     if (!p.used_in_filter[i] || (size_t)p.used_col[i] >= b->col_span.size()) continue;
     const uint32_t sp = b->col_span[(size_t)p.used_col[i]];
     if (sp <= 24576u) span = std::max(span, sp);  // larger columns are read from global memory
   }
-  p.cw_stage_bytes = span;
-  p.cw_stage = (w + 15u) & ~15u; w = p.cw_stage + p.cw_stage_bytes;
-  p.cw_bytes = (w + 127u) & ~127u;
+  p.cw.stage_bytes = span;
+  p.cw.stage = r16(w);
+  p.cw.bytes = r128(p.cw.stage + span);
 }
 
+// obgpu_project_kernel: [staged block or packed column regions][scratch = sel | bm | wpre | per-warp rle | plans], or the scratch
+// alone when that does not fit; obgpu_project_sparse_kernel next to it with the sparse split
+static void layout_project_cta(const obgpu_batch *b, ScanParams &p, const ScanKnobs &k, bool sparse_split, int max_smem) {
+  ProjCtaLayout &l = p.cp;
+  // stage only the projected columns when that is clearly less than the whole block (upper bound: per-column maximum region
+  // over the batch's blocks)
+  const uint32_t block_bytes = r128(b->max_block_bytes + 16u);
+  uint64_t sum = 0;
+  bool known = p.n_proj > 0;
+  for (int i = 0; i < p.n_proj && known; ++i) {
+    const size_t col = (size_t)p.used_col[p.proj_used[i]];
+    if (col >= b->col_span.size() || b->col_span[col] == 0xffffffffu) known = false;   // no single region (CS string bytes)
+    else sum += b->col_span[col];
+  }
+  l.compact = known && sum * 4 <= (uint64_t)block_bytes * 3;
+  const int want = k.project_compact ? atoi(k.project_compact) : -1;
+  if (want == 0 || (known && want == 1)) l.compact = want;
+  l.scratch = l.compact ? r128((uint32_t)sum) : block_bytes;   // after the staged block or column regions
+  uint32_t s = 0;
+  l.sel = s;  s += r16(p.rows_cap * 2u);
+  l.bm = s;   s += r16(p.words_cap * 4u);
+  l.wpre = s; s += r16(p.words_cap * 4u);
+  l.w = warp_rle(p);
+  l.wscr = s; s += l.w.bytes * (uint32_t)kWarps;
+  l.plans = s; s += (uint32_t)sizeof(ColDesc) * (uint32_t)std::max(p.n_proj, 1);
+  l.total = l.scratch + r128(s);
+  l.no_stage = (int)l.total > max_smem && l.scratch > 0;
+  if (l.no_stage) {
+    // the blocks (or the projected column regions) do not fit next to the scratch: no staging at all, and no per-warp run
+    // tables either (the global path looks runs up by binary search); sel | bm | wpre stay where they are
+    l.compact = l.scratch = 0;
+    l.w = {0u, 0u};
+    l.plans = l.wscr;
+    l.total = r128(l.plans + (uint32_t)sizeof(ColDesc) * (uint32_t)std::max(p.n_proj, 1));
+  }
+  l.sparse_split = sparse_split;
+  l.tiles = sparse_split ? 8 : 1;
+  l.sparse_warp = r16((p.rows_cap / 16u + 32u) * 2u) + (uint32_t)sizeof(ColDesc);
+}
 
-// Small-block pipelined kernels (scan_small.cuh): which of them this scan can use, and their per-warp layouts.
-static void layout_pipe(obgpu_batch *b, ScanParams &p, int max_smem) {
-  p.pipe_count = p.pipe_project = 0;
-  p.pc_rec = p.pp_rec = p.pc_all_coded = 0;
-  if (!pipe_wanted(b->max_rows)) return;
-  auto r16 = [](uint32_t v) { return (v + 15u) & ~15u; };
-  // n column areas back to back in a region slot: column i (block column col(i)) at off[i], with its widest span in the batch rounded
-  // to 16 bytes as its budget span[i]. Returns the bytes of all n, or 0xffffffff for a column with no bounded span or one over cap.
-  auto pack_spans = [&](int n, auto col, const std::vector<uint32_t> &spans, uint32_t cap, uint32_t *off, uint32_t *span) {
-    uint32_t at = 0;
-    for (int i = 0; i < n; ++i) {
-      const size_t c = (size_t)col(i);
-      const uint32_t sp = c < spans.size() ? spans[c] : 0xffffffffu;
-      if (sp == 0xffffffffu || sp > cap) return 0xffffffffu;
-      off[i] = at;
-      span[i] = r16(sp);
-      at += r16(sp);
-    }
-    return at;
-  };
-  // stage records serve used column i when every block's record can stand in for its plan on that path, and the blocks agree on
-  // the column's type (the record leaves the type facts to the scan)
-  auto rec_ok = [&](int i, uint32_t gap) {
-    const size_t col = (size_t)p.used_col[i];
-    if (b->d_stage == nullptr || col >= b->col_stage_gaps.size() || (b->col_stage_gaps[col] & gap) || b->col_types[col] == 0xff) return false;
-    const uint8_t t = b->col_types[col];
-    p.used_sc[i] = (uint8_t)obf::store_class_of(t);
-    p.used_elem_len[i] = (uint8_t)obf::datum_len_of(t);
-    p.used_int_mask[i] = obf::integer_mask_of(t);
-    return true;
-  };
-  // ---- count: every filter column (= the first pf_n used columns) has a bounded region ----------------------
-  if (p.n_nodes > 0 && p.simple_shape != 0) {
-    int nf = 0;
-    bool ok = true;
-    while (nf < p.n_used && p.used_in_filter[nf]) ++nf;
-    for (int i = nf; i < p.n_used; ++i) ok = ok && !p.used_in_filter[i];
-    ok = ok && nf > 0 && nf <= 8;
-    const uint32_t off = ok ? pack_spans(nf, [&](int i) { return p.used_col[i]; }, b->col_span, 12288u, p.pf_off, p.pf_span) : 0xffffffffu;
-    if (off != 0xffffffffu) {
-      p.pf_n = nf;
-      // records: every block has at most 1024 rows (bitmap in registers) and every leaf takes a lean path (lean_leaf) on
-      // a column whose records all serve the filter
-      bool rec = b->max_rows <= 1024u;
-      const int n_leaves = p.n_nodes == 1 ? 1 : p.n_nodes - 1;
-      for (int i = 0; i < n_leaves && rec; ++i) {
-        const FilterNodeDev &nd = p.nodes[i];
-        rec = nd.op != OP_FALSE && nd.op != OP_TRUE && nd.slot >= 0 && nd.used_idx < nf && rec_ok(nd.used_idx, SR_NOT_FILTER);
-        if (rec) rec = p.used_sc[nd.used_idx] == 5 ? (nd.op == OP_EQ || nd.op == OP_NE || nd.op == OP_IN) : nd.range_ok != 0;
+// n column areas back to back in a pipelined kernel's region slot: column i (block column col(i)) at off[i], its widest span rounded
+// to 16 bytes as budget span[i]. Returns the bytes of all n, or 0xffffffff for a column with no bounded span or one over cap.
+template <class Col>
+static uint32_t pack_spans(int n, Col col, const std::vector<uint32_t> &spans, uint32_t cap, uint32_t *off, uint32_t *span) {
+  uint32_t at = 0;
+  for (int i = 0; i < n; ++i) {
+    const size_t c = (size_t)col(i);
+    const uint32_t sp = c < spans.size() ? spans[c] : 0xffffffffu;
+    if (sp == 0xffffffffu || sp > cap) return 0xffffffffu;
+    off[i] = at;
+    span[i] = r16(sp);
+    at += r16(sp);
+  }
+  return at;
+}
+
+// Stage records serve used column i when every block's record can stand in for its plan on that path, and the blocks agree on
+// the column's type (the record leaves the type facts to the scan, stored here)
+static bool records_serve(const obgpu_batch *b, ScanParams &p, int i, uint32_t gap) {
+  const size_t col = (size_t)p.used_col[i];
+  if (b->d_stage == nullptr || col >= b->col_stage_gaps.size() || (b->col_stage_gaps[col] & gap) || b->col_types[col] == 0xff) return false;
+  const uint8_t t = b->col_types[col];
+  p.used_sc[i] = (uint8_t)obf::store_class_of(t);
+  p.used_elem_len[i] = (uint8_t)obf::datum_len_of(t);
+  p.used_int_mask[i] = obf::integer_mask_of(t);
+  return true;
+}
+
+// obgpu_count_pipe_kernel: its instantiation (plans, records, records with every filter column coded) and layout, after the batch
+// codes of the record kernel's columns. COUNT_CTA when the filter does not suit it or two CTAs per SM do not fit.
+static ScanCount layout_count_pipe(obgpu_batch *b, ScanParams &p, const ScanKnobs &k, int max_smem) {
+  if (p.simple_shape == 0) return COUNT_CTA;
+  int nf = 0;
+  while (nf < p.n_used && p.used_in_filter[nf]) ++nf;
+  for (int i = nf; i < p.n_used; ++i) if (p.used_in_filter[i]) return COUNT_CTA;
+  CountPipeLayout l{};
+  const uint32_t off = nf > 0 && nf <= 8 ? pack_spans(nf, [&](int i) { return p.used_col[i]; }, b->col_span, 12288u, l.off, l.span) : 0xffffffffu;
+  if (off == 0xffffffffu) return COUNT_CTA;
+  l.n = nf;
+  // records: every block has at most 1024 rows (bitmap in registers) and every leaf takes a lean path (lean_leaf) on a column
+  // whose records all serve the filter
+  bool rec = b->max_rows <= 1024u;
+  const int n_leaves = p.n_nodes == 1 ? 1 : p.n_nodes - 1;
+  for (int i = 0; i < n_leaves && rec; ++i) {
+    const FilterNodeDev &nd = p.nodes[i];
+    rec = nd.op != OP_FALSE && nd.op != OP_TRUE && nd.slot >= 0 && nd.used_idx < nf && records_serve(b, p, nd.used_idx, SR_NOT_FILTER);
+    if (rec) rec = p.used_sc[nd.used_idx] == 5 ? (nd.op == OP_EQ || nd.op == OP_NE || nd.op == OP_IN) : nd.range_ok != 0;
+  }
+  // batch codes: a filter column among the first four (with records every leaf on it is a record leaf: an EQ / NE / IN on a
+  // string, a range on an integer) stages its refs and its block's code slice instead of its region, when its codes exist or can
+  // be built now
+  uint32_t region = off;
+  if (rec && b->codes_allowed && !(k.str_codes && atoi(k.str_codes) == 0)) {
+    region = 0;
+    for (int i = 0; i < nf; ++i) {
+      const ColCodes *sc = i < 4 ? &batch_codes(b, p.used_col[i]) : nullptr;
+      l.off[i] = region;
+      if (sc && sc->state == 1) {
+        l.coded |= 1 << i;
+        l.span[i] = r16(sc->refs_span);
+        l.code_at[i] = kCountHdrBytes + region + l.span[i];
+        l.code_words = std::max<int32_t>(l.code_words, (sc->n_codes + 31) / 32);
+        p.codes[i] = sc->d_codes;
+        p.code_off16[i] = sc->d_off16;
+        region += r16(sc->codes_span);
       }
-      p.pc_rec = rec ? 1 : 0;
-      // batch codes: a filter column among the first four (with records every leaf on it is a record leaf: an EQ / NE / IN on a
-      // string, a range on an integer) stages its refs and its block's code slice instead of its region, when its codes exist or can
-      // be built now
-      uint32_t coded_off = off;
-      p.pf_coded = 0;
-      const char *ce = getenv("OBGPU_STR_CODES");   // testing knob: 0 keeps every leaf on its per-block dictionary
-      if (rec && b->codes_allowed && !(ce && atoi(ce) == 0)) {
-        uint32_t at = 0;
-        for (int i = 0; i < nf; ++i) {
-          const ColCodes *sc = i < 4 ? &batch_codes(b, p.used_col[i]) : nullptr;
-          p.pf_off[i] = at;
-          if (sc && sc->state == 1) {
-            p.pf_coded |= 1 << i;
-            p.pf_span[i] = r16(sc->refs_span);
-            p.pf_codes[i] = kCountHdrBytes + at + p.pf_span[i];
-            p.codes[i] = sc->d_codes;
-            p.code_off16[i] = sc->d_off16;
-            p.code_words = std::max<int32_t>(p.code_words, (sc->n_codes + 31) / 32);
-            at += p.pf_span[i] + r16(sc->codes_span);
-          } else {
-            p.pf_span[i] = r16(b->col_span[(size_t)p.used_col[i]]);
-            at += p.pf_span[i];
-          }
-        }
-        coded_off = at;
-      }
-      // every filter column coded: the count kernel's CodedLeaves instantiation, which needs no bitmap, survivor or bitset scratch
-      p.pc_all_coded = rec && p.pf_coded == (1 << nf) - 1;
-      p.pc_meta_bytes = kMetaPlans + (uint32_t)nf * (rec ? kCountEnt<true> : kCountEnt<false>);
-      p.pc_region_bytes = kCountHdrBytes + coded_off;
-      uint32_t w = 0;
-      p.pc_meta = w;   w += 3u * p.pc_meta_bytes;
-      p.pc_region = w; w += 2u * p.pc_region_bytes;
-      p.pc_bm = w;     // spilled bitmap + survivor list
-      if (!p.pc_all_coded) w += r16(std::max(p.words_cap, 32u) * 4u) + r16(p.rows_cap * 2u);
-      p.pc_bitset = w;
-      if (!p.pc_all_coded) w += r16((uint32_t)p.n_slots * (uint32_t)p.bitset_words * 4u);
-      p.pc_bar = w;    w += 16u;
-      p.pc_bytes = ((w + 127u) & ~127u) + 128u;   // slack: ragged tail words read a few refs past the staged region
-      if (p.pc_bytes * (uint32_t)kWarps * 2u <= (uint32_t)max_smem) p.pipe_count = 1;   // at least two CTAs per SM
+      region += l.span[i];
     }
   }
-  // ---- project ------------------------------------------------------------------------------------------------------
+  // every filter column coded: the CodedLeaves instantiation, which needs no bitmap, survivor or bitset scratch
+  const bool all_coded = rec && l.coded == (1 << nf) - 1;
+  l.meta_bytes = kMetaPlans + (uint32_t)nf * (rec ? kCountEnt<true> : kCountEnt<false>);
+  l.region_bytes = kCountHdrBytes + region;
+  uint32_t w = 0;
+  l.meta = w;   w += 3u * l.meta_bytes;
+  l.region = w; w += 2u * l.region_bytes;
+  l.bm = w;     // spilled bitmap + survivor list
+  if (!all_coded) w += r16(std::max(p.words_cap, 32u) * 4u) + r16(p.rows_cap * 2u);
+  l.bitset = w;
+  if (!all_coded) w += bitset_bytes(p);
+  l.bar = w;    w += 16u;
+  l.bytes = r128(w) + 128u;   // slack: ragged tail words read a few refs past the staged region
+  if (l.bytes * (uint32_t)kWarps * 2u > (uint32_t)max_smem) return COUNT_CTA;   // at least two CTAs per SM
+  p.pc = l;
+  return all_coded ? COUNT_PIPE_CODED : rec ? COUNT_PIPE_RECORDS : COUNT_PIPE_PLANS;
+}
+
+// obgpu_project_pipe_kernel: its instantiation (plans or records) and layout. PROJ_NONE when a projected column has no bounded
+// span or two CTAs per SM do not fit.
+static ScanProj layout_project_pipe(const obgpu_batch *b, ScanParams &p, int max_smem) {
+  ProjPipeLayout l{};
+  // one lane per projected column computes and issues its byte ranges
+  const uint32_t off = p.n_proj <= 32 ? pack_spans(p.n_proj, [&](int i) { return p.used_col[p.proj_used[i]]; }, b->col_pspan, 16384u,
+                                                   l.off, l.span) : 0xffffffffu;
+  if (off == 0xffffffffu) return PROJ_NONE;
+  bool rec = true;
+  for (int i = 0; i < p.n_proj && rec; ++i) rec = records_serve(b, p, p.proj_used[i], SR_NOT_FLAT);
+  l.meta_bytes = kMetaPlans + (uint32_t)std::max(p.n_proj, 1) * (rec ? kProjEnt<true> : kProjEnt<false>);
+  l.hdr_bytes = r16((2u * (uint32_t)kMaxProj + 1u) * 4u);   // deltas + flags
+  l.bm_bytes = r16(p.words_cap * 4u);
+  l.region_bytes = l.hdr_bytes + l.bm_bytes + off;
+  l.w = warp_rle(p);
+  uint32_t w = 0;
+  l.meta = w;   w += 3u * l.meta_bytes;
+  l.region = w; w += 2u * l.region_bytes;
+  l.sel = w;    w += r16(p.rows_cap * 2u);
+  l.wscr = w;   w += l.w.bytes;
+  l.bar = w;    w += 16u;
+  l.bytes = r128(w);
+  if (l.bytes * (uint32_t)kWarps * 2u > (uint32_t)max_smem) return PROJ_NONE;
+  p.pp = l;
+  return rec ? PROJ_PIPE_RECORDS : PROJ_PIPE_PLANS;
+}
+
+// The kernels of one scan, and their layouts in p. The count kernel is chosen first: the record kernels build the batch codes
+// they use before they are laid out. Fails (NOT_SUPPORTED) when a CTA kernel it needs does not fit shared memory.
+static int plan_scan(obgpu_batch *b, ScanParams &p, bool ext_bm, int64_t cap, ScanPlan &plan) {
+  obgpu_ctx *ctx = b->ctx;
+  const int max_smem = ctx->max_smem_optin;
+  const ScanKnobs k = scan_knobs();
+  const bool pipe = pipe_wanted(b->max_rows, k);
+  assign_rle_slots(b, p);
+  plan.count = ext_bm ? COUNT_BITMAP : p.n_nodes == 0 ? COUNT_NONE : pipe ? layout_count_pipe(b, p, k, max_smem) : COUNT_CTA;
+  if (plan.count == COUNT_CTA) layout_count_cta(b, p);
+  plan.proj = PROJ_NONE;
   if (p.n_proj + p.want_row_ids > 0) {
-    // one lane per projected column computes and issues its byte ranges
-    const uint32_t off = p.n_proj <= 32 ? pack_spans(p.n_proj, [&](int i) { return p.used_col[p.proj_used[i]]; }, b->col_pspan, 16384u,
-                                                     p.pp_off, p.pp_span) : 0xffffffffu;
-    if (off != 0xffffffffu) {
-      bool rec = true;
-      for (int i = 0; i < p.n_proj && rec; ++i) rec = rec_ok(p.proj_used[i], SR_NOT_FLAT);
-      p.pp_rec = rec ? 1 : 0;
-      p.pp_meta_bytes = kMetaPlans + (uint32_t)std::max(p.n_proj, 1) * (rec ? kProjEnt<true> : kProjEnt<false>);
-      p.pp_hdr_bytes = r16((2u * (uint32_t)kMaxProj + 1u) * 4u);   // deltas + flags
-      p.pp_bm_bytes = r16(p.words_cap * 4u);
-      p.pp_region_bytes = p.pp_hdr_bytes + p.pp_bm_bytes + off;
-      // warp-private RLE scratch: [run values][run table] (same shape as the CTA kernel's)
-      p.pw_rle = p.n_rle_slots > 0 ? (((uint32_t)p.rle_runs_cap + 2u) * 8u) : 0u;
-      p.pw_bytes = r16(p.pw_rle + (p.n_rle_slots > 0 ? p.words_cap * 6u : 0u));
-      uint32_t w = 0;
-      p.pp_meta = w;   w += 3u * p.pp_meta_bytes;
-      p.pp_region = w; w += 2u * p.pp_region_bytes;
-      p.pp_sel = w;    w += r16(p.rows_cap * 2u);
-      p.pp_wscr = w;   w += p.pw_bytes;
-      p.pp_bar = w;    w += 16u;
-      p.pp_bytes = (w + 127u) & ~127u;
-      if (p.pp_bytes * (uint32_t)kWarps * 2u <= (uint32_t)max_smem) p.pipe_project = 1;
+    if (pipe) plan.proj = layout_project_pipe(b, p, max_smem);
+    if (plan.proj == PROJ_NONE) {
+      // the caller's selectivity estimate (max_selected_rows) says at most 1/16 of the rows survive: sparse blocks take the warp kernel
+      const bool selects = plan.count != COUNT_NONE;
+      bool sparse = selects && cap * 16 <= b->total_rows;
+      if (k.sparse_split) sparse = atoi(k.sparse_split) ? selects : false;
+      layout_project_cta(b, p, k, sparse, max_smem);
+      plan.proj = sparse ? PROJ_CTA_SPARSE : PROJ_CTA;
+      if ((int)p.cp.total > max_smem) {
+        ctx->err = "scan working set exceeds shared memory";
+        return OBGPU_NOT_SUPPORTED;
+      }
     }
   }
+  if (plan.count == COUNT_CTA && (int)(p.cw.bytes * (uint32_t)kWarps) > max_smem) {
+    ctx->err = "filter working set exceeds shared memory";
+    return OBGPU_NOT_SUPPORTED;
+  }
+  return OBGPU_SUCCESS;
+}
+
+// Persistent grid of a pipelined kernel: the CTAs that fit on the device at once (*occ per SM), and no more than the blocks need
+static int persistent_grid(const obgpu_ctx *ctx, const void *kern, int smem, int n, int *occ) {
+  *occ = 1;
+  cudaOccupancyMaxActiveBlocksPerMultiprocessor(occ, kern, kThreads, smem);
+  return std::min((n + kWarps - 1) / kWarps, std::max(1, *occ) * ctx->sm_count);
 }
 
 // ---- pushed-down aggregates over the dense projected columns ------------------------------------------
@@ -2682,17 +2753,10 @@ static int scan_common(obgpu_batch *b, const obgpu_scan_spec *spec, const obgpu_
   p.want_row_ids = spec->want_row_ids ? 1 : 0;
   p.string_base = spec->string_base;
   r->string_base = spec->string_base;
-  // the caller's selectivity estimate (max_selected_rows): when it says at most 1/16 of the rows survive, most
-  // blocks will be sparse and the warp-per-block kernel takes them
-  const bool selects = p.n_nodes > 0 || ext_bm != nullptr;   // some rows may be dropped: bitmap words + counts exist
-  p.sparse_split = (selects && r->cap * 16 <= b->total_rows) ? 1 : 0;
-  if (const char *e = getenv("OBGPU_SPARSE_SPLIT")) p.sparse_split = atoi(e) ? (selects ? 1 : 0) : 0;  // testing knob
-  layout_smem_scan(b, p, ctx->max_smem_optin);
-  layout_pipe(b, p, ctx->max_smem_optin);
-  if ((int)p.smem_total > ctx->max_smem_optin && !p.pipe_project) {
-    ctx->err = "scan working set exceeds shared memory";
-    return OBGPU_NOT_SUPPORTED;
-  }
+  ScanPlan plan;
+  ret = plan_scan(b, p, ext_bm != nullptr, r->cap, plan);
+  if (ret != OBGPU_SUCCESS) return ret;
+  const bool selects = plan.count != COUNT_NONE;   // some rows may be dropped: bitmap words + counts exist
   // ---- result arena: [zeroed region | data] ---------------------------------------------------------
   const int32_t n = b->n_blocks;
   Scratch arena(ctx);
@@ -2709,8 +2773,8 @@ static int scan_common(obgpu_batch *b, const obgpu_scan_spec *spec, const obgpu_
   const bool use_skip = b->d_agg != nullptr && p.n_nodes > 0;
   const size_t o_blk_const = use_skip ? arena.take((size_t)n) : 0;
   const size_t o_leaf_const = use_skip ? arena.take((size_t)n * (size_t)p.n_nodes) : 0;
-  const bool coded = p.pipe_count && p.pc_rec && p.pf_coded && !ext_bm;
-  const size_t o_code_bits = coded ? arena.take((size_t)p.n_slots * (size_t)p.code_words * 4) : 0;
+  const bool coded = p.pc.coded != 0;
+  const size_t o_code_bits = coded ? arena.take((size_t)p.n_slots * (size_t)p.pc.code_words * 4) : 0;
   size_t o_data[kMaxProj], o_lens[kMaxProj];
   for (int c = 0; c < spec->n_proj; ++c) {
     const int t = b->col_types[(size_t)spec->proj_cols[c]];
@@ -2746,7 +2810,6 @@ static int scan_common(obgpu_batch *b, const obgpu_scan_spec *spec, const obgpu_
   p.row_ids = spec->want_row_ids ? (int32_t *)(a + o_rid) : nullptr;
   p.out_cap = r->cap;
   p.code_bits = coded ? (const uint32_t *)(a + o_code_bits) : nullptr;
-  if (!coded) p.pf_coded = p.pc_all_coded = 0;
   for (int c = 0; c < spec->n_proj; ++c) {
     r->cols[c].data = a + o_data[c];
     r->cols[c].lens = r->cols[c].is_string ? (int32_t *)(a + o_lens[c]) : nullptr;
@@ -2772,48 +2835,44 @@ static int scan_common(obgpu_batch *b, const obgpu_scan_spec *spec, const obgpu_
     p.blk_const = a + o_blk_const;
     p.leaf_const = a + o_leaf_const;
   }
-  if (ext_bm) {   // ObCGRowScanner::get_next_rows(bitmap): another column group's filter already chose the rows
-    obgpu_bitmap_slice_kernel<<<(unsigned)(((int64_t)n * 32 + 127) / 128), 128, 0, ctx->stream>>>(
-        ext_bm->d_words, ext_bm->n_rows, ext_row_offset, b->d_row_start, b->d_rows, b->d_bm_word_off, n, p.bitmap_words, p.counts);
-    ctx->launches++;
-  } else if (p.n_nodes > 0) {
-    const uint32_t cw_total = p.cw_bytes * (uint32_t)kWarps;
-    if ((int)cw_total > ctx->max_smem_optin) {
-      ctx->err = "filter working set exceeds shared memory";
-      return OBGPU_NOT_SUPPORTED;
-    }
-    if (p.pipe_count) {
-      const int smem = (int)(p.pc_bytes * (uint32_t)kWarps);
-      int occ = 1;
-      const void *kern = p.pc_all_coded ? (const void *)static_cast<void (*)(ScanParams, CodedLeaves)>(obgpu_count_pipe_kernel<true>)
-                         : p.pc_rec     ? (const void *)static_cast<void (*)(ScanParams)>(obgpu_count_pipe_kernel<true>)
-                                        : (const void *)static_cast<void (*)(ScanParams)>(obgpu_count_pipe_kernel<false>);
-      cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, kThreads, smem);
-      ctx->last_pc_bytes = (int32_t)p.pc_bytes;
-      ctx->last_count_ctas = occ;
-      ctx->last_count_kernel = p.pc_all_coded ? OBGPU_COUNT_PIPE_CODED : p.pc_rec ? OBGPU_COUNT_PIPE_RECORDS : OBGPU_COUNT_PIPE_PLANS;
-      const int grid = std::min((n + kWarps - 1) / kWarps, std::max(1, occ) * ctx->sm_count);
-      if (p.pc_rec && p.pf_coded) {
-        // the leaves on coded columns, once over each column's distinct values
-        const int n_leaves = p.n_nodes == 1 ? 1 : p.n_nodes - 1;
-        for (int i = 0; i < n_leaves; ++i) {
-          const FilterNodeDev &nd = p.nodes[i];
-          if (!((p.pf_coded >> nd.used_idx) & 1)) continue;
-          const ColCodes &sc = b->col_codes[(size_t)p.used_col[nd.used_idx]];
-          obgpu_code_leaf_kernel<<<(p.code_words * 32 + 255) / 256, 256, 0, ctx->stream>>>(p, i, sc.d_table, sc.n_codes, p.code_words,
-                                                                                          const_cast<uint32_t *>(p.code_bits) + nd.slot * p.code_words);
-          ctx->launches++;
-        }
-      }
-      if (p.pc_all_coded) obgpu_count_pipe_kernel<true><<<grid, kThreads, smem, ctx->stream>>>(p, CodedLeaves{});
-      else if (p.pc_rec) obgpu_count_pipe_kernel<true><<<grid, kThreads, smem, ctx->stream>>>(p);
-      else obgpu_count_pipe_kernel<false><<<grid, kThreads, smem, ctx->stream>>>(p);
-    } else {
+  switch (plan.count) {
+    case COUNT_NONE: break;
+    case COUNT_BITMAP:   // ObCGRowScanner::get_next_rows(bitmap): another column group's filter already chose the rows
+      obgpu_bitmap_slice_kernel<<<(unsigned)(((int64_t)n * 32 + 127) / 128), 128, 0, ctx->stream>>>(
+          ext_bm->d_words, ext_bm->n_rows, ext_row_offset, b->d_row_start, b->d_rows, b->d_bm_word_off, n, p.bitmap_words, p.counts);
+      break;
+    case COUNT_CTA:
       ctx->last_pc_bytes = ctx->last_count_ctas = ctx->last_count_kernel = 0;
-      obgpu_count_kernel<<<(n + kWarps - 1) / kWarps, kThreads, cw_total, ctx->stream>>>(p);
+      obgpu_count_kernel<<<(n + kWarps - 1) / kWarps, kThreads, p.cw.bytes * (uint32_t)kWarps, ctx->stream>>>(p);
+      break;
+    case COUNT_PIPE_PLANS:
+    case COUNT_PIPE_RECORDS:
+    case COUNT_PIPE_CODED: {
+      const int smem = (int)(p.pc.bytes * (uint32_t)kWarps);
+      const void *kern = plan.count == COUNT_PIPE_CODED ? (const void *)static_cast<void (*)(ScanParams, CodedLeaves)>(obgpu_count_pipe_kernel<true>)
+                       : plan.count == COUNT_PIPE_RECORDS ? (const void *)static_cast<void (*)(ScanParams)>(obgpu_count_pipe_kernel<true>)
+                                                          : (const void *)static_cast<void (*)(ScanParams)>(obgpu_count_pipe_kernel<false>);
+      int occ, grid = persistent_grid(ctx, kern, smem, n, &occ);
+      ctx->last_pc_bytes = (int32_t)p.pc.bytes;
+      ctx->last_count_ctas = occ;
+      ctx->last_count_kernel = plan.count;
+      // the leaves on coded columns, once over each column's distinct values
+      const int n_leaves = p.n_nodes == 1 ? 1 : p.n_nodes - 1;
+      for (int i = 0; i < n_leaves; ++i) {
+        const FilterNodeDev &nd = p.nodes[i];
+        if (!((p.pc.coded >> nd.used_idx) & 1)) continue;
+        const ColCodes &sc = b->col_codes[(size_t)p.used_col[nd.used_idx]];
+        obgpu_code_leaf_kernel<<<(p.pc.code_words * 32 + 255) / 256, 256, 0, ctx->stream>>>(p, i, sc.d_table, sc.n_codes, p.pc.code_words,
+                                                                                           const_cast<uint32_t *>(p.code_bits) + nd.slot * p.pc.code_words);
+        ctx->launches++;
+      }
+      if (plan.count == COUNT_PIPE_CODED) obgpu_count_pipe_kernel<true><<<grid, kThreads, smem, ctx->stream>>>(p, CodedLeaves{});
+      else if (plan.count == COUNT_PIPE_RECORDS) obgpu_count_pipe_kernel<true><<<grid, kThreads, smem, ctx->stream>>>(p);
+      else obgpu_count_pipe_kernel<false><<<grid, kThreads, smem, ctx->stream>>>(p);
+      break;
     }
-    ctx->launches++;
   }
+  ctx->launches += plan.count != COUNT_NONE;
   {
     const int n_chunks = (n + kPrefixChunk - 1) / kPrefixChunk;
     const uint32_t *cnts = selects ? p.counts : b->d_rows;
@@ -2821,24 +2880,23 @@ static int scan_common(obgpu_batch *b, const obgpu_scan_spec *spec, const obgpu_
     obgpu_prefix_fix_kernel<<<n_chunks + 1, 256, 0, ctx->stream>>>(n, n_chunks, p.sel_offset, (const unsigned long long *)(a + o_chunk));
     ctx->launches += 2;
   }
-  if (p.n_proj + p.want_row_ids > 0) {
-    p.proj_tiles = p.sparse_split ? 8 : 1;
-    if (p.pipe_project) {
-      const int smem = (int)(p.pp_bytes * (uint32_t)kWarps);
-      int occ = 1;
-      const auto kern = p.pp_rec ? obgpu_project_pipe_kernel<true> : obgpu_project_pipe_kernel<false>;
-      cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, kThreads, smem);
-      const int grid = std::min((n + kWarps - 1) / kWarps, std::max(1, occ) * ctx->sm_count);
-      kern<<<grid, kThreads, smem, ctx->stream>>>(p);
-    } else if (p.sparse_split) obgpu_project_kernel<true><<<(n + p.proj_tiles - 1) / p.proj_tiles, kThreads, p.smem_total, ctx->stream>>>(p);
-    else obgpu_project_kernel<false><<<n, kThreads, p.smem_total, ctx->stream>>>(p);
-    ctx->launches++;
-    if (p.sparse_split && !p.pipe_project) {
-      const uint32_t per_warp = (((p.rows_cap / 16u + 32u) * 2u + 15u) & ~15u) + (uint32_t)sizeof(ColDesc);
-      obgpu_project_sparse_kernel<<<(n + kWarps - 1) / kWarps, kThreads, per_warp * (uint32_t)kWarps, ctx->stream>>>(p);
-      ctx->launches++;
+  switch (plan.proj) {
+    case PROJ_NONE: break;
+    case PROJ_CTA: obgpu_project_kernel<false><<<n, kThreads, p.cp.total, ctx->stream>>>(p); break;
+    case PROJ_CTA_SPARSE:
+      obgpu_project_kernel<true><<<(n + p.cp.tiles - 1) / p.cp.tiles, kThreads, p.cp.total, ctx->stream>>>(p);
+      obgpu_project_sparse_kernel<<<(n + kWarps - 1) / kWarps, kThreads, p.cp.sparse_warp * (uint32_t)kWarps, ctx->stream>>>(p);
+      break;
+    case PROJ_PIPE_PLANS:
+    case PROJ_PIPE_RECORDS: {
+      const int smem = (int)(p.pp.bytes * (uint32_t)kWarps);
+      const auto kern = plan.proj == PROJ_PIPE_RECORDS ? obgpu_project_pipe_kernel<true> : obgpu_project_pipe_kernel<false>;
+      int occ;
+      kern<<<persistent_grid(ctx, (const void *)kern, smem, n, &occ), kThreads, smem, ctx->stream>>>(p);
+      break;
     }
   }
+  ctx->launches += (plan.proj != PROJ_NONE) + (plan.proj == PROJ_CTA_SPARSE);
   const cudaError_t launched = cudaGetLastError();
   if (ctx->profiling) {
     cudaEventRecord(ctx->ev1[pslot], ctx->stream);
@@ -3152,7 +3210,7 @@ int run_filter_block(obgpu_batch *b, int32_t block, const obgpu_filter *f, int64
   if (p.n_nodes == 0) return OBGPU_INVALID_ARGUMENT;
   if (count == 0) return OBGPU_SUCCESS;
   layout_smem(b, p);
-  if ((int)p.smem_total > ctx->max_smem_optin) return OBGPU_NOT_SUPPORTED;
+  if ((int)p.blk.total > ctx->max_smem_optin) return OBGPU_NOT_SUPPORTED;
   Scratch tmp(ctx);
   const size_t o_status = tmp.take(64, 64), o_bytes = tmp.take((size_t)count, 64);
   CUDA_TRY(ctx, tmp.alloc());
@@ -3164,7 +3222,7 @@ int run_filter_block(obgpu_batch *b, int32_t block, const obgpu_filter *f, int64
   p.bm_word_off = b->d_bm_word_off;
   p.n_blocks = b->n_blocks;
   p.status = tmp.at<int32_t>(o_status);
-  obgpu_filter_block_kernel<<<1, kThreads, p.smem_total, ctx->stream>>>(p, block, start, count, d_bytes);
+  obgpu_filter_block_kernel<<<1, kThreads, p.blk.total, ctx->stream>>>(p, block, start, count, d_bytes);
   CUDA_TRY(ctx, cudaGetLastError());
   ctx->launches++;
   int32_t *hs = (int32_t *)ctx->h_pinned;
@@ -3189,7 +3247,7 @@ int run_project_block(obgpu_batch *b, int32_t block, int32_t col, const int32_t 
   p.n_used = 1;
   p.used_col[0] = col;
   layout_smem(b, p);
-  if ((int)p.smem_total > ctx->max_smem_optin) return OBGPU_NOT_SUPPORTED;
+  if ((int)p.blk.total > ctx->max_smem_optin) return OBGPU_NOT_SUPPORTED;
   const size_t el = want_string ? 8 : (size_t)elem_len;
   const int64_t total = vec_offset + row_cap;
   const size_t null_words32 = (size_t)((total + 63) / 64) * 2;
@@ -3218,7 +3276,7 @@ int run_project_block(obgpu_batch *b, int32_t block, int32_t col, const int32_t 
   p.has_null = (int32_t *)(a + 64);
   p.string_base = string_base;
   p.xf = reinterpret_cast<const XformRecFwd *>(b->d_xf);
-  obgpu_project_block_kernel<<<1, kThreads, p.smem_total, ctx->stream>>>(
+  obgpu_project_block_kernel<<<1, kThreads, p.blk.total, ctx->stream>>>(
       p, block, (const int32_t *)(a + o_rid), row_cap, vec_offset, a + o_data,
       want_string ? (int32_t *)(a + o_lens) : nullptr, (uint32_t *)(a + o_nulls), (int32_t)el);
   CUDA_TRY(ctx, cudaGetLastError());

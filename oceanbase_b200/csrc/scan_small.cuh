@@ -294,7 +294,7 @@ template <bool REC> constexpr uint32_t kProjEnt = REC ? 64u : (uint32_t)sizeof(C
 
 // One lean leaf on the K_DICT column of descriptor d (width <= 32) staged at sbit (generic address rs_col): returns the lane's
 // bitmap word. A plan's leaf that is neither an integer range nor a string EQ / NE / IN falls back to the generic dictionary bitset
-// (build_dict_bitset, over bv pointed at the staged column); layout_pipe gives a scan records only when no leaf needs it.
+// (build_dict_bitset, over bv pointed at the staged column); plan_scan gives a scan records only when no leaf needs it.
 template <class D>
 __device__ __forceinline__ uint32_t lean_leaf(const ScanParams &p, const FilterNodeDev &nd, const D &d, uint32_t sbit, const uint8_t *rs_col,
                                               uint32_t *bits, uint32_t *bm, uint32_t mybm, uint32_t myvalid, uint32_t nwords,
@@ -441,56 +441,56 @@ __device__ __forceinline__ void warp_pipeline(int n_blocks, uint64_t *bars, int 
 // Count, pipelined. Per warp: meta ring (3 slots: block record + the filter columns' plans, or their stage records when
 // REC), region ring (2 slots: header with the per-column deltas + the filter columns' regions), bitmap words, predicate bitsets.
 // CODED (every filter column has batch codes, REC): a block's work is only the coded row pass of each leaf -- no lean_leaf, no
-// survivor path, no per-block bitset -- and layout_pipe gives the warp no bitmap, survivor or bitset scratch.
+// survivor path, no per-block bitset -- and layout_count_pipe gives the warp no bitmap, survivor or bitset scratch.
 // =================================================================================================
 template <bool REC, bool CODED>
 __device__ __forceinline__ void count_pipe(const ScanParams &p) {
   static_assert(REC || !CODED, "batch codes are staged with stage records");
   constexpr uint32_t kEnt = kCountEnt<REC>;
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  uint8_t *wr = g_smem + (uint32_t)warp * p.pc_bytes;
-  uint32_t *bm = reinterpret_cast<uint32_t *>(wr + p.pc_bm);
-  uint32_t *bitsets = reinterpret_cast<uint32_t *>(wr + p.pc_bitset);
-  const int nf = p.pf_n;
+  uint8_t *wr = g_smem + (uint32_t)warp * p.pc.bytes;
+  uint32_t *bm = reinterpret_cast<uint32_t *>(wr + p.pc.bm);
+  uint32_t *bitsets = reinterpret_cast<uint32_t *>(wr + p.pc.bitset);
+  const int nf = p.pc.n;
   const Team t = warp_team(lane);
   // skip-index verdict of the block whose meta was issued last: fetched two blocks ahead of the block's work, it decides whether
   // regions() stages the block and travels to work() in the region slot's header
   uint32_t verdict = 0;
 
-  uint8_t *meta0 = wr + p.pc_meta, *reg0 = wr + p.pc_region;
-  uint64_t *bars = reinterpret_cast<uint64_t *>(wr + p.pc_bar);
+  uint8_t *meta0 = wr + p.pc.meta, *reg0 = wr + p.pc.region;
+  uint64_t *bars = reinterpret_cast<uint64_t *>(wr + p.pc.bar);
   auto meta = [&](int b, int ms) {
     if (b >= p.n_blocks) return;
-    uint8_t *m = meta0 + (uint32_t)ms * p.pc_meta_bytes;
+    uint8_t *m = meta0 + (uint32_t)ms * p.pc.meta_bytes;
     if (p.blk_const != nullptr) verdict = p.blk_const[b];
     issue_meta<REC, false, kEnt>(p, b, smem_u32(m), nf, [&](int i) { return p.used_col[i]; }, lane);
     // a coded column's first code of the block, in the meta slot's otherwise unused sel_offset bytes (4 per column)
-    if (REC && lane < 4 && ((p.pf_coded >> lane) & 1)) cp_async4(smem_u32(m) + kMetaSel + 4u * (uint32_t)lane, p.code_off16[lane] + b);
+    if (REC && lane < 4 && ((p.pc.coded >> lane) & 1)) cp_async4(smem_u32(m) + kMetaSel + 4u * (uint32_t)lane, p.code_off16[lane] + b);
   };
-  // region slot: [int32 delta[kPipeMaxFilterCols] | declined mask | verdict] (64 bytes) then the regions at p.pf_off[i]
+  // region slot: [int32 delta[kPipeMaxFilterCols] | declined mask | verdict] (64 bytes) then the regions at p.pc.off[i]
   auto regions = [&](int b, int ms, int rsl) {
     if (b >= p.n_blocks) return;
-    const uint8_t *m = meta0 + (uint32_t)ms * p.pc_meta_bytes;
-    uint8_t *rs = reg0 + (uint32_t)rsl * p.pc_region_bytes;
+    const uint8_t *m = meta0 + (uint32_t)ms * p.pc.meta_bytes;
+    uint8_t *rs = reg0 + (uint32_t)rsl * p.pc.region_bytes;
     uint64_t *bar = bars + rsl;
     const BlockRec &rec = *reinterpret_cast<const BlockRec *>(m);
     int32_t *hdr = reinterpret_cast<int32_t *>(rs);
     uint32_t r[4] = {0, 0, 0, 0}, cb = 0;
     bool bad = false;
     if (lane < nf && rec.rows != 0 && verdict == 0) {
-      if (REC && (CODED || ((p.pf_coded >> lane) & 1))) {
+      if (REC && (CODED || ((p.pc.coded >> lane) & 1))) {
         // coded column: its refs and its code slice
         const StageRec &sr = *reinterpret_cast<const StageRec *>(m + kMetaPlans + (uint32_t)lane * kEnt);
         coded_refs_range(sr, rec.rows, r[0], r[1]);
         cb = (((uint32_t)sr.dict_count + 7u) >> 3) * 16u;
-        bad = r[1] - r[0] > p.pf_span[lane] || r[1] > ((rec.size + 15u) & ~15u) + 32u;
+        bad = r[1] - r[0] > p.pc.span[lane] || r[1] > ((rec.size + 15u) & ~15u) + 32u;
         if (bad) r[0] = r[1] = cb = 0;
         // issued before the slot's expect_tx (the slot's phase cannot complete before that arrival): the address dies here
-        if (cb != 0) tma_bulk_g2s(rs + p.pf_codes[lane], p.codes[lane] + (size_t)*reinterpret_cast<const uint32_t *>(m + kMetaSel + 4u * lane) * 8u, cb, bar);
+        if (cb != 0) tma_bulk_g2s(rs + p.pc.code_at[lane], p.codes[lane] + (size_t)*reinterpret_cast<const uint32_t *>(m + kMetaSel + 4u * lane) * 8u, cb, bar);
       } else {
-        bad = staged_ranges<REC, true>(rec, m + kMetaPlans + (uint32_t)lane * kEnt, p.pf_span[lane], r) == 0;
+        bad = staged_ranges<REC, true>(rec, m + kMetaPlans + (uint32_t)lane * kEnt, p.pc.span[lane], r) == 0;
       }
-      hdr[lane] = (int32_t)(kCountHdrBytes + p.pf_off[lane]) - (int32_t)r[0];
+      hdr[lane] = (int32_t)(kCountHdrBytes + p.pc.off[lane]) - (int32_t)r[0];
     }
     const uint32_t badmask = __ballot_sync(0xffffffffu, bad);
     if (lane == 0) {
@@ -501,12 +501,12 @@ __device__ __forceinline__ void count_pipe(const ScanParams &p) {
     const uint32_t total = warp_sum_u32(r[1] - r[0] + cb);
     if (lane == 0) mbar_expect_tx(bar, total);
     __syncwarp();
-    if (r[1] > r[0]) tma_bulk_g2s(rs + kCountHdrBytes + p.pf_off[lane], p.image + rec.off + r[0], r[1] - r[0], bar);
+    if (r[1] > r[0]) tma_bulk_g2s(rs + kCountHdrBytes + p.pc.off[lane], p.image + rec.off + r[0], r[1] - r[0], bar);
   };
 
   auto work = [&](int blk, int ms, int rsl) {
-    const uint8_t *m = meta0 + (uint32_t)ms * p.pc_meta_bytes;
-    uint8_t *rs = reg0 + (uint32_t)rsl * p.pc_region_bytes;
+    const uint8_t *m = meta0 + (uint32_t)ms * p.pc.meta_bytes;
+    uint8_t *rs = reg0 + (uint32_t)rsl * p.pc.region_bytes;
     const BlockRec rec = *reinterpret_cast<const BlockRec *>(m);
     const int32_t *hdr = reinterpret_cast<const int32_t *>(rs);
     const uint32_t rows = rec.rows;
@@ -523,7 +523,7 @@ __device__ __forceinline__ void count_pipe(const ScanParams &p) {
         const FilterNodeDev &nd = p.nodes[i];
         if (p.leaf_const != nullptr && p.leaf_const[(int64_t)blk * p.n_nodes + i] != 0) continue;
         mybm = lean_rows_coded(p, desc_of(p, ents[nd.used_idx], nd.used_idx), (smem_u32(rs) + (uint32_t)hdr[nd.used_idx]) * 8u,
-                               smem_u32(rs) + p.pf_codes[nd.used_idx], (uint32_t)(nd.slot * p.code_words), mybm, myvalid, nwords, and_mode, lane);
+                               smem_u32(rs) + p.pc.code_at[nd.used_idx], (uint32_t)(nd.slot * p.pc.code_words), mybm, myvalid, nwords, and_mode, lane);
         if (i + 1 < n_leaves && !__any_sync(0xffffffffu, and_mode ? mybm != 0u : mybm != myvalid)) break;   // early-out
       }
       if ((uint32_t)lane < nwords) gbm[lane] = mybm;
@@ -547,7 +547,7 @@ __device__ __forceinline__ void count_pipe(const ScanParams &p) {
     };
     uint32_t cnt = 0;
     if (REC || nwords <= 32u) {
-      // ---- lean path (with records every block has at most 1024 rows: layout_pipe): the block's bitmap lives in registers
+      // ---- lean path (with records every block has at most 1024 rows: plan_scan): the block's bitmap lives in registers
       // (lane g owns word g); dictionary-coded leaves run through explicit shared-memory loads, everything else (plans only)
       // through the generic leaf code on a spilled bitmap
       const uint32_t myvalid = (uint32_t)lane < nwords ? valid_mask_of(rows, (uint32_t)lane) : 0u;
@@ -556,10 +556,10 @@ __device__ __forceinline__ void count_pipe(const ScanParams &p) {
         const FilterNodeDev &nd = p.nodes[i];
         if (p.leaf_const != nullptr && p.leaf_const[(int64_t)blk * p.n_nodes + i] != 0) continue;
         const auto &d = desc_of(p, ents[nd.used_idx], nd.used_idx);
-        // with records every leaf is lean (layout_pipe)
-        if (REC && ((p.pf_coded >> nd.used_idx) & 1)) {
-          mybm = lean_rows_coded(p, d, (smem_u32(rs) + (uint32_t)hdr[nd.used_idx]) * 8u, smem_u32(rs) + p.pf_codes[nd.used_idx],
-                                 (uint32_t)(nd.slot * p.code_words), mybm, myvalid, nwords, and_mode, lane);
+        // with records every leaf is lean (plan_scan)
+        if (REC && ((p.pc.coded >> nd.used_idx) & 1)) {
+          mybm = lean_rows_coded(p, d, (smem_u32(rs) + (uint32_t)hdr[nd.used_idx]) * 8u, smem_u32(rs) + p.pc.code_at[nd.used_idx],
+                                 (uint32_t)(nd.slot * p.pc.code_words), mybm, myvalid, nwords, and_mode, lane);
         } else if (REC || (d.kind == K_DICT && nd.slot >= 0 && nd.op != OP_FALSE && nd.op != OP_TRUE && d.width <= 32u)) {
           mybm = lean_leaf(p, nd, d, (smem_u32(rs) + (uint32_t)hdr[nd.used_idx]) * 8u, rs + hdr[nd.used_idx],
                            bitsets + nd.slot * p.bitset_words, bm, mybm, myvalid, nwords, and_mode, c.b, t, lane);
@@ -639,7 +639,7 @@ __global__ void __launch_bounds__(kThreads, 10) obgpu_count_pipe_kernel(const __
 
 // =================================================================================================
 // Projection, pipelined. Meta slot: [record | sel_offset pair | n_proj plans] (kMetaSel, kMetaPlans); region slot:
-// [header: per column {delta0, delta1} + flags | bitmap words | column byte ranges at p.pp_off[pc]].
+// [header: per column {delta0, delta1} + flags | bitmap words | column byte ranges at p.pp.off[pc]].
 // =================================================================================================
 #define ROW(j) (IDENT ? (uint32_t)(j) : (uint32_t)sel[j])
 template <bool IDENT>
@@ -768,25 +768,25 @@ template <bool REC>
 __global__ void __launch_bounds__(kThreads) obgpu_project_pipe_kernel(const __grid_constant__ ScanParams p) {
   constexpr uint32_t kEnt = kProjEnt<REC>;
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  uint8_t *wr = g_smem + (uint32_t)warp * p.pp_bytes;
-  uint16_t *sel = reinterpret_cast<uint16_t *>(wr + p.pp_sel);
-  uint8_t *wscr = wr + p.pp_wscr;
+  uint8_t *wr = g_smem + (uint32_t)warp * p.pp.bytes;
+  uint16_t *sel = reinterpret_cast<uint16_t *>(wr + p.pp.sel);
+  uint8_t *wscr = wr + p.pp.wscr;
   const int np = p.n_proj;
-  const uint32_t hdr_bytes = p.pp_hdr_bytes, bm_bytes = p.pp_bm_bytes;
+  const uint32_t hdr_bytes = p.pp.hdr_bytes, bm_bytes = p.pp.bm_bytes;
   const Team t = warp_team(lane);
 
-  uint8_t *meta0 = wr + p.pp_meta, *reg0 = wr + p.pp_region;
-  uint64_t *bars = reinterpret_cast<uint64_t *>(wr + p.pp_bar);
+  uint8_t *meta0 = wr + p.pp.meta, *reg0 = wr + p.pp.region;
+  uint64_t *bars = reinterpret_cast<uint64_t *>(wr + p.pp.bar);
   auto meta = [&](int b, int ms) {
     if (b >= p.n_blocks) return;
-    uint8_t *m = meta0 + (uint32_t)ms * p.pp_meta_bytes;
+    uint8_t *m = meta0 + (uint32_t)ms * p.pp.meta_bytes;
     issue_meta<REC, true, kEnt>(p, b, smem_u32(m), np, [&](int i) { return p.used_col[p.proj_used[i]]; }, lane);
   };
   // what a block needs beyond its meta: nothing (no selected row / overflow / corrupt), or bitmap words + column ranges
   auto regions = [&](int b, int ms, int rsl) {
     if (b >= p.n_blocks) return;
-    const uint8_t *m = meta0 + (uint32_t)ms * p.pp_meta_bytes;
-    uint8_t *rs = reg0 + (uint32_t)rsl * p.pp_region_bytes;
+    const uint8_t *m = meta0 + (uint32_t)ms * p.pp.meta_bytes;
+    uint8_t *rs = reg0 + (uint32_t)rsl * p.pp.region_bytes;
     uint64_t *bar = bars + rsl;
     const BlockRec &rec = *reinterpret_cast<const BlockRec *>(m);
     const int64_t base = *reinterpret_cast<const int64_t *>(m + kMetaSel);
@@ -805,8 +805,8 @@ __global__ void __launch_bounds__(kThreads) obgpu_project_pipe_kernel(const __gr
     uint32_t r[4] = {0, 0, 0, 0};
     int nr = 0;
     if (lane < np) {
-      nr = staged_ranges<REC, false>(rec, m + kMetaPlans + (uint32_t)lane * kEnt, p.pp_span[lane], r);
-      const uint32_t o0 = hdr_bytes + bm_bytes + p.pp_off[lane], o1 = o0 + (r[1] - r[0]);
+      nr = staged_ranges<REC, false>(rec, m + kMetaPlans + (uint32_t)lane * kEnt, p.pp.span[lane], r);
+      const uint32_t o0 = hdr_bytes + bm_bytes + p.pp.off[lane], o1 = o0 + (r[1] - r[0]);
       hdr[2 * lane] = (int32_t)o0 - (int32_t)r[0];
       hdr[2 * lane + 1] = nr == 2 ? (int32_t)o1 - (int32_t)r[2] : (int32_t)o0 - (int32_t)r[0];
     }
@@ -818,7 +818,7 @@ __global__ void __launch_bounds__(kThreads) obgpu_project_pipe_kernel(const __gr
     if (lane == 0) mbar_expect_tx(bar, total);
     __syncwarp();
     if (lane < np && nr >= 1) {
-      uint8_t *dst0 = rs + hdr_bytes + bm_bytes + p.pp_off[lane];
+      uint8_t *dst0 = rs + hdr_bytes + bm_bytes + p.pp.off[lane];
       const uint8_t *gblk = p.image + rec.off;
       tma_bulk_g2s(dst0, gblk + r[0], len0, bar);
       if (nr == 2) tma_bulk_g2s(dst0 + len0, gblk + r[2], len1, bar);
@@ -826,8 +826,8 @@ __global__ void __launch_bounds__(kThreads) obgpu_project_pipe_kernel(const __gr
   };
 
   auto work = [&](int blk, int ms, int rsl) {
-    uint8_t *m = meta0 + (uint32_t)ms * p.pp_meta_bytes;
-    uint8_t *rs = reg0 + (uint32_t)rsl * p.pp_region_bytes;
+    uint8_t *m = meta0 + (uint32_t)ms * p.pp.meta_bytes;
+    uint8_t *rs = reg0 + (uint32_t)rsl * p.pp.region_bytes;
     const BlockRec rec = *reinterpret_cast<const BlockRec *>(m);
     const int64_t base = *reinterpret_cast<const int64_t *>(m + kMetaSel);
     const uint32_t cnt = (uint32_t)(*reinterpret_cast<const int64_t *>(m + kMetaSel + 8u) - base);
@@ -861,11 +861,11 @@ __global__ void __launch_bounds__(kThreads) obgpu_project_pipe_kernel(const __gr
     view_from_rec(rec, nullptr, c.b);
     c.bitsets = nullptr;
     c.descs = plans;
-    c.rle_base = wscr + p.pw_rle;
+    c.rle_base = wscr + p.pp.w.rle;
     c.rle_slot_bytes = 0;
     c.rle_starts_bytes = p.words_cap * 4u;
     const uint64_t blk_addr = block_string_addr(p, blk, rec.off);
-    // with records every projected column is flat in every block (layout_pipe)
+    // with records every projected column is flat in every block (plan_scan)
     const bool flat = lane < np && !((badmask >> lane) & 1u) && (REC || (plans[lane].ok && flat_kind(plans[lane])));
     const uint32_t flatmask = __ballot_sync(0xffffffffu, flat);
     if (flatmask != 0u) {
@@ -895,7 +895,7 @@ __global__ void __launch_bounds__(kThreads) obgpu_project_pipe_kernel(const __gr
       }
       c.b.s = rs + d0;
       c.sbit = (smem_u32(rs) + (uint32_t)d0) * 8u;
-      project_column_staged(p, c, wdesc, pc, sel, cnt, base, blk_addr, all_rows, rows, wscr, t);
+      project_column_staged(p, c, wdesc, pc, sel, cnt, base, blk_addr, all_rows, rows, wscr, p.pp.w.rle, t);
       __syncwarp();
     }
   };
