@@ -179,6 +179,24 @@ int obgpu_batch_string_codes(const obgpu_batch *batch, int32_t col, int32_t *sta
 #define OBGPU_COUNT_PIPE_RECORDS 2 /* stage records, every leaf lean */
 #define OBGPU_COUNT_PIPE_CODED 3   /* stage records, every filter column on batch codes: coded row passes only */
 int obgpu_ctx_count_layout(const obgpu_ctx *ctx, int32_t *pc_bytes, int32_t *ctas_per_sm, int32_t *kernel);
+/* The kernels the ctx's last obgpu_scan / obgpu_scan_bitmap chose: the count kernel (OBGPU_SCAN_COUNT_*), the projection kernel
+ * (OBGPU_SCAN_PROJ_*) and how the projection kernel stages the blocks (OBGPU_SCAN_PROJ_FLAG_* bits, CTA projection kernels only).
+ * All 0 when that call failed before choosing them. */
+#define OBGPU_SCAN_COUNT_NONE 0          /* no filter: every row is selected */
+#define OBGPU_SCAN_COUNT_PIPE_PLANS OBGPU_COUNT_PIPE_PLANS
+#define OBGPU_SCAN_COUNT_PIPE_RECORDS OBGPU_COUNT_PIPE_RECORDS
+#define OBGPU_SCAN_COUNT_PIPE_CODED OBGPU_COUNT_PIPE_CODED
+#define OBGPU_SCAN_COUNT_CTA 4           /* one warp per block, working set in a CTA's shared memory */
+#define OBGPU_SCAN_COUNT_BITMAP 5        /* obgpu_scan_bitmap: the rows come from the range bitmap */
+#define OBGPU_SCAN_PROJ_NONE 0           /* nothing projected and no row ids */
+#define OBGPU_SCAN_PROJ_CTA 1            /* one CTA per block */
+#define OBGPU_SCAN_PROJ_CTA_SPARSE 2     /* the same with sparse blocks on a warp per block (max_selected_rows <= 1/16 of the rows) */
+#define OBGPU_SCAN_PROJ_PIPE_PLANS 3     /* small-block pipelined kernel on decode plans */
+#define OBGPU_SCAN_PROJ_PIPE_RECORDS 4   /* small-block pipelined kernel on stage records */
+#define OBGPU_SCAN_PROJ_FLAG_COMPACT 1   /* stages the projected columns' regions only */
+#define OBGPU_SCAN_PROJ_FLAG_NO_STAGE 2  /* decodes every block from global memory: a block does not fit shared memory */
+#define OBGPU_SCAN_PROJ_FLAG_SPARSE 4    /* the sparse split of OBGPU_SCAN_PROJ_CTA_SPARSE */
+int obgpu_ctx_scan_plan(const obgpu_ctx *ctx, int32_t *count_kernel, int32_t *proj_kernel, int32_t *proj_flags);
 /* Disk-format bytes into the block cache: n_macro_blocks macro blocks of macro_block_size bytes each (ObMacroBlock,
  * blocksstable/ob_macro_block.cpp:455-520: ObMacroBlockCommonHeader, ObSSTableMacroBlockHeader, micro-blocks back to back) are
  * validated and walked ON THE DEVICE (ObMacroBlockCommonHeader::check_integrity ob_macro_block_common_header.cpp:54-69,

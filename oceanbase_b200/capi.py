@@ -193,6 +193,7 @@ def declared_signatures():
         # batch codes of string and integer columns alike (include/obgpu_scan.h)
         "obgpu_batch_string_codes": (C.c_int, [vp, i32, P(i32), P(i32), P(C.c_float)]),
         "obgpu_ctx_count_layout": (C.c_int, [vp, P(i32), P(i32), P(i32)]),
+        "obgpu_ctx_scan_plan": (C.c_int, [vp, P(i32), P(i32), P(i32)]),
         "obgpu_scan": (C.c_int, [vp, P(ScanSpec), P(vp)]),
         "obgpu_result_free": (None, [vp]),
         "obgpu_result_info_get": (C.c_int, [vp, P(ResultInfo)]),

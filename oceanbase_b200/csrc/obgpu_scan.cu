@@ -1836,6 +1836,8 @@ struct obgpu_ctx {
   int64_t prof_count = 0;
   // small-block count kernel of the last scan (obgpu_ctx_count_layout): per-warp shared memory, CTAs per SM, OBGPU_COUNT_PIPE_*
   int32_t last_pc_bytes = 0, last_count_ctas = 0, last_count_kernel = 0;
+  // kernels of the last scan (obgpu_ctx_scan_plan): OBGPU_SCAN_COUNT_*, OBGPU_SCAN_PROJ_*, OBGPU_SCAN_PROJ_FLAG_*
+  int32_t last_plan_count = 0, last_plan_proj = 0, last_plan_flags = 0;
 };
 
 // Device scratch of one host call: slices reserved with take(), then one cudaMallocAsync of their total on the ctx stream.
@@ -2288,10 +2290,12 @@ static int build_filter(obgpu_ctx *ctx, const obgpu_batch *b, const obgpu_filter
   return OBGPU_SUCCESS;
 }
 
-// The kernels of one scan (plan_scan). The pipelined count kernels are numbered as obgpu_ctx_count_layout reports them.
-enum ScanCount { COUNT_NONE = 0, COUNT_PIPE_PLANS = OBGPU_COUNT_PIPE_PLANS, COUNT_PIPE_RECORDS = OBGPU_COUNT_PIPE_RECORDS,
-                 COUNT_PIPE_CODED = OBGPU_COUNT_PIPE_CODED, COUNT_CTA, COUNT_BITMAP };
-enum ScanProj { PROJ_NONE, PROJ_CTA, PROJ_CTA_SPARSE, PROJ_PIPE_PLANS, PROJ_PIPE_RECORDS };
+// The kernels of one scan (plan_scan), numbered as obgpu_ctx_scan_plan reports them
+enum ScanCount { COUNT_NONE = OBGPU_SCAN_COUNT_NONE, COUNT_PIPE_PLANS = OBGPU_SCAN_COUNT_PIPE_PLANS,
+                 COUNT_PIPE_RECORDS = OBGPU_SCAN_COUNT_PIPE_RECORDS, COUNT_PIPE_CODED = OBGPU_SCAN_COUNT_PIPE_CODED,
+                 COUNT_CTA = OBGPU_SCAN_COUNT_CTA, COUNT_BITMAP = OBGPU_SCAN_COUNT_BITMAP };
+enum ScanProj { PROJ_NONE = OBGPU_SCAN_PROJ_NONE, PROJ_CTA = OBGPU_SCAN_PROJ_CTA, PROJ_CTA_SPARSE = OBGPU_SCAN_PROJ_CTA_SPARSE,
+                PROJ_PIPE_PLANS = OBGPU_SCAN_PROJ_PIPE_PLANS, PROJ_PIPE_RECORDS = OBGPU_SCAN_PROJ_PIPE_RECORDS };
 struct ScanPlan { ScanCount count; ScanProj proj; };
 
 // run-table slots for used columns that are RLE-coded in some block, and the row capacity every layout is sized by
@@ -2721,12 +2725,23 @@ extern "C" {
 
 int obgpu_scan(obgpu_batch *b, const obgpu_scan_spec *spec, obgpu_result **out) { return scan_common(b, spec, nullptr, 0, out); }
 
+int obgpu_ctx_scan_plan(const obgpu_ctx *ctx, int32_t *count_kernel, int32_t *proj_kernel, int32_t *proj_flags) {
+  if (!ctx || !count_kernel || !proj_kernel || !proj_flags) return OBGPU_INVALID_ARGUMENT;
+  *count_kernel = ctx->last_plan_count;
+  *proj_kernel = ctx->last_plan_proj;
+  *proj_flags = ctx->last_plan_flags;
+  return OBGPU_SUCCESS;
+}
+
 }  // extern "C"
 
 static int scan_common(obgpu_batch *b, const obgpu_scan_spec *spec, const obgpu_cg_bitmap *ext_bm, int64_t ext_row_offset, obgpu_result **out) {
   if (!b || !spec || !out) return OBGPU_INVALID_ARGUMENT;
   if (ext_bm && spec->filter && spec->filter->n_nodes > 0) return OBGPU_INVALID_ARGUMENT;   // the bitmap IS the selection
   obgpu_ctx *ctx = b->ctx;
+  // the read-outs describe this scan only: zero until its plan is chosen, and the count layout zero unless a pipelined count runs
+  ctx->last_plan_count = ctx->last_plan_proj = ctx->last_plan_flags = 0;
+  ctx->last_pc_bytes = ctx->last_count_ctas = ctx->last_count_kernel = 0;
   if (spec->n_proj < 0 || spec->n_proj > kMaxProj || (spec->n_proj > 0 && !spec->proj_cols))
     return spec->n_proj > kMaxProj ? OBGPU_NOT_SUPPORTED : OBGPU_INVALID_ARGUMENT;
   cudaSetDevice(ctx->device);
@@ -2756,6 +2771,11 @@ static int scan_common(obgpu_batch *b, const obgpu_scan_spec *spec, const obgpu_
   ScanPlan plan;
   ret = plan_scan(b, p, ext_bm != nullptr, r->cap, plan);
   if (ret != OBGPU_SUCCESS) return ret;
+  ctx->last_plan_count = plan.count;
+  ctx->last_plan_proj = plan.proj;
+  if (plan.proj == PROJ_CTA || plan.proj == PROJ_CTA_SPARSE)
+    ctx->last_plan_flags = (p.cp.compact ? OBGPU_SCAN_PROJ_FLAG_COMPACT : 0) | (p.cp.no_stage ? OBGPU_SCAN_PROJ_FLAG_NO_STAGE : 0) |
+                           (p.cp.sparse_split ? OBGPU_SCAN_PROJ_FLAG_SPARSE : 0);
   const bool selects = plan.count != COUNT_NONE;   // some rows may be dropped: bitmap words + counts exist
   // ---- result arena: [zeroed region | data] ---------------------------------------------------------
   const int32_t n = b->n_blocks;
@@ -2842,7 +2862,6 @@ static int scan_common(obgpu_batch *b, const obgpu_scan_spec *spec, const obgpu_
           ext_bm->d_words, ext_bm->n_rows, ext_row_offset, b->d_row_start, b->d_rows, b->d_bm_word_off, n, p.bitmap_words, p.counts);
       break;
     case COUNT_CTA:
-      ctx->last_pc_bytes = ctx->last_count_ctas = ctx->last_count_kernel = 0;
       obgpu_count_kernel<<<(n + kWarps - 1) / kWarps, kThreads, p.cw.bytes * (uint32_t)kWarps, ctx->stream>>>(p);
       break;
     case COUNT_PIPE_PLANS:

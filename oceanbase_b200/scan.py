@@ -122,6 +122,13 @@ class ScanContext:
     def last_error(self) -> str:
         return (lib.obgpu_ctx_last_error(self._h) or b"").decode()
 
+    def last_plan(self):
+        """(count kernel, projection kernel, projection flags) the last scan on this ctx chose: obgpu_ctx_scan_plan, numbered
+        as OBGPU_SCAN_COUNT_* / OBGPU_SCAN_PROJ_* / OBGPU_SCAN_PROJ_FLAG_* in include/obgpu_scan.h."""
+        cnt, proj, flags = C.c_int32(0), C.c_int32(0), C.c_int32(0)
+        check(lib.obgpu_ctx_scan_plan(self._h, C.byref(cnt), C.byref(proj), C.byref(flags)), "obgpu_ctx_scan_plan", self._h)
+        return cnt.value, proj.value, flags.value
+
     def open_batch(self, table, device_image_ptr: Optional[int] = None, host_view: bool = True,
                    image_size: Optional[int] = None, compressor: Optional[int] = None) -> "PageBatch":
         return PageBatch(self, table, device_image_ptr, host_view, image_size, compressor)
