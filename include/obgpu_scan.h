@@ -469,6 +469,26 @@ int obgpu_block_group_by(obgpu_batch *batch, int32_t block, int32_t group_col, c
  * [host_group_off[b], host_group_off[b + 1]) of the group axis (host_group_off: n_blocks + 1 entries, may be NULL). */
 int obgpu_result_group_by(obgpu_result *res, int32_t group_col, const obgpu_group_agg *aggs, int32_t n_aggs,
                           int64_t *host_group_off, int64_t *host_out, int64_t out_cap_groups, int64_t *total_groups);
+/* GROUP BY over every block of a scan with the groups keyed by VALUE across the page batch: the rows the scan selected (all
+ * rows without a filter; the bitmap of a capacity-overflowed scan, as obgpu_result_group_by) are grouped by the value of
+ * group_col, one group per distinct non-NULL value that some selected row holds, plus the NULL group when some selected row
+ * is NULL. aggs as obgpu_result_group_by. The groups stay on the device with the result until obgpu_result_free or the next
+ * call; *n_groups, *key_bytes (string keys: total bytes, else 0) and *has_null_group (the NULL group is then the last) are set.
+ *   Order: ascending keys, the NULL group last. Integer keys in the column's own order (signed classes signed, unsigned ones
+ *   unsigned: the MIN / MAX order); string keys bytewise as unsigned bytes, a proper prefix first, the empty string a group of
+ *   its own. A value is one group whatever its dictionary entry looks like in each block (entry width, CS base, PAX or CS).
+ *   String keys compare as bytes, like the device's string leaves: under a non-binary collation these groups are never
+ *   coarser than SQL's, so a hash GROUP BY above can merge the groups that collate equal.
+ *   OBGPU_NOT_SUPPORTED (the ctx stays usable): group_col not dictionary coded in every block (as obgpu_result_group_by),
+ *   more than 65 536 distinct values in its dictionaries over the batch, a string entry of 65 536 bytes or more or a batch
+ *   image of 2^37 bytes or more (string keys), SUM_PRODUCT, an aggregate on a string column. The scan's own error first. */
+int obgpu_result_group_by_values(obgpu_result *res, int32_t group_col, const obgpu_group_agg *aggs, int32_t n_aggs,
+                                 int64_t *n_groups, int64_t *key_bytes, int32_t *has_null_group);
+/* The last obgpu_result_group_by_values' groups: host_keys[g] = the value as its 64-bit image (integer classes, as MIN / MAX
+ * hand it back; 0 for the NULL group), or, for string columns, n_groups + 1 offsets into host_key_heap (key_bytes bytes; the
+ * NULL group is empty). host_out is [n_aggs][n_groups][2], laid out as obgpu_result_group_by's out. One synchronisation.
+ * OBGPU_INVALID_ARGUMENT when the result has no groups (no successful obgpu_result_group_by_values since the last one). */
+int obgpu_result_fetch_groups(obgpu_result *res, int64_t *host_keys, void *host_key_heap, int64_t *host_out);
 
 /* =============================================================================================
  * String cells as BYTES. HEX_PACKING / STRING_DIFF / STRING_PREFIX columns rebuild their values (ObHexStringDecoder,

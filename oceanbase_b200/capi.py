@@ -230,6 +230,8 @@ def declared_signatures():
         "obgpu_filter_dict_pass": (C.c_int, [vp, i32, i32, vp, i64, i32, i64, i64, vp]),
         "obgpu_block_group_by": (C.c_int, [vp, i32, i32, vp, i32, vp, i64, vp, i64, P(i64)]),
         "obgpu_result_group_by": (C.c_int, [vp, i32, vp, i32, vp, vp, i64, P(i64)]),
+        "obgpu_result_group_by_values": (C.c_int, [vp, i32, vp, i32, P(i64), P(i64), P(i32)]),
+        "obgpu_result_fetch_groups": (C.c_int, [vp, vp, vp, vp]),
         "obgpu_version": (C.c_char_p, []),
         # include/obgpu_compaction.h
         "obgpu_batch_decode_column": (C.c_int, [vp, i32, vp, vp]),

@@ -1964,6 +1964,11 @@ struct obgpu_result {
   int32_t str_cols[kMaxProj] = {0};
   int64_t str_row_begin = 0, str_rows = 0;
   int64_t str_col_off[kMaxProj + 1] = {0};
+  // obgpu_result_group_by_values: its groups (group_values.cuh), kept for obgpu_result_fetch_groups; gv_groups < 0: none
+  void *d_gv = nullptr;
+  int64_t gv_groups = -1, gv_key_bytes = 0;
+  int32_t gv_n_aggs = 0;
+  bool gv_str = false;
 };
 
 static thread_local std::string g_last_global_err;
@@ -3000,6 +3005,7 @@ void obgpu_result_free(obgpu_result *r) {
   cudaSetDevice(r->ctx->device);
   if (r->arena) cudaFreeAsync(r->arena, r->ctx->stream);
   if (r->d_str) cudaFreeAsync(r->d_str, r->ctx->stream);
+  if (r->d_gv) cudaFreeAsync(r->d_gv, r->ctx->stream);
   delete r;
 }
 
@@ -3423,6 +3429,7 @@ int obgpu_project_datums(obgpu_batch *batch, int32_t block, int32_t col, const i
 
 // ---- dictionary surface: distinct values, references, black filter on one dictionary column, GROUP BY ----
 #include "dict_ops.cuh"
+#include "group_values.cuh"   // GROUP BY over a scan, one group per distinct value of the batch
 
 // ---- major-compaction merge (include/obgpu_compaction.h) -----------------------------------------
 #include "../../include/obgpu_compaction.h"

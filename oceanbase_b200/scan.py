@@ -519,6 +519,33 @@ class ScanResult:
                                         max(total.value, 1), C.byref(total)), "obgpu_result_group_by", self.batch.ctx._h)
         return goff, out[:, :total.value]
 
+    def group_by_values(self, group_col, aggs):
+        """GROUP BY over every block of the scan with one group per distinct value of group_col (obgpu_result_group_by_values):
+        returns (keys, out). keys: one per group in ascending order -- Python ints in the column's value domain (unsigned
+        types non-negative) or bytes -- and None for the NULL group, which comes last; out: int64 [n_aggs][n_groups][2]."""
+        spec = np.array([(k, c) for k, c in aggs], dtype=np.int32).reshape(-1, 2)
+        ng, kb, hn = C.c_int64(0), C.c_int64(0), C.c_int32(0)
+        check(lib.obgpu_result_group_by_values(self._h, group_col, spec.ctypes.data, len(aggs), C.byref(ng), C.byref(kb), C.byref(hn)),
+              "obgpu_result_group_by_values", self.batch.ctx._h)
+        n = ng.value
+        keys = np.zeros(n + 1, dtype=np.int64)
+        heap = np.zeros(max(kb.value, 1), dtype=np.uint8)
+        out = np.zeros((len(aggs), max(n, 1), 2), dtype=np.int64)
+        check(lib.obgpu_result_fetch_groups(self._h, keys.ctypes.data, heap.ctypes.data, out.ctypes.data), "obgpu_result_fetch_groups",
+              self.batch.ctx._h)
+        obj_type, dlen = C.c_int32(0), C.c_int32(0)
+        check(lib.obgpu_batch_column_type(self.batch._h, group_col, C.byref(obj_type), C.byref(dlen)), "obgpu_batch_column_type",
+              self.batch.ctx._h)
+        if dlen.value == 0:
+            vals = [bytes(heap[keys[g]:keys[g + 1]]) for g in range(n)]
+        else:
+            vals = [int(v) for v in keys[:n].tolist()]
+            if obj_type.value in (capi.OBJ_UINT64, capi.OBJ_UINT32, capi.OBJ_UTINYINT, capi.OBJ_USMALLINT, capi.OBJ_UMEDIUMINT, capi.OBJ_YEAR):
+                vals = [v & ((1 << 64) - 1) for v in vals]
+        if hn.value:
+            vals[-1] = None
+        return vals, out[:, :n]
+
     def fetch_datums(self, i, row_begin=0, row_count=None):
         """Column i as ObDatum[] (datum format): (datums structured array, slots uint64 array or None for strings)."""
         c = self.col(i)
