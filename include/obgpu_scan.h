@@ -487,8 +487,31 @@ int obgpu_result_group_by_values(obgpu_result *res, int32_t group_col, const obg
 /* The last obgpu_result_group_by_values' groups: host_keys[g] = the value as its 64-bit image (integer classes, as MIN / MAX
  * hand it back; 0 for the NULL group), or, for string columns, n_groups + 1 offsets into host_key_heap (key_bytes bytes; the
  * NULL group is empty). host_out is [n_aggs][n_groups][2], laid out as obgpu_result_group_by's out. One synchronisation.
- * OBGPU_INVALID_ARGUMENT when the result has no groups (no successful obgpu_result_group_by_values since the last one). */
+ * OBGPU_INVALID_ARGUMENT when the result has no groups (no successful obgpu_result_group_by_values since the last one), or
+ * when its groups are keyed by more than one column (obgpu_result_group_by_columns). */
 int obgpu_result_fetch_groups(obgpu_result *res, int64_t *host_keys, void *host_key_heap, int64_t *host_out);
+/* GROUP BY over every block of a scan keyed by the TUPLE of values of 1..4 columns (GROUP BY a, b, ...): the rows the scan
+ * selected, as obgpu_result_group_by_values, one group per distinct tuple (value of group_cols[0], ..., value of
+ * group_cols[n_group_cols - 1]) that some selected row holds; NULL in any column is a value of its own. A column may be named
+ * twice. aggs as obgpu_result_group_by_values (1..16). The groups replace the result's previous ones (either call) and stay
+ * on the device until obgpu_result_free or the next call; *n_groups and *key_bytes (the string key heap's size, else 0) are set.
+ *   Order: lexicographic over group_cols in the caller's order, each column ordered as obgpu_result_group_by_values orders it
+ *   (NULL last within the column). With n_group_cols == 1 the groups and aggregates are exactly obgpu_result_group_by_values'.
+ *   The fold keeps its accumulators in shared memory when (P x (n_aggs + 1) x 16) bytes fit 48 KiB, P = the product over
+ *   the columns of (distinct values + 1); in global memory indexed by the tuple when P <= 2^20; and otherwise hashes the
+ *   tuples of the selected rows first.
+ *   OBGPU_NOT_SUPPORTED (the ctx stays usable): any refusal of obgpu_result_group_by_values for any group column; P of
+ *   2^64 - 1 or more; more than 4 194 304 distinct tuples among the selected rows when P > 2^20. OBGPU_INVALID_ARGUMENT:
+ *   n_group_cols outside 1..4, a column out of range, a NULL pointer. A failed call leaves the result with no groups. */
+int obgpu_result_group_by_columns(obgpu_result *res, const int32_t *group_cols, int32_t n_group_cols, const obgpu_group_agg *aggs,
+                                  int32_t n_aggs, int64_t *n_groups, int64_t *key_bytes);
+/* The last groups of either call, any number of columns: host_keys is [n_group_cols][n_groups + 1] -- per integer column the
+ * value's 64-bit image as obgpu_result_fetch_groups gives it (0 where NULL), per string column n_groups + 1 offsets into the
+ * one host_key_heap, each string column's bytes following the previous string column's (a NULL key is empty);
+ * host_key_nulls is [n_group_cols][n_groups], 1 where that column's key is NULL; host_out is [n_aggs][n_groups][2].
+ * One synchronisation. OBGPU_INVALID_ARGUMENT when the result has no groups. */
+int obgpu_result_fetch_group_columns(obgpu_result *res, int64_t *host_keys, uint8_t *host_key_nulls, void *host_key_heap,
+                                     int64_t *host_out);
 
 /* =============================================================================================
  * String cells as BYTES. HEX_PACKING / STRING_DIFF / STRING_PREFIX columns rebuild their values (ObHexStringDecoder,

@@ -232,6 +232,8 @@ def declared_signatures():
         "obgpu_result_group_by": (C.c_int, [vp, i32, vp, i32, vp, vp, i64, P(i64)]),
         "obgpu_result_group_by_values": (C.c_int, [vp, i32, vp, i32, P(i64), P(i64), P(i32)]),
         "obgpu_result_fetch_groups": (C.c_int, [vp, vp, vp, vp]),
+        "obgpu_result_group_by_columns": (C.c_int, [vp, vp, i32, vp, i32, P(i64), P(i64)]),
+        "obgpu_result_fetch_group_columns": (C.c_int, [vp, vp, vp, vp, vp]),
         "obgpu_version": (C.c_char_p, []),
         # include/obgpu_compaction.h
         "obgpu_batch_decode_column": (C.c_int, [vp, i32, vp, vp]),

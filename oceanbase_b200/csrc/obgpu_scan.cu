@@ -1964,11 +1964,12 @@ struct obgpu_result {
   int32_t str_cols[kMaxProj] = {0};
   int64_t str_row_begin = 0, str_rows = 0;
   int64_t str_col_off[kMaxProj + 1] = {0};
-  // obgpu_result_group_by_values: its groups (group_values.cuh), kept for obgpu_result_fetch_groups; gv_groups < 0: none
+  // obgpu_result_group_by_values / _by_columns: their groups (group_values.cuh), kept for obgpu_result_fetch_groups /
+  // obgpu_result_fetch_group_columns; gv_groups < 0: none
   void *d_gv = nullptr;
   int64_t gv_groups = -1, gv_key_bytes = 0;
-  int32_t gv_n_aggs = 0;
-  bool gv_str = false;
+  int32_t gv_n_aggs = 0, gv_n_cols = 0;
+  uint32_t gv_str_mask = 0;   // bit c: group column c is a string column
 };
 
 static thread_local std::string g_last_global_err;

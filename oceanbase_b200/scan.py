@@ -546,6 +546,39 @@ class ScanResult:
             vals[-1] = None
         return vals, out[:, :n]
 
+    def group_by_columns(self, group_cols, aggs):
+        """GROUP BY over every block of the scan with one group per distinct tuple of values of group_cols (1..4 columns,
+        obgpu_result_group_by_columns): returns (keys, out). keys: one tuple per group, in lexicographic order over group_cols,
+        each element a Python int in its column's value domain (unsigned types non-negative), bytes, or None for NULL (last
+        within its column); out: int64 [n_aggs][n_groups][2]."""
+        cols = np.array(list(group_cols), dtype=np.int32)
+        spec = np.array([(k, c) for k, c in aggs], dtype=np.int32).reshape(-1, 2)
+        ng, kb = C.c_int64(0), C.c_int64(0)
+        check(lib.obgpu_result_group_by_columns(self._h, cols.ctypes.data, len(cols), spec.ctypes.data, len(aggs), C.byref(ng), C.byref(kb)),
+              "obgpu_result_group_by_columns", self.batch.ctx._h)
+        n, nc = ng.value, len(cols)
+        keys = np.zeros((nc, n + 1), dtype=np.int64)
+        nulls = np.zeros((nc, max(n, 1)), dtype=np.uint8)
+        heap = np.zeros(max(kb.value, 1), dtype=np.uint8)
+        out = np.zeros((len(aggs), max(n, 1), 2), dtype=np.int64)
+        check(lib.obgpu_result_fetch_group_columns(self._h, keys.ctypes.data, nulls.ctypes.data, heap.ctypes.data, out.ctypes.data),
+              "obgpu_result_fetch_group_columns", self.batch.ctx._h)
+        heap_b = heap.tobytes()
+        per_col = []
+        for c, gc in enumerate(cols.tolist()):
+            obj_type, dlen = C.c_int32(0), C.c_int32(0)
+            check(lib.obgpu_batch_column_type(self.batch._h, gc, C.byref(obj_type), C.byref(dlen)), "obgpu_batch_column_type",
+                  self.batch.ctx._h)
+            k = keys[c].tolist()
+            if dlen.value == 0:
+                vals = [heap_b[k[g]:k[g + 1]] for g in range(n)]
+            elif obj_type.value in (capi.OBJ_UINT64, capi.OBJ_UINT32, capi.OBJ_UTINYINT, capi.OBJ_USMALLINT, capi.OBJ_UMEDIUMINT, capi.OBJ_YEAR):
+                vals = [v & ((1 << 64) - 1) for v in k[:n]]
+            else:
+                vals = k[:n]
+            per_col.append([None if z else v for v, z in zip(vals, nulls[c, :n].tolist())])
+        return list(zip(*per_col)) if n else [], out[:, :n]
+
     def fetch_datums(self, i, row_begin=0, row_count=None):
         """Column i as ObDatum[] (datum format): (datums structured array, slots uint64 array or None for strings)."""
         c = self.col(i)
