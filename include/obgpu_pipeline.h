@@ -95,6 +95,22 @@ const char *obgpu_pipeline_last_error(const obgpu_pipeline *p);
 /* Number of page batches (and their first blocks) a spec is cut into: lets the caller size the result arrays. */
 int obgpu_pipeline_plan(const obgpu_host_scan_spec *spec, int32_t *n_batches, int64_t *rows_cap_needed_hint);
 int obgpu_pipeline_scan(obgpu_pipeline *p, const obgpu_host_scan_spec *spec, obgpu_host_scan_result *result);
+/* GROUP BY group_cols (1..4 store indexes) over every row of the spec's table that its filter selects, with the groups of every
+ * page batch merged on the device: each worker opens its batch as obgpu_pipeline_scan does, scans it with nothing projected,
+ * groups it with obgpu_result_group_by_columns and adds the groups to one accumulator on the pipeline's first ctx (adds are
+ * serialised). Only the groups reach the host, through *out (obgpu_groups_fetch), which the caller frees before destroying
+ * the pipeline. The groups are those of obgpu_result_group_by_columns over the whole table as one batch.
+ *   From spec: image, offsets, sizes, n_blocks, filter, blocks_per_batch, ramp, compressor_type, zero_copy, agg_rows / agg_off.
+ *   It asks for no rows: no_row_output must be 1, out_row_ids, out_block_begin and out_block_count NULL, n_aggs 0; otherwise
+ *   OBGPU_INVALID_ARGUMENT. result is filled as obgpu_pipeline_scan fills it, with batch_row_begin all 0, no aggregates and
+ *   d2h_bytes 0.
+ *   The 65 536-value cap of obgpu_result_group_by_values applies PER PAGE BATCH: a table whose dictionaries hold more distinct
+ *   values in all is grouped as long as no batch's dictionaries do.
+ *   The first refusal of any batch (a column not dictionary coded, more than 65 536 values in one batch's dictionaries, an
+ *   over-long string key, a mismatch between batches' column types, ...) is returned, with its text in
+ *   obgpu_pipeline_last_error; *out is then NULL and the pipeline stays usable. */
+int obgpu_pipeline_group_by(obgpu_pipeline *p, const obgpu_host_scan_spec *spec, const int32_t *group_cols, int32_t n_group_cols,
+                            const obgpu_group_agg *aggs, int32_t n_aggs, obgpu_host_scan_result *result, obgpu_groups **out);
 
 #ifdef __cplusplus
 }

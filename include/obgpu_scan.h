@@ -512,6 +512,32 @@ int obgpu_result_group_by_columns(obgpu_result *res, const int32_t *group_cols, 
  * One synchronisation. OBGPU_INVALID_ARGUMENT when the result has no groups. */
 int obgpu_result_fetch_group_columns(obgpu_result *res, int64_t *host_keys, uint8_t *host_key_nulls, void *host_key_heap,
                                      int64_t *host_out);
+/* A device group accumulator: merges, by value, the groups of several scan results -- typically one per page batch of a
+ * table -- into the groups one obgpu_result_group_by_columns over all their rows would give. It lives on ctx's device, works
+ * on a stream of its own (an add never waits for other work queued on ctx), and holds its groups in device memory, growing as
+ * they arrive; n_group_cols (1..4) and aggs (1..16, as obgpu_result_group_by_columns)
+ * are what every added result's groups must have. Not thread-safe, as every handle here: callers serialise adds.
+ *   Same groups as one batch: whatever the cut of the rows into results, the order of the adds and the ctxs the results were
+ *   scanned on, obgpu_groups_fetch returns byte for byte what obgpu_result_group_by_columns returns over the same rows opened
+ *   as one batch (when that call accepts them): keys, NULL flags, key heap and aggregates, in its order. COUNT and SUM add in
+ *   128 bits; MIN / MAX compare in the column's own signed or unsigned order. */
+typedef struct obgpu_groups obgpu_groups;
+int obgpu_groups_create(obgpu_ctx *ctx, int32_t n_group_cols, const obgpu_group_agg *aggs, int32_t n_aggs, obgpu_groups **out);
+void obgpu_groups_free(obgpu_groups *groups);
+/* Merges the result's current groups (its last obgpu_result_group_by_columns / _values) into the accumulator. Synchronous:
+ * when it returns, the groups have been consumed and the result (and its batch) may be freed. The result may belong to another
+ * ctx on the same device; the add's error text and kernel launches are that ctx's (obgpu_ctx_last_error, _launch_count).
+ *   OBGPU_NOT_SUPPORTED: another number of group columns, other aggregate kinds or columns, a group or aggregate column of
+ *   another obj_type than in the first add, or more than 2^31 - 1 groups (the accumulator's plus the result's).
+ *   OBGPU_INVALID_ARGUMENT: a result with no groups, or on another device. OBGPU_ALLOCATE_MEMORY_FAILED: the device memory to
+ *   grow into is not there. A refused or failed add leaves the accumulator as it was. */
+int obgpu_groups_add(obgpu_groups *groups, obgpu_result *res);
+/* *n_groups, *key_bytes (the key heap obgpu_groups_fetch fills), and per group column its obj_type and datum length as
+ * obgpu_batch_column_type gives them (0 and -1 before the first add). Any pointer may be NULL. */
+int obgpu_groups_info(obgpu_groups *groups, int64_t *n_groups, int64_t *key_bytes, int32_t *obj_types, int32_t *datum_lens);
+/* The groups in obgpu_result_fetch_group_columns' host layout and order. Sorts them on the first fetch after an add; later
+ * fetches copy the cached result. One synchronisation. */
+int obgpu_groups_fetch(obgpu_groups *groups, int64_t *host_keys, uint8_t *host_key_nulls, void *host_key_heap, int64_t *host_out);
 
 /* =============================================================================================
  * String cells as BYTES. HEX_PACKING / STRING_DIFF / STRING_PREFIX columns rebuild their values (ObHexStringDecoder,

@@ -20,5 +20,5 @@ from .sstable import (  # noqa: F401
     Column, TableImage, encode_table, encode_block, agg_row_write, block_agg_row, table_agg_rows,
 )
 from .scan import (  # noqa: F401
-    White, And, Or, ScanContext, PageBatch, ScanResult, CGBitmap, flatten_filter, DATUM_DTYPE, DATUM_NULL_BIT,
+    White, And, Or, ScanContext, PageBatch, ScanResult, CGBitmap, GroupAccumulator, flatten_filter, DATUM_DTYPE, DATUM_NULL_BIT,
 )

@@ -45,6 +45,7 @@ constexpr int kMaxGroupCols = 4;
 constexpr uint32_t kRankCap = 256;                // dictionary entries a warp maps to ranks in shared memory; larger: probe per row
 constexpr size_t kRankBytes = (size_t)kWarpsPerCta * kRankCap * 4;   // a CTA's rank arrays of one group column
 constexpr size_t kSharedAccBudget = 48u << 10;    // CTA-private accumulators, P x (n_aggs + 1) x 16 bytes, when they fit
+constexpr size_t kMaxFoldSmem = kMaxGroupCols * kRankBytes + kSharedAccBudget;   // the most dynamic shared memory a fold launch takes
 constexpr uint64_t kDenseGroups = 1ull << 20;     // the most ids the global path indexes directly; more: hashed
 constexpr uint32_t kHashSlots = 1u << 23;         // the hashed path's id table (64 MiB)
 constexpr uint32_t kHashGroups = 1u << 22;        // the most distinct ids the hashed path takes: the table at most half full
@@ -570,7 +571,9 @@ static int group_by_columns(obgpu_result *r, const int32_t *cols, int n_cols, co
   const auto launch = [&](int pth, size_t acc_smem) -> int {
     const FoldFn fold = n_cols > 1 ? fold_fn<MULTI>(pth) : fp.gc[0].str ? fold_fn<ONE_STR>(pth) : fold_fn<ONE_INT>(pth);
     const size_t smem = rank_smem + acc_smem;
-    CUDA_TRY(ctx, cudaFuncSetAttribute(fold, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    // the attribute is the kernel's, shared by every ctx and thread of the process: always the one largest value any launch
+    // needs, so that concurrent calls (one per pipeline worker) never lower it under another's launch
+    CUDA_TRY(ctx, cudaFuncSetAttribute(fold, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kMaxFoldSmem));
     unsigned grid = key_grid;
     if (pth == PATH_SHARED) {   // few CTAs, each folding many blocks: one flush per resident CTA
       int per_sm = 0;
@@ -709,9 +712,34 @@ static int group_by_columns(obgpu_result *r, const int32_t *cols, int n_cols, co
   r->gv_n_aggs = n_aggs;
   r->gv_n_cols = n_cols;
   r->gv_str_mask = str_mask;
+  for (int k = 0; k < n_aggs; ++k) {
+    r->gv_kind[k] = aggs[k].kind;
+    r->gv_agg_col[k] = aggs[k].col;
+    r->gv_agg_type[k] = aggs[k].col >= 0 ? b->col_types[(size_t)aggs[k].col] : -1;
+  }
+  r->gv_sgn_key = 0;
+  for (int c = 0; c < n_cols; ++c) {
+    r->gv_key_type[c] = b->col_types[(size_t)cols[c]];
+    if (st[c]->sgn_key) r->gv_sgn_key |= 1u << c;
+  }
+  r->gv_sgn_agg = gp.sgn_agg;
   *n_groups = ng;
   *key_bytes = kb;
   if (has_null) *has_null = null_last;
+  return OBGPU_SUCCESS;
+}
+
+// groups in the GroupBuf layout at gv -> the host layout of obgpu_result_fetch_group_columns; one synchronisation
+static int copy_groups(obgpu_ctx *ctx, const uint8_t *gv, int64_t ng, int n_cols, int n_aggs, int64_t key_bytes, int64_t *host_keys,
+                       uint8_t *host_key_nulls, void *host_key_heap, int64_t *host_out) {
+  const GroupBuf lay(ng, n_cols, n_aggs, key_bytes);
+  CUDA_TRY(ctx, cudaMemcpyAsync(host_keys, gv, lay.out, cudaMemcpyDeviceToHost, ctx->stream));
+  if (ng > 0) {
+    CUDA_TRY(ctx, cudaMemcpyAsync(host_out, gv + lay.out, lay.nulls - lay.out, cudaMemcpyDeviceToHost, ctx->stream));
+    CUDA_TRY(ctx, cudaMemcpyAsync(host_key_nulls, gv + lay.nulls, (size_t)n_cols * (size_t)ng, cudaMemcpyDeviceToHost, ctx->stream));
+  }
+  if (key_bytes > 0) CUDA_TRY(ctx, cudaMemcpyAsync(host_key_heap, gv + lay.heap, (size_t)key_bytes, cudaMemcpyDeviceToHost, ctx->stream));
+  CUDA_TRY(ctx, cudaStreamSynchronize(ctx->stream));
   return OBGPU_SUCCESS;
 }
 
@@ -758,20 +786,9 @@ int obgpu_result_fetch_groups(obgpu_result *r, int64_t *host_keys, void *host_ke
 int obgpu_result_fetch_group_columns(obgpu_result *r, int64_t *host_keys, uint8_t *host_key_nulls, void *host_key_heap, int64_t *host_out) {
   if (!r || r->gv_groups < 0 || !host_keys || !host_key_nulls || !host_out || (r->gv_key_bytes > 0 && !host_key_heap))
     return OBGPU_INVALID_ARGUMENT;
-  obgpu_ctx *ctx = r->ctx;
-  cudaSetDevice(ctx->device);
-  const int64_t ng = r->gv_groups;
-  const gvals::GroupBuf lay(ng, r->gv_n_cols, r->gv_n_aggs, r->gv_key_bytes);
-  const uint8_t *gv = (const uint8_t *)r->d_gv;
-  CUDA_TRY(ctx, cudaMemcpyAsync(host_keys, gv, lay.out, cudaMemcpyDeviceToHost, ctx->stream));
-  if (ng > 0) {
-    CUDA_TRY(ctx, cudaMemcpyAsync(host_out, gv + lay.out, lay.nulls - lay.out, cudaMemcpyDeviceToHost, ctx->stream));
-    CUDA_TRY(ctx, cudaMemcpyAsync(host_key_nulls, gv + lay.nulls, (size_t)r->gv_n_cols * (size_t)ng, cudaMemcpyDeviceToHost, ctx->stream));
-  }
-  if (r->gv_key_bytes > 0)
-    CUDA_TRY(ctx, cudaMemcpyAsync(host_key_heap, gv + lay.heap, (size_t)r->gv_key_bytes, cudaMemcpyDeviceToHost, ctx->stream));
-  CUDA_TRY(ctx, cudaStreamSynchronize(ctx->stream));
-  return OBGPU_SUCCESS;
+  cudaSetDevice(r->ctx->device);
+  return gvals::copy_groups(r->ctx, (const uint8_t *)r->d_gv, r->gv_groups, r->gv_n_cols, r->gv_n_aggs, r->gv_key_bytes, host_keys,
+                            host_key_nulls, host_key_heap, host_out);
 }
 
 }  // extern "C"

@@ -43,6 +43,44 @@ inline bool compressor_ok(int32_t c) {
          c == OBGPU_COMPRESSOR_LZ4_1_9_1;
 }
 
+// opens blocks [b0, b1) of the spec as a page batch (the image rebased to the batch's first block) and attaches their skip
+// index; *lo / *hi: the batch's byte range of the image
+inline int open_batch(obgpu_ctx *ctx, const obgpu_host_scan_spec *s, int32_t b0, int32_t b1, int64_t *lo, int64_t *hi, obgpu_batch **out) {
+  *lo = s->offsets[b0];
+  *hi = b1 < s->n_blocks ? s->offsets[b1] : s->image_size;
+  std::vector<int64_t> offs((size_t)(b1 - b0));
+  for (int32_t i = b0; i < b1; ++i) offs[(size_t)(i - b0)] = s->offsets[i] - *lo;
+  const uint8_t *img = (const uint8_t *)s->image + *lo;
+  obgpu_batch *batch = nullptr;
+  int ret = s->compressor_type ? obgpu_batch_open_compressed(ctx, img, *hi - *lo, offs.data(), s->sizes + b0, b1 - b0, 0, s->compressor_type, &batch)
+            : s->zero_copy     ? obgpu_batch_open(ctx, img, *hi - *lo, offs.data(), s->sizes + b0, b1 - b0, 1, img, &batch)   // the pinned host image IS the device image
+                               : obgpu_batch_open(ctx, img, *hi - *lo, offs.data(), s->sizes + b0, b1 - b0, 0, nullptr, &batch);
+  if (ret != OBGPU_SUCCESS) return ret;
+  batch->codes_allowed = false;   // scanned once: batch string codes would cost more than they save
+  if (s->agg_rows && s->agg_off) {   // offsets keep their table-wide base: the entry rebases them
+    ret = obgpu_batch_set_agg_rows(batch, s->agg_rows, s->agg_off + b0);
+    if (ret != OBGPU_SUCCESS) {
+      obgpu_batch_close(batch);
+      return ret;
+    }
+  }
+  *out = batch;
+  return OBGPU_SUCCESS;
+}
+
+// what obgpu_pipeline_scan and obgpu_pipeline_group_by refuse alike before any batch is opened
+inline int check_source(obgpu_pipeline *p, const obgpu_host_scan_spec *s) {
+  if (!compressor_ok(s->compressor_type)) {
+    p->err = "compressor_type " + std::to_string(s->compressor_type) + " is not decoded on the device";
+    return OBGPU_NOT_SUPPORTED;
+  }
+  if (s->compressor_type && s->zero_copy) {
+    p->err = "zero_copy with a compressor: the decoder reads every stored byte";
+    return OBGPU_NOT_SUPPORTED;
+  }
+  return OBGPU_SUCCESS;
+}
+
 inline void add128(int64_t acc[2], int64_t lo, int64_t hi) {
   const uint64_t nlo = (uint64_t)acc[0] + (uint64_t)lo;
   acc[1] = (int64_t)((uint64_t)acc[1] + (uint64_t)hi + (nlo < (uint64_t)acc[0] ? 1u : 0u));
@@ -101,14 +139,7 @@ int obgpu_pipeline_scan(obgpu_pipeline *p, const obgpu_host_scan_spec *s, obgpu_
   if (!p || !s || !res || s->n_blocks <= 0 || !s->image || !s->offsets || !s->sizes || s->n_proj < 0 || s->n_aggs < 0 || s->n_aggs > 16)
     return OBGPU_INVALID_ARGUMENT;
   if (!s->no_row_output && s->n_proj > 0 && (!s->out_data || !s->out_nulls)) return OBGPU_INVALID_ARGUMENT;
-  if (!obpipe::compressor_ok(s->compressor_type)) {
-    p->err = "compressor_type " + std::to_string(s->compressor_type) + " is not decoded on the device";
-    return OBGPU_NOT_SUPPORTED;
-  }
-  if (s->compressor_type && s->zero_copy) {
-    p->err = "zero_copy with a compressor: the decoder reads every stored byte";
-    return OBGPU_NOT_SUPPORTED;
-  }
+  if (const int ret = obpipe::check_source(p, s); ret != OBGPU_SUCCESS) return ret;
   const bool heaps = s->out_heap && !s->no_row_output;
   if (heaps)
     for (int32_t c = 0; c < s->n_proj; ++c)
@@ -159,10 +190,7 @@ int obgpu_pipeline_scan(obgpu_pipeline *p, const obgpu_host_scan_spec *s, obgpu_
       const int32_t b = next.fetch_add(1);
       if (b >= nb || first_err.load() != OBGPU_SUCCESS) return;
       const int32_t b0 = bounds[(size_t)b], b1 = bounds[(size_t)b + 1];
-      const int64_t lo = s->offsets[b0];
-      const int64_t hi = b1 < s->n_blocks ? s->offsets[b1] : s->image_size;
-      std::vector<int64_t> offs((size_t)(b1 - b0));
-      for (int32_t i = b0; i < b1; ++i) offs[(size_t)(i - b0)] = s->offsets[i] - lo;
+      int64_t lo = 0, hi = 0;
       obgpu_batch *batch = nullptr;
       obgpu_result *r = nullptr;
       auto fail = [&](int code) {
@@ -174,19 +202,8 @@ int obgpu_pipeline_scan(obgpu_pipeline *p, const obgpu_host_scan_spec *s, obgpu_
         if (r) obgpu_result_free(r);
         if (batch) obgpu_batch_close(batch);
       };
-      int ret = s->compressor_type
-                    ? obgpu_batch_open_compressed(ctx, (const uint8_t *)s->image + lo, hi - lo, offs.data(), s->sizes + b0, b1 - b0, 0,
-                                                  s->compressor_type, &batch)
-                : s->zero_copy
-                    ? obgpu_batch_open(ctx, (const uint8_t *)s->image + lo, hi - lo, offs.data(), s->sizes + b0, b1 - b0, 1,
-                                       (const uint8_t *)s->image + lo, &batch)   // the pinned host image IS the device image
-                    : obgpu_batch_open(ctx, (const uint8_t *)s->image + lo, hi - lo, offs.data(), s->sizes + b0, b1 - b0, 0, nullptr, &batch);
+      int ret = obpipe::open_batch(ctx, s, b0, b1, &lo, &hi, &batch);
       if (ret != OBGPU_SUCCESS) { fail(ret); return; }
-      batch->codes_allowed = false;   // scanned once: batch string codes would cost more than they save
-      if (s->agg_rows && s->agg_off) {   // offsets keep their table-wide base: the entry rebases them
-        ret = obgpu_batch_set_agg_rows(batch, s->agg_rows, s->agg_off + b0);
-        if (ret != OBGPU_SUCCESS) { fail(ret); return; }
-      }
       std::vector<int32_t> heap_cols;   // projected string columns whose bytes go to a heap
       if (!s->no_row_output) {
         // a string column whose values the device rebuilt (HEX_PACKING / STRING_DIFF / STRING_PREFIX) or decoded (compressed
@@ -354,6 +371,97 @@ int obgpu_pipeline_scan(obgpu_pipeline *p, const obgpu_host_scan_spec *s, obgpu_
     res->kernel_launches += obgpu_ctx_launch_count(p->ctxs[i]) - launches0[i];
   }
   return first_err.load();
+}
+
+int obgpu_pipeline_group_by(obgpu_pipeline *p, const obgpu_host_scan_spec *s, const int32_t *group_cols, int32_t n_group_cols,
+                            const obgpu_group_agg *aggs, int32_t n_aggs, obgpu_host_scan_result *res, obgpu_groups **out) {
+  if (!p || !s || !res || !out || s->n_blocks <= 0 || !s->image || !s->offsets || !s->sizes || !group_cols || n_group_cols < 1 ||
+      n_group_cols > gvals::kMaxGroupCols || !aggs || n_aggs < 1 || n_aggs > 16)
+    return OBGPU_INVALID_ARGUMENT;
+  *out = nullptr;
+  if (!s->no_row_output || s->out_row_ids || s->out_block_begin || s->out_block_count || s->n_aggs != 0) {
+    p->err = "a GROUP BY through the pipeline returns groups only: no_row_output 1, no row ids, block tables or scalar aggregates";
+    return OBGPU_INVALID_ARGUMENT;
+  }
+  if (const int ret = obpipe::check_source(p, s); ret != OBGPU_SUCCESS) return ret;
+  std::vector<int32_t> bounds;
+  obpipe::batch_bounds(s->n_blocks, obpipe::default_bpb(s), std::max(0, s->ramp), bounds);
+  const int32_t nb = (int32_t)bounds.size() - 1;
+  if (nb > res->n_batches_cap || !res->batch_row_begin || !res->batch_rows) return OBGPU_BUF_NOT_ENOUGH;
+  obgpu_groups *acc = nullptr;
+  if (const int ret = obgpu_groups_create(p->ctxs[0], n_group_cols, aggs, n_aggs, &acc); ret != OBGPU_SUCCESS) {
+    p->err = obgpu_ctx_last_error(p->ctxs[0]);
+    return ret;
+  }
+  for (int32_t b = 0; b < nb; ++b) {
+    res->batch_row_begin[b] = 0;
+    if (res->batch_block_begin) res->batch_block_begin[b] = bounds[(size_t)b];
+  }
+  if (res->batch_block_begin) res->batch_block_begin[nb] = s->n_blocks;
+  res->n_batches = nb;
+  res->total_rows = res->selected_rows = 0;
+  res->h2d_bytes = res->d2h_bytes = res->kernel_launches = 0;
+  memset(res->agg_out, 0, sizeof(res->agg_out));
+
+  std::atomic<int32_t> next{0};
+  std::atomic<int> first_err{OBGPU_SUCCESS};
+  std::mutex mu;   // the accumulator, result totals, error text
+  std::vector<int64_t> launches0;
+  for (obgpu_ctx *c : p->ctxs) launches0.push_back(obgpu_ctx_launch_count(c));
+
+  auto worker = [&](obgpu_ctx *ctx) {
+    for (;;) {
+      const int32_t b = next.fetch_add(1);
+      if (b >= nb || first_err.load() != OBGPU_SUCCESS) return;
+      int64_t lo = 0, hi = 0;
+      obgpu_batch *batch = nullptr;
+      obgpu_result *r = nullptr;
+      obgpu_result_info info{};
+      int ret = obpipe::open_batch(ctx, s, bounds[(size_t)b], bounds[(size_t)b + 1], &lo, &hi, &batch);
+      if (ret == OBGPU_SUCCESS) {
+        obgpu_scan_spec spec{};   // nothing projected; the capacity is the batch's rows
+        spec.filter = s->filter;
+        ret = obgpu_scan(batch, &spec, &r);
+      }
+      if (ret == OBGPU_SUCCESS) ret = obgpu_result_info_get(r, &info);
+      int64_t ng = 0, kb = 0;
+      if (ret == OBGPU_SUCCESS) ret = obgpu_result_group_by_columns(r, group_cols, n_group_cols, aggs, n_aggs, &ng, &kb);
+      if (ret == OBGPU_SUCCESS) {
+        std::lock_guard<std::mutex> g(mu);
+        if (first_err.load() == OBGPU_SUCCESS) ret = obgpu_groups_add(acc, r);
+        if (ret == OBGPU_SUCCESS) {
+          res->batch_rows[b] = info.selected_rows;
+          res->total_rows += info.total_rows;
+          res->selected_rows += info.selected_rows;
+          if (!s->zero_copy) res->h2d_bytes += hi - lo;   // zero copy: the kernels read what they reference, the library copies nothing
+        }
+      }
+      if (ret != OBGPU_SUCCESS) {
+        int expected = OBGPU_SUCCESS;
+        if (first_err.compare_exchange_strong(expected, ret)) {
+          std::lock_guard<std::mutex> g(mu);
+          p->err = obgpu_ctx_last_error(ctx);
+        }
+      }
+      if (r) obgpu_result_free(r);
+      if (batch) obgpu_batch_close(batch);
+      if (ret != OBGPU_SUCCESS) return;
+    }
+  };
+  std::vector<std::thread> th;
+  for (size_t i = 1; i < p->ctxs.size(); ++i) th.emplace_back(worker, p->ctxs[i]);
+  worker(p->ctxs[0]);
+  for (auto &t : th) t.join();
+  for (size_t i = 0; i < p->ctxs.size(); ++i) {
+    obgpu_ctx_synchronize(p->ctxs[i]);
+    res->kernel_launches += obgpu_ctx_launch_count(p->ctxs[i]) - launches0[i];
+  }
+  if (first_err.load() != OBGPU_SUCCESS) {
+    obgpu_groups_free(acc);
+    return first_err.load();
+  }
+  *out = acc;
+  return OBGPU_SUCCESS;
 }
 
 }  // extern "C"

@@ -1970,6 +1970,11 @@ struct obgpu_result {
   int64_t gv_groups = -1, gv_key_bytes = 0;
   int32_t gv_n_aggs = 0, gv_n_cols = 0;
   uint32_t gv_str_mask = 0;   // bit c: group column c is a string column
+  // what obgpu_groups_add checks and orders by: the aggregates' kinds, columns and columns' obj_types, each group column's
+  // obj_type, and which order keys have their sign bit flipped (bit c: group column c; bit k: aggregate k's MIN / MAX)
+  int32_t gv_kind[16] = {0}, gv_agg_col[16] = {0}, gv_agg_type[16] = {0};
+  int32_t gv_key_type[4] = {0};   // gvals::kMaxGroupCols
+  uint32_t gv_sgn_key = 0, gv_sgn_agg = 0;
 };
 
 static thread_local std::string g_last_global_err;
@@ -3431,6 +3436,7 @@ int obgpu_project_datums(obgpu_batch *batch, int32_t block, int32_t col, const i
 // ---- dictionary surface: distinct values, references, black filter on one dictionary column, GROUP BY ----
 #include "dict_ops.cuh"
 #include "group_values.cuh"   // GROUP BY over a scan, one group per distinct value of the batch
+#include "group_merge.cuh"    // the groups of several scans merged by value on the device (obgpu_groups)
 
 // ---- major-compaction merge (include/obgpu_compaction.h) -----------------------------------------
 #include "../../include/obgpu_compaction.h"

@@ -15,7 +15,7 @@ import numpy as np
 
 from . import capi
 from .capi import lib
-from .scan import flatten_filter
+from .scan import GroupAccumulator, flatten_filter
 from .sstable import TableImage
 
 
@@ -123,6 +123,19 @@ class HostScanOutput:
     kernel_launches: int
     block_begin: Optional[np.ndarray] = None  # want_block_tables: int64 [n_blocks] output row where block i's selected rows start
     block_count: Optional[np.ndarray] = None  # ... and int64 [n_blocks] how many there are
+
+
+@dataclass
+class GroupByStats:
+    """What obgpu_pipeline_group_by reports besides the groups: the batch cut and totals, as obgpu_pipeline_scan reports them."""
+    n_batches: int
+    batch_block_begin: np.ndarray    # int32 [n_batches + 1]
+    batch_rows: np.ndarray           # int64 [n_batches]: selected rows of every batch
+    total_rows: int
+    selected_rows: int
+    h2d_bytes: int
+    d2h_bytes: int
+    kernel_launches: int
 
 
 def plan(table: TableImage, blocks_per_batch: int, selectivity_hint: float, ramp: int = 0):
@@ -317,6 +330,43 @@ class HostScanPipeline:
                              int(res.d2h_bytes), int(res.kernel_launches), block_begin, block_count)
         out._keep = (keep, outputs, row_ids)
         return out
+
+    def group_by(self, table: TableImage, filter, group_cols: Sequence[int], aggs: Sequence[tuple], blocks_per_batch: int = 0,
+                 ramp: int = 0, compressor: int = 0, zero_copy: bool = False, agg_rows: Optional[np.ndarray] = None,
+                 agg_off: Optional[np.ndarray] = None):
+        """GROUP BY group_cols (1..4 store indexes) over the rows of a host table that filter selects, every page batch grouped
+        and its groups merged on the device (obgpu_pipeline_group_by). aggs: (kind, store col or -1) as
+        ScanResult.group_by_columns takes them. Returns (keys, out, GroupByStats); keys and out are exactly what
+        ScanResult.group_by_columns returns over the whole table as one batch. blocks_per_batch 0: n_blocks / 12."""
+        spec, keep = self._spec(table, filter, [], blocks_per_batch, 1.0, ramp, 0, agg_rows, agg_off)
+        spec.no_row_output = 1
+        spec.compressor_type = int(compressor)
+        spec.zero_copy = 1 if zero_copy else 0   # table.image must then be pinned host memory (the kernels read it over PCIe)
+        nb, cap = C.c_int32(0), C.c_int64(0)
+        capi.check(lib.obgpu_pipeline_plan(C.byref(spec), C.byref(nb), C.byref(cap)), "obgpu_pipeline_plan")
+        cols = np.array(list(group_cols), dtype=np.int32)
+        gspec = np.array([(k, c) for k, c in aggs], dtype=np.int32).reshape(-1, 2)
+        res = capi.HostScanResult()
+        row_begin = np.zeros(nb.value + 1, dtype=np.int64)
+        rows = np.zeros(nb.value + 1, dtype=np.int64)
+        blk_begin = np.zeros(nb.value + 2, dtype=np.int32)
+        res.batch_row_begin, res.batch_rows, res.batch_block_begin = row_begin.ctypes.data, rows.ctypes.data, blk_begin.ctypes.data
+        res.n_batches_cap = nb.value
+        h = C.c_void_p()
+        code = lib.obgpu_pipeline_group_by(self._h, C.byref(spec), cols.ctypes.data, len(cols), gspec.ctypes.data if len(aggs) else None,
+                                           len(aggs), C.byref(res), C.byref(h))
+        if code != capi.OB_SUCCESS:
+            raise capi.ObGpuError(code, "obgpu_pipeline_group_by", (lib.obgpu_pipeline_last_error(self._h) or b"").decode())
+        self.launch_count += res.kernel_launches
+        acc = GroupAccumulator(h, len(cols), len(aggs), self)
+        try:
+            keys, out = acc.fetch()
+        finally:
+            acc.free()
+        n = res.n_batches
+        stats = GroupByStats(n, blk_begin[:n + 1].copy(), rows[:n].copy(), int(res.total_rows), int(res.selected_rows), int(res.h2d_bytes),
+                             int(res.d2h_bytes), int(res.kernel_launches))
+        return keys, out, stats
 
     def _column_shapes(self, table, proj, compressor=0):
         """(is_string, elem_len) of the projected columns, read from the first block's column headers. A stored block's

@@ -86,6 +86,23 @@ def flatten_filter(expr: Optional[FilterExpr], node_cls=capi.FilterNode, param_c
     return f, (node_arr, param_arr, keep)
 
 
+def group_tuples(keys, nulls, heap, n, types):
+    """Groups in obgpu_result_fetch_group_columns' host layout -> one tuple per group: per column (obj_type, datum_len) of
+    types, a Python int in the column's value domain (unsigned types non-negative), bytes, or None for NULL."""
+    heap_b = heap.tobytes()
+    per_col = []
+    for c, (obj_type, dlen) in enumerate(types):
+        k = keys[c].tolist()
+        if dlen == 0:
+            vals = [heap_b[k[g]:k[g + 1]] for g in range(n)]
+        elif obj_type in (capi.OBJ_UINT64, capi.OBJ_UINT32, capi.OBJ_UTINYINT, capi.OBJ_USMALLINT, capi.OBJ_UMEDIUMINT, capi.OBJ_YEAR):
+            vals = [v & ((1 << 64) - 1) for v in k[:n]]
+        else:
+            vals = k[:n]
+        per_col.append([None if z else v for v, z in zip(vals, nulls[c, :n].tolist())])
+    return list(zip(*per_col)) if n else []
+
+
 # ---- context / batch / result ----------------------------------------------------------------------
 class ScanContext:
     """obgpu_ctx: one per worker thread (device + stream)."""
@@ -128,6 +145,10 @@ class ScanContext:
         cnt, proj, flags = C.c_int32(0), C.c_int32(0), C.c_int32(0)
         check(lib.obgpu_ctx_scan_plan(self._h, C.byref(cnt), C.byref(proj), C.byref(flags)), "obgpu_ctx_scan_plan", self._h)
         return cnt.value, proj.value, flags.value
+
+    def group_accumulator(self, n_group_cols: int, aggs) -> "GroupAccumulator":
+        """obgpu_groups on this ctx: merges the groups of ScanResult.group_by_columns / group_by_values of several results by value."""
+        return GroupAccumulator.create(self, n_group_cols, aggs)
 
     def open_batch(self, table, device_image_ptr: Optional[int] = None, host_view: bool = True,
                    image_size: Optional[int] = None, compressor: Optional[int] = None) -> "PageBatch":
@@ -563,21 +584,13 @@ class ScanResult:
         out = np.zeros((len(aggs), max(n, 1), 2), dtype=np.int64)
         check(lib.obgpu_result_fetch_group_columns(self._h, keys.ctypes.data, nulls.ctypes.data, heap.ctypes.data, out.ctypes.data),
               "obgpu_result_fetch_group_columns", self.batch.ctx._h)
-        heap_b = heap.tobytes()
-        per_col = []
-        for c, gc in enumerate(cols.tolist()):
+        types = []
+        for gc in cols.tolist():
             obj_type, dlen = C.c_int32(0), C.c_int32(0)
             check(lib.obgpu_batch_column_type(self.batch._h, gc, C.byref(obj_type), C.byref(dlen)), "obgpu_batch_column_type",
                   self.batch.ctx._h)
-            k = keys[c].tolist()
-            if dlen.value == 0:
-                vals = [heap_b[k[g]:k[g + 1]] for g in range(n)]
-            elif obj_type.value in (capi.OBJ_UINT64, capi.OBJ_UINT32, capi.OBJ_UTINYINT, capi.OBJ_USMALLINT, capi.OBJ_UMEDIUMINT, capi.OBJ_YEAR):
-                vals = [v & ((1 << 64) - 1) for v in k[:n]]
-            else:
-                vals = k[:n]
-            per_col.append([None if z else v for v, z in zip(vals, nulls[c, :n].tolist())])
-        return list(zip(*per_col)) if n else [], out[:, :n]
+            types.append((obj_type.value, dlen.value))
+        return group_tuples(keys, nulls, heap, n, types), out[:, :n]
 
     def fetch_datums(self, i, row_begin=0, row_count=None):
         """Column i as ObDatum[] (datum format): (datums structured array, slots uint64 array or None for strings)."""
@@ -659,6 +672,67 @@ class ScanResult:
         if self._h:
             if self.batch.ctx._h:
                 lib.obgpu_result_free(self._h)
+            self._h = C.c_void_p()
+
+    def __del__(self):
+        try:
+            self.free()
+        except Exception:
+            pass
+
+
+class GroupAccumulator:
+    """obgpu_groups: the groups of several scan results (any page batches, any ctx of the device) merged by value on the device.
+    fetch() returns (keys, out) in exactly ScanResult.group_by_columns' shape: what that call returns over all the added rows
+    as one batch."""
+
+    def __init__(self, handle, n_group_cols: int, n_aggs: int, owner, ctx: Optional[ScanContext] = None):
+        self._h = handle
+        self.n_cols, self.n_aggs = n_group_cols, n_aggs
+        self.owner = owner   # what its ctx belongs to (a ScanContext or a HostScanPipeline): freed only while that is open
+        self.ctx = ctx
+
+    @classmethod
+    def create(cls, ctx: ScanContext, n_group_cols: int, aggs):
+        spec = np.array([(k, c) for k, c in aggs], dtype=np.int32).reshape(-1, 2)
+        h = C.c_void_p()
+        check(lib.obgpu_groups_create(ctx._h, n_group_cols, spec.ctypes.data if len(aggs) else None, len(aggs), C.byref(h)),
+              "obgpu_groups_create", ctx._h)
+        return cls(h, n_group_cols, len(aggs), ctx, ctx)
+
+    def add(self, result: "ScanResult"):
+        """Merge the result's current groups in; the result may be freed afterwards."""
+        check(lib.obgpu_groups_add(self._h, result._h), "obgpu_groups_add", result.batch.ctx._h)
+
+    def info(self):
+        """(n_groups, key_bytes, [(obj_type, datum_len) per group column])"""
+        ng, kb = C.c_int64(0), C.c_int64(0)
+        types, lens = np.zeros(4, dtype=np.int32), np.zeros(4, dtype=np.int32)
+        check(lib.obgpu_groups_info(self._h, C.byref(ng), C.byref(kb), types.ctypes.data, lens.ctypes.data), "obgpu_groups_info",
+              self.ctx._h if self.ctx else None)
+        return ng.value, kb.value, list(zip(types[:self.n_cols].tolist(), lens[:self.n_cols].tolist()))
+
+    def fetch_raw(self):
+        """(keys int64 [n_cols][n + 1], nulls uint8 [n_cols][n], heap uint8, out int64 [n_aggs][n][2]): the host layout of
+        obgpu_result_fetch_group_columns."""
+        n, kb, _ = self.info()
+        keys = np.zeros((self.n_cols, n + 1), dtype=np.int64)
+        nulls = np.zeros((self.n_cols, max(n, 1)), dtype=np.uint8)
+        heap = np.zeros(max(kb, 1), dtype=np.uint8)
+        out = np.zeros((self.n_aggs, max(n, 1), 2), dtype=np.int64)
+        check(lib.obgpu_groups_fetch(self._h, keys.ctypes.data, nulls.ctypes.data, heap.ctypes.data, out.ctypes.data), "obgpu_groups_fetch",
+              self.ctx._h if self.ctx else None)
+        return keys, nulls[:, :n], heap[:kb], out[:, :n]
+
+    def fetch(self):
+        n, _, types = self.info()
+        keys, nulls, heap, out = self.fetch_raw()
+        return group_tuples(keys, nulls, heap, n, types), out
+
+    def free(self):
+        if self._h:
+            if self.owner._h:
+                lib.obgpu_groups_free(self._h)
             self._h = C.c_void_p()
 
     def __del__(self):
