@@ -111,6 +111,22 @@ int obgpu_pipeline_scan(obgpu_pipeline *p, const obgpu_host_scan_spec *spec, obg
  *   obgpu_pipeline_last_error; *out is then NULL and the pipeline stays usable. */
 int obgpu_pipeline_group_by(obgpu_pipeline *p, const obgpu_host_scan_spec *spec, const int32_t *group_cols, int32_t n_group_cols,
                             const obgpu_group_agg *aggs, int32_t n_aggs, obgpu_host_scan_result *result, obgpu_groups **out);
+/* ORDER BY keys LIMIT k over every row of the spec's table that its filter selects: each worker opens its batch as
+ * obgpu_pipeline_group_by does, scans it with nothing projected, takes its rows with obgpu_result_top_rows and merges them, under
+ * the pipeline's mutex, into one device-resident set of at most k rows (at most 2k rows ordered per merge, k kept). Positions are
+ * made table-wide: a row's block is the index into the spec's block list. The rows are byte for byte those of
+ * obgpu_result_top_rows over the whole table opened as one batch, whatever the batch cut, ramp or worker count. *n_rows and
+ * *heap_bytes are set; obgpu_pipeline_fetch_top_rows copies the rows out in obgpu_result_fetch_top_rows' layout, and they stay
+ * with the pipeline until its next obgpu_pipeline_top_rows or obgpu_pipeline_destroy.
+ *   Spec and result as obgpu_pipeline_group_by: no_row_output 1, no row ids, block tables or scalar aggregates
+ *   (OBGPU_INVALID_ARGUMENT otherwise). Arguments as obgpu_result_top_rows. The first refusal of any batch (including a key or
+ *   output column whose obj_type differs between batches) is returned with its text in obgpu_pipeline_last_error; the
+ *   pipeline then holds no rows and stays usable. */
+int obgpu_pipeline_top_rows(obgpu_pipeline *p, const obgpu_host_scan_spec *spec, const obgpu_sort_key *keys, int32_t n_keys,
+                            const int32_t *out_cols, int32_t n_out, int64_t k, obgpu_host_scan_result *result, int64_t *n_rows,
+                            int64_t *heap_bytes);
+int obgpu_pipeline_fetch_top_rows(obgpu_pipeline *p, int32_t *host_block, int32_t *host_row, int64_t *host_vals, uint8_t *host_nulls,
+                                  void *host_heap);
 
 #ifdef __cplusplus
 }

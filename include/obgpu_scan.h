@@ -512,6 +512,35 @@ int obgpu_result_group_by_columns(obgpu_result *res, const int32_t *group_cols, 
  * One synchronisation. OBGPU_INVALID_ARGUMENT when the result has no groups. */
 int obgpu_result_fetch_group_columns(obgpu_result *res, int64_t *host_keys, uint8_t *host_key_nulls, void *host_key_heap,
                                      int64_t *host_out);
+/* ORDER BY key, ... LIMIT k over every block of a scan: the first min(k, selected) of the rows the scan selected (all rows
+ * without a filter; the bitmap of a capacity-overflowed scan or of obgpu_scan_bitmap, as obgpu_result_group_by_values), in the
+ * order of keys[0..n_keys), and the values of out_cols[0..n_out) in those rows. No key table is built: a key or output column of
+ * any encoding the scan decodes works (RAW, bit-packed, INTEGER_BASE_DIFF, DICT, RLE, CONST, the CS codecs, rebuilt and
+ * decompressed strings). The rows replace the result's previous ones, stay on the device until obgpu_result_free or the next
+ * call, and are independent of its groups; *n_rows and *heap_bytes (the string output heap's size) are set.
+ *   Order: lexicographic over the keys in the caller's order. Integers in the column's own signed or unsigned order (the MIN /
+ *   MAX order), strings bytewise as unsigned bytes with a proper prefix first (binary, whatever the collation, as group keys);
+ *   desc reverses a key's value order and nulls_first puts its NULLs before every value (else after). Equal tuples are ordered
+ *   by position -- block, then row -- so the answer is unique. A column may be named twice and may be a key and an output.
+ *   OBGPU_INVALID_ARGUMENT: n_keys outside 1..4, n_out outside 0..16, k < 1, a column out of range, a NULL pointer.
+ *   OBGPU_NOT_SUPPORTED (the ctx stays usable): k above 65 536; a key or output column that is not of an integer or string class
+ *   in every block, or whose decode plan in some block is not usable. OBGPU_ALLOCATE_MEMORY_FAILED: the scratch (about 25 bytes
+ *   per selected row) is not there. The scan's own error first. A refused or failed call leaves the result with no rows. */
+typedef struct obgpu_sort_key {
+  int32_t col;         /* store index of an integer-class, VARCHAR or CHAR column */
+  int32_t desc;        /* 0 ascending, 1 descending */
+  int32_t nulls_first; /* 1: NULL before every value, 0: after */
+} obgpu_sort_key;
+int obgpu_result_top_rows(obgpu_result *res, const obgpu_sort_key *keys, int32_t n_keys, const int32_t *out_cols, int32_t n_out,
+                          int64_t k, int64_t *n_rows, int64_t *heap_bytes);
+/* The last obgpu_result_top_rows' rows, in order: host_block[i] the block index in the batch and host_row[i] the block-relative
+ * row id (as obgpu_result_fetch_row_ids gives it) of row i; per output column the layout of obgpu_result_fetch_group_columns:
+ * host_vals is [n_out][n_rows + 1] -- an integer's 64-bit image as MIN / MAX return it (0 where NULL), or for a string column
+ * n_rows + 1 offsets into the one host_heap, each string column's bytes following the previous one's (a NULL is empty) --
+ * and host_nulls is [n_out][n_rows], 1 where NULL. String bytes are copies. One synchronisation. OBGPU_INVALID_ARGUMENT when
+ * the result holds no rows (no successful obgpu_result_top_rows since the last one) or a needed pointer is NULL. */
+int obgpu_result_fetch_top_rows(obgpu_result *res, int32_t *host_block, int32_t *host_row, int64_t *host_vals, uint8_t *host_nulls,
+                                void *host_heap);
 /* A device group accumulator: merges, by value, the groups of several scan results -- typically one per page batch of a
  * table -- into the groups one obgpu_result_group_by_columns over all their rows would give. It lives on ctx's device, works
  * on a stream of its own (an add never waits for other work queued on ctx), and holds its groups in device memory, growing as

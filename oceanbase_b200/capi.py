@@ -187,6 +187,8 @@ def declared_signatures():
         "obgpu_pipeline_plan": (C.c_int, [P(HostScanSpec), P(i32), P(i64)]),
         "obgpu_pipeline_scan": (C.c_int, [vp, P(HostScanSpec), P(HostScanResult)]),
         "obgpu_pipeline_group_by": (C.c_int, [vp, P(HostScanSpec), vp, i32, vp, i32, P(HostScanResult), P(vp)]),
+        "obgpu_pipeline_top_rows": (C.c_int, [vp, P(HostScanSpec), vp, i32, vp, i32, i64, P(HostScanResult), P(i64), P(i64)]),
+        "obgpu_pipeline_fetch_top_rows": (C.c_int, [vp, vp, vp, vp, vp, vp]),
         "obgpu_batch_open": (C.c_int, [vp, vp, i64, vp, vp, i32, i32, vp, P(vp)]),
         "obgpu_batch_close": (None, [vp]),
         "obgpu_batch_block_info": (C.c_int, [vp, i32, P(i64), P(i32)]),
@@ -235,6 +237,8 @@ def declared_signatures():
         "obgpu_result_fetch_groups": (C.c_int, [vp, vp, vp, vp]),
         "obgpu_result_group_by_columns": (C.c_int, [vp, vp, i32, vp, i32, P(i64), P(i64)]),
         "obgpu_result_fetch_group_columns": (C.c_int, [vp, vp, vp, vp, vp]),
+        "obgpu_result_top_rows": (C.c_int, [vp, vp, i32, vp, i32, i64, P(i64), P(i64)]),
+        "obgpu_result_fetch_top_rows": (C.c_int, [vp, vp, vp, vp, vp, vp]),
         "obgpu_groups_create": (C.c_int, [vp, i32, vp, i32, P(vp)]),
         "obgpu_groups_free": (None, [vp]),
         "obgpu_groups_add": (C.c_int, [vp, vp]),

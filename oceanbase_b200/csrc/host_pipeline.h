@@ -13,6 +13,11 @@ struct obgpu_pipeline {
   int device = 0;
   std::vector<obgpu_ctx *> ctxs;
   std::string err;
+  // obgpu_pipeline_top_rows: its rows as a fetch buffer (topn::TopBuf) on ctxs[0], kept for obgpu_pipeline_fetch_top_rows;
+  // top_rows < 0: none
+  void *d_top = nullptr;
+  int64_t top_rows = -1, top_heap = 0;
+  int32_t top_n_out = 0;
 };
 
 namespace obpipe {
@@ -111,6 +116,10 @@ int obgpu_pipeline_create(int device, int32_t n_streams, obgpu_pipeline **out) {
 
 void obgpu_pipeline_destroy(obgpu_pipeline *p) {
   if (!p) return;
+  if (p->d_top) {
+    cudaSetDevice(p->device);
+    cudaFree(p->d_top);
+  }
   for (obgpu_ctx *c : p->ctxs) obgpu_ctx_destroy(c);
   delete p;
 }
@@ -462,6 +471,163 @@ int obgpu_pipeline_group_by(obgpu_pipeline *p, const obgpu_host_scan_spec *s, co
   }
   *out = acc;
   return OBGPU_SUCCESS;
+}
+
+int obgpu_pipeline_top_rows(obgpu_pipeline *p, const obgpu_host_scan_spec *s, const obgpu_sort_key *keys, int32_t n_keys,
+                            const int32_t *out_cols, int32_t n_out, int64_t k, obgpu_host_scan_result *res, int64_t *n_rows,
+                            int64_t *heap_bytes) {
+  if (!p) return OBGPU_INVALID_ARGUMENT;
+  cudaSetDevice(p->device);
+  if (p->d_top) cudaFree(p->d_top);   // a refused call leaves no rows
+  p->d_top = nullptr;
+  p->top_rows = -1;
+  p->top_heap = 0;
+  p->top_n_out = 0;
+  if (!s || !res || s->n_blocks <= 0 || !s->image || !s->offsets || !s->sizes) return OBGPU_INVALID_ARGUMENT;
+  if (const int a = topn::check_args(keys, n_keys, out_cols, n_out, k, n_rows, heap_bytes, 1u << 30); a != OBGPU_SUCCESS) {
+    if (a == OBGPU_NOT_SUPPORTED) p->err = "top rows: k above 65536";
+    return a;
+  }
+  if (!s->no_row_output || s->out_row_ids || s->out_block_begin || s->out_block_count || s->n_aggs != 0) {
+    p->err = "top rows through the pipeline return rows only: no_row_output 1, no row ids, block tables or scalar aggregates";
+    return OBGPU_INVALID_ARGUMENT;
+  }
+  if (const int ret = obpipe::check_source(p, s); ret != OBGPU_SUCCESS) return ret;
+  std::vector<int32_t> bounds;
+  obpipe::batch_bounds(s->n_blocks, obpipe::default_bpb(s), std::max(0, s->ramp), bounds);
+  const int32_t nb = (int32_t)bounds.size() - 1;
+  if (nb > res->n_batches_cap || !res->batch_row_begin || !res->batch_rows) return OBGPU_BUF_NOT_ENOUGH;
+  for (int32_t b = 0; b < nb; ++b) {
+    res->batch_row_begin[b] = 0;
+    if (res->batch_block_begin) res->batch_block_begin[b] = bounds[(size_t)b];
+  }
+  if (res->batch_block_begin) res->batch_block_begin[nb] = s->n_blocks;
+  res->n_batches = nb;
+  res->total_rows = res->selected_rows = 0;
+  res->h2d_bytes = res->d2h_bytes = res->kernel_launches = 0;
+  memset(res->agg_out, 0, sizeof(res->agg_out));
+  topn::Key key[topn::kMaxKeys]{};
+  for (int i = 0; i < n_keys; ++i) key[i] = topn::Key{keys[i].col, keys[i].desc ? 1 : 0, keys[i].nulls_first ? 1 : 0, 0};
+
+  std::atomic<int32_t> next{0};
+  std::atomic<int> first_err{OBGPU_SUCCESS};
+  std::mutex mu;   // the merged set, its column facts, result totals, error text
+  topn::TopSet acc;                 // the rows so far, positions table-wide; one ctx's memory, complete whenever mu is free
+  obgpu_ctx *acc_ctx = nullptr;
+  bool have = false;                // a batch has set the column facts below
+  uint32_t str_mask = 0, sgn_mask = 0;
+  int32_t types[topn::kMaxKeys + topn::kMaxOut] = {0}, col_str[topn::kMaxKeys + topn::kMaxOut] = {0};
+  std::vector<int64_t> launches0;
+  for (obgpu_ctx *c : p->ctxs) launches0.push_back(obgpu_ctx_launch_count(c));
+
+  auto worker = [&](obgpu_ctx *ctx) {
+    for (;;) {
+      const int32_t b = next.fetch_add(1);
+      if (b >= nb || first_err.load() != OBGPU_SUCCESS) return;
+      int64_t lo = 0, hi = 0;
+      obgpu_batch *batch = nullptr;
+      obgpu_result *r = nullptr;
+      obgpu_result_info info{};
+      int ret = obpipe::open_batch(ctx, s, bounds[(size_t)b], bounds[(size_t)b + 1], &lo, &hi, &batch);
+      if (ret == OBGPU_SUCCESS) {
+        obgpu_scan_spec spec{};   // nothing projected; the capacity is the batch's rows
+        spec.filter = s->filter;
+        ret = obgpu_scan(batch, &spec, &r);
+      }
+      if (ret == OBGPU_SUCCESS) ret = obgpu_result_info_get(r, &info);
+      int64_t nr = 0, hb = 0;
+      if (ret == OBGPU_SUCCESS) ret = obgpu_result_top_rows(r, keys, n_keys, out_cols, n_out, k, &nr, &hb);
+      if (ret == OBGPU_SUCCESS) {
+        std::lock_guard<std::mutex> g(mu);
+        const int n_cols = n_keys + n_out;
+        if (!have) {
+          have = true;
+          str_mask = r->top_str;
+          sgn_mask = r->top_sgn;
+          for (int c = 0; c < n_cols; ++c) types[c] = r->tset_types[c];
+        } else if (r->top_str != str_mask || r->top_sgn != sgn_mask || memcmp(types, r->tset_types, sizeof(int32_t) * (size_t)n_cols) != 0) {
+          ctx->err = "top rows: a key or output column has another obj_type in another page batch";
+          ret = OBGPU_NOT_SUPPORTED;
+        }
+        if (ret == OBGPU_SUCCESS && first_err.load() == OBGPU_SUCCESS) {
+          const topn::TopSet bs = topn::set_of(r);
+          for (int c = 0; c < n_cols; ++c) {
+            const int sc = obf::store_class_of((uint8_t)types[c]);
+            col_str[c] = sc == 5;
+            if (c < n_keys) key[c].str = sc == 5;
+          }
+          // acc (table-wide positions) and this batch's rows (blocks + the batch's first block), k kept; synchronous, so that
+          // acc is complete for the next worker and the result may go
+          topn::TopSet merged;
+          ret = topn::order_sets(ctx, acc, bs, (uint64_t)bounds[(size_t)b], n_keys, key, col_str, k, merged);
+          if (ret == OBGPU_SUCCESS && cudaStreamSynchronize(ctx->stream) != cudaSuccess) {
+            ctx->err = "top rows: the merge failed";
+            ret = OBGPU_ERR_SYS;
+          }
+          if (ret == OBGPU_SUCCESS) {
+            if (acc.mem) topn::free_set(ctx, acc);   // acc_ctx's work on it finished before it was released
+            acc = merged;
+            acc_ctx = ctx;
+            res->batch_rows[b] = info.selected_rows;
+            res->total_rows += info.total_rows;
+            res->selected_rows += info.selected_rows;
+            if (!s->zero_copy) res->h2d_bytes += hi - lo;
+          } else {
+            topn::free_set(ctx, merged);
+          }
+        }
+      }
+      if (ret != OBGPU_SUCCESS) {
+        int expected = OBGPU_SUCCESS;
+        if (first_err.compare_exchange_strong(expected, ret)) {
+          std::lock_guard<std::mutex> g(mu);
+          p->err = obgpu_ctx_last_error(ctx);
+        }
+      }
+      if (r) obgpu_result_free(r);
+      if (batch) obgpu_batch_close(batch);
+      if (ret != OBGPU_SUCCESS) return;
+    }
+  };
+  std::vector<std::thread> th;
+  for (size_t i = 1; i < p->ctxs.size(); ++i) th.emplace_back(worker, p->ctxs[i]);
+  worker(p->ctxs[0]);
+  for (auto &t : th) t.join();
+  for (size_t i = 0; i < p->ctxs.size(); ++i) obgpu_ctx_synchronize(p->ctxs[i]);
+  int ret = first_err.load();
+  obgpu_ctx *c0 = p->ctxs[0];
+  if (ret == OBGPU_SUCCESS) {   // no batch selected a row: the set is empty
+    void *buf = nullptr;
+    int64_t heap = 0;
+    ret = topn::emit(c0, acc, n_keys, n_out, str_mask, sgn_mask, &buf, &heap);
+    if (ret == OBGPU_SUCCESS) {
+      p->d_top = buf;
+      p->top_rows = acc.n;
+      p->top_heap = heap;
+      p->top_n_out = n_out;
+      *n_rows = acc.n;
+      *heap_bytes = heap;
+    } else {
+      p->err = obgpu_ctx_last_error(c0);
+    }
+  }
+  if (acc.mem) topn::free_set(c0, acc);
+  for (size_t i = 0; i < p->ctxs.size(); ++i) {
+    obgpu_ctx_synchronize(p->ctxs[i]);
+    res->kernel_launches += obgpu_ctx_launch_count(p->ctxs[i]) - launches0[i];
+  }
+  (void)acc_ctx;
+  return ret;
+}
+
+int obgpu_pipeline_fetch_top_rows(obgpu_pipeline *p, int32_t *host_block, int32_t *host_row, int64_t *host_vals, uint8_t *host_nulls,
+                                  void *host_heap) {
+  if (!p || p->top_rows < 0 || !host_block || !host_row || (p->top_n_out > 0 && (!host_vals || !host_nulls)) || (p->top_heap > 0 && !host_heap))
+    return OBGPU_INVALID_ARGUMENT;
+  cudaSetDevice(p->device);
+  const int ret = topn::fetch(p->ctxs[0], p->d_top, p->top_rows, p->top_n_out, p->top_heap, host_block, host_row, host_vals, host_nulls, host_heap);
+  if (ret != OBGPU_SUCCESS) p->err = obgpu_ctx_last_error(p->ctxs[0]);
+  return ret;
 }
 
 }  // extern "C"

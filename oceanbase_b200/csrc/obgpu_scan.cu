@@ -1975,6 +1975,13 @@ struct obgpu_result {
   int32_t gv_kind[16] = {0}, gv_agg_col[16] = {0}, gv_agg_type[16] = {0};
   int32_t gv_key_type[4] = {0};   // gvals::kMaxGroupCols
   uint32_t gv_sgn_key = 0, gv_sgn_agg = 0;
+  // obgpu_result_top_rows: its rows (top_rows.cuh) as a fetch buffer (topn::TopBuf, obgpu_result_fetch_top_rows) and as a
+  // self-contained set (topn::SetLay, merged by obgpu_pipeline_top_rows); top_rows < 0: none
+  void *d_top = nullptr, *d_tset = nullptr;
+  int64_t top_rows = -1, top_heap = 0, tset_heap = 0;
+  int32_t top_n_out = 0, tset_cols = 0;
+  uint32_t top_str = 0, top_sgn = 0;   // bit j: output column j is a string / has its order key's sign bit flipped
+  int32_t tset_types[20] = {0};        // each set column's obj_type (topn::kMaxKeys + topn::kMaxOut)
 };
 
 static thread_local std::string g_last_global_err;
@@ -3012,6 +3019,8 @@ void obgpu_result_free(obgpu_result *r) {
   if (r->arena) cudaFreeAsync(r->arena, r->ctx->stream);
   if (r->d_str) cudaFreeAsync(r->d_str, r->ctx->stream);
   if (r->d_gv) cudaFreeAsync(r->d_gv, r->ctx->stream);
+  if (r->d_top) cudaFreeAsync(r->d_top, r->ctx->stream);
+  if (r->d_tset) cudaFreeAsync(r->d_tset, r->ctx->stream);
   delete r;
 }
 
@@ -3437,6 +3446,7 @@ int obgpu_project_datums(obgpu_batch *batch, int32_t block, int32_t col, const i
 #include "dict_ops.cuh"
 #include "group_values.cuh"   // GROUP BY over a scan, one group per distinct value of the batch
 #include "group_merge.cuh"    // the groups of several scans merged by value on the device (obgpu_groups)
+#include "top_rows.cuh"       // ORDER BY ... LIMIT k over a scan: the first k selected rows in key order
 
 // ---- major-compaction merge (include/obgpu_compaction.h) -----------------------------------------
 #include "../../include/obgpu_compaction.h"

@@ -15,7 +15,7 @@ import numpy as np
 
 from . import capi
 from .capi import lib
-from .scan import GroupAccumulator, flatten_filter
+from .scan import GroupAccumulator, fetch_top_rows, flatten_filter, sort_keys
 from .sstable import TableImage
 
 
@@ -367,6 +367,70 @@ class HostScanPipeline:
         stats = GroupByStats(n, blk_begin[:n + 1].copy(), rows[:n].copy(), int(res.total_rows), int(res.selected_rows), int(res.h2d_bytes),
                              int(res.d2h_bytes), int(res.kernel_launches))
         return keys, out, stats
+
+    def top_rows(self, table: TableImage, filter, keys, out_cols: Sequence[int], k: int, blocks_per_batch: int = 0, ramp: int = 0,
+                 compressor: int = 0, zero_copy: bool = False, agg_rows: Optional[np.ndarray] = None, agg_off: Optional[np.ndarray] = None):
+        """ORDER BY keys LIMIT k over the rows of a host table that filter selects, every page batch's rows merged on the device
+        (obgpu_pipeline_top_rows). keys and out_cols as ScanResult.top_rows takes them. Returns (positions, rows, stats):
+        positions one (block index in the table, row) per row; positions and rows are exactly what ScanResult.top_rows returns
+        over the whole table as one batch. blocks_per_batch 0: n_blocks / 12."""
+        spec, keep = self._spec(table, filter, [], blocks_per_batch, 1.0, ramp, 0, agg_rows, agg_off)
+        spec.no_row_output = 1
+        spec.compressor_type = int(compressor)
+        spec.zero_copy = 1 if zero_copy else 0
+        nb, cap = C.c_int32(0), C.c_int64(0)
+        capi.check(lib.obgpu_pipeline_plan(C.byref(spec), C.byref(nb), C.byref(cap)), "obgpu_pipeline_plan")
+        karr, cols = sort_keys(keys), np.array(list(out_cols), dtype=np.int32)
+        res = capi.HostScanResult()
+        row_begin = np.zeros(nb.value + 1, dtype=np.int64)
+        rows = np.zeros(nb.value + 1, dtype=np.int64)
+        blk_begin = np.zeros(nb.value + 2, dtype=np.int32)
+        res.batch_row_begin, res.batch_rows, res.batch_block_begin = row_begin.ctypes.data, rows.ctypes.data, blk_begin.ctypes.data
+        res.n_batches_cap = nb.value
+        nr, hb = C.c_int64(0), C.c_int64(0)
+        code = lib.obgpu_pipeline_top_rows(self._h, C.byref(spec), karr.ctypes.data, len(karr), cols.ctypes.data if len(cols) else None,
+                                           len(cols), k, C.byref(res), C.byref(nr), C.byref(hb))
+        if code != capi.OB_SUCCESS:
+            raise capi.ObGpuError(code, "obgpu_pipeline_top_rows", (lib.obgpu_pipeline_last_error(self._h) or b"").decode())
+        self.launch_count += res.kernel_launches
+
+        def fetch(*a):
+            capi.check(lib.obgpu_pipeline_fetch_top_rows(self._h, *a), "obgpu_pipeline_fetch_top_rows")
+        positions, out = fetch_top_rows(fetch, nr.value, hb.value, self._column_types(table, cols.tolist(), compressor))
+        n = res.n_batches
+        stats = GroupByStats(n, blk_begin[:n + 1].copy(), rows[:n].copy(), int(res.total_rows), int(res.selected_rows), int(res.h2d_bytes),
+                             int(res.d2h_bytes), int(res.kernel_launches))
+        return positions, out, stats
+
+    def _column_types(self, table, cols, compressor=0):
+        """(obj_type, datum length; 0 for strings) of columns, read from the first block's column headers, or from the block
+        opened on the device when it is stored compressed"""
+        from .capi import OBJ_VARCHAR, OBJ_CHAR
+        if compressor:
+            from .scan import PageBatch, ScanContext
+            from .sstable import TableImage as _T
+            ctx = ScanContext(self.device)
+            o, n = int(table.offsets[0]), int(table.sizes[0])
+            one = _T(np.ascontiguousarray(table.image[o:o + n]), np.zeros(1, dtype=np.int64), np.array([n], dtype=np.int64), 0, table.n_cols)
+            batch = PageBatch(ctx, one, compressor=compressor)
+            out = []
+            try:
+                for c in cols:
+                    t, dl = C.c_int32(0), C.c_int32(0)
+                    capi.check(lib.obgpu_batch_column_type(batch._h, c, C.byref(t), C.byref(dl)), "obgpu_batch_column_type", ctx._h)
+                    out.append((t.value, dl.value))
+            finally:
+                batch.close()
+                ctx.close()
+            return out
+        blk = table.block(0)
+        hs = int(blk[4:8].view(np.uint32)[0])
+        cs = int(blk[20]) == 3
+        out = []
+        for c in cols:
+            t = int(blk[hs + 12 + 4 * c + 3]) if cs else int(blk[hs + 16 * c + 3])
+            out.append((t, 0 if t in (OBJ_VARCHAR, OBJ_CHAR) else capi.datum_len_of(t)))
+        return out
 
     def _column_shapes(self, table, proj, compressor=0):
         """(is_string, elem_len) of the projected columns, read from the first block's column headers. A stored block's

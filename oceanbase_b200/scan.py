@@ -103,6 +103,25 @@ def group_tuples(keys, nulls, heap, n, types):
     return list(zip(*per_col)) if n else []
 
 
+def sort_keys(keys):
+    """sort keys (a store column, or (col, desc, nulls_first)) -> the int32 [n][3] array of obgpu_sort_key"""
+    ks = [(kk, 0, 0) if isinstance(kk, int) else tuple(int(x) for x in kk) for kk in keys]
+    return np.array(ks, dtype=np.int32).reshape(-1, 3)
+
+
+def fetch_top_rows(fetch, n, heap_bytes, types):
+    """rows in obgpu_result_fetch_top_rows' layout (fetch(blocks, rows, vals, nulls, heap) fills it) -> (positions, rows) as
+    ScanResult.top_rows returns them; types: (obj_type, datum_len) per output column"""
+    no = len(types)
+    blocks, rows = np.zeros(max(n, 1), dtype=np.int32), np.zeros(max(n, 1), dtype=np.int32)
+    vals = np.zeros((no, n + 1), dtype=np.int64)
+    nulls = np.zeros((no, max(n, 1)), dtype=np.uint8)
+    heap = np.zeros(max(heap_bytes, 1), dtype=np.uint8)
+    fetch(blocks.ctypes.data, rows.ctypes.data, vals.ctypes.data, nulls.ctypes.data, heap.ctypes.data)
+    positions = list(zip(blocks[:n].tolist(), rows[:n].tolist()))
+    return positions, (group_tuples(vals, nulls, heap, n, types) if no else [()] * n)
+
+
 # ---- context / batch / result ----------------------------------------------------------------------
 class ScanContext:
     """obgpu_ctx: one per worker thread (device + stream)."""
@@ -591,6 +610,25 @@ class ScanResult:
                   self.batch.ctx._h)
             types.append((obj_type.value, dlen.value))
         return group_tuples(keys, nulls, heap, n, types), out[:, :n]
+
+    def top_rows(self, keys, out_cols, k):
+        """ORDER BY keys LIMIT k over every block of the scan (obgpu_result_top_rows): the first min(k, selected) selected rows.
+        keys: 1..4 sort keys, each a store column or a (col, desc, nulls_first) tuple (ascending, NULLs last by default);
+        out_cols: 0..16 store columns. Returns (positions, rows): positions one (block, block-relative row) per row, in order;
+        rows one tuple per row, the out_cols values as Python ints in their column's value domain (unsigned types
+        non-negative), bytes, or None for NULL. Ties are ordered by position."""
+        karr, cols = sort_keys(keys), np.array(list(out_cols), dtype=np.int32)
+        nr, hb = C.c_int64(0), C.c_int64(0)
+        check(lib.obgpu_result_top_rows(self._h, karr.ctypes.data, len(karr), cols.ctypes.data if len(cols) else None, len(cols), k,
+                                        C.byref(nr), C.byref(hb)), "obgpu_result_top_rows", self.batch.ctx._h)
+        types = []
+        for oc in cols.tolist():
+            obj_type, dlen = C.c_int32(0), C.c_int32(0)
+            check(lib.obgpu_batch_column_type(self.batch._h, oc, C.byref(obj_type), C.byref(dlen)), "obgpu_batch_column_type",
+                  self.batch.ctx._h)
+            types.append((obj_type.value, dlen.value))
+        return fetch_top_rows(lambda *a: check(lib.obgpu_result_fetch_top_rows(self._h, *a), "obgpu_result_fetch_top_rows",
+                                               self.batch.ctx._h), nr.value, hb.value, types)
 
     def fetch_datums(self, i, row_begin=0, row_count=None):
         """Column i as ObDatum[] (datum format): (datums structured array, slots uint64 array or None for strings)."""
