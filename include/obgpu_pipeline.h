@@ -111,6 +111,14 @@ int obgpu_pipeline_scan(obgpu_pipeline *p, const obgpu_host_scan_spec *spec, obg
  *   obgpu_pipeline_last_error; *out is then NULL and the pipeline stays usable. */
 int obgpu_pipeline_group_by(obgpu_pipeline *p, const obgpu_host_scan_spec *spec, const int32_t *group_cols, int32_t n_group_cols,
                             const obgpu_group_agg *aggs, int32_t n_aggs, obgpu_host_scan_result *result, obgpu_groups **out);
+/* GROUP BY as obgpu_pipeline_group_by, with each page batch grouped by obgpu_result_group_by_any: group columns of any
+ * encoding, each batch on the path its blocks allow, and the groups of both paths merged into one accumulator. Spec, result,
+ * *out and the spec refusals are obgpu_pipeline_group_by's; a batch refusal is obgpu_result_group_by_any's. The groups are those
+ * of obgpu_result_group_by_any over the whole table as one batch. *cells_batches (may be NULL): how many batches took
+ * OBGPU_GROUP_PATH_CELLS (0 after a failure). */
+int obgpu_pipeline_group_by_any(obgpu_pipeline *p, const obgpu_host_scan_spec *spec, const int32_t *group_cols, int32_t n_group_cols,
+                                const obgpu_group_agg *aggs, int32_t n_aggs, obgpu_host_scan_result *result, obgpu_groups **out,
+                                int32_t *cells_batches);
 /* ORDER BY keys LIMIT k over every row of the spec's table that its filter selects: each worker opens its batch as
  * obgpu_pipeline_group_by does, scans it with nothing projected, takes its rows with obgpu_result_top_rows and merges them, under
  * the pipeline's mutex, into one device-resident set of at most k rows (at most 2k rows ordered per merge, k kept). Positions are

@@ -512,6 +512,23 @@ int obgpu_result_group_by_columns(obgpu_result *res, const int32_t *group_cols, 
  * One synchronisation. OBGPU_INVALID_ARGUMENT when the result has no groups. */
 int obgpu_result_fetch_group_columns(obgpu_result *res, int64_t *host_keys, uint8_t *host_key_nulls, void *host_key_heap,
                                      int64_t *host_out);
+/* GROUP BY group_cols as obgpu_result_group_by_columns, for group columns of ANY encoding the scan decodes. Arguments, the
+ * group slot and its fetches (obgpu_result_fetch_group_columns, obgpu_result_fetch_groups for one column, obgpu_groups_add)
+ * are obgpu_result_group_by_columns'. Where that call succeeds, the groups are byte for byte its groups: keys, NULL flags, key
+ * heap and aggregates, in its order. The library picks the path from the batch and returns it in *path (may be NULL):
+ *   OBGPU_GROUP_PATH_DICT   every group column is dictionary coded in every block: obgpu_result_group_by_columns runs.
+ *   OBGPU_GROUP_PATH_CELLS  some group column is not, or the dictionary fold refuses for a limit of its own (65 536 values in
+ *                           a column's dictionaries, 4 194 304 hashed tuples, a string key of 65 536 bytes or more, an image of
+ *                           2^37 bytes or more): a hash fold over each selected row's decoded cells. A group column only has to
+ *                           be of an integer or string class with a usable plan in every block.
+ *   OBGPU_NOT_SUPPORTED (the ctx stays usable): a group column of another class or with an unusable plan in some block; the
+ *   aggregate refusals of obgpu_result_group_by_columns; more than 2^31 - 1 groups. OBGPU_INVALID_ARGUMENT as
+ *   obgpu_result_group_by_columns. OBGPU_ALLOCATE_MEMORY_FAILED: the group table (up to about 24 bytes per selected row and
+ *   group column plus 16 per aggregate) is not there. A failed call leaves the result with no groups and *path 0. */
+#define OBGPU_GROUP_PATH_DICT 1
+#define OBGPU_GROUP_PATH_CELLS 2
+int obgpu_result_group_by_any(obgpu_result *res, const int32_t *group_cols, int32_t n_group_cols, const obgpu_group_agg *aggs,
+                              int32_t n_aggs, int64_t *n_groups, int64_t *key_bytes, int32_t *path);
 /* ORDER BY key, ... LIMIT k over every block of a scan: the first min(k, selected) of the rows the scan selected (all rows
  * without a filter; the bitmap of a capacity-overflowed scan or of obgpu_scan_bitmap, as obgpu_result_group_by_values), in the
  * order of keys[0..n_keys), and the values of out_cols[0..n_out) in those rows. No key table is built: a key or output column of

@@ -111,6 +111,7 @@ class AggCell(C.Structure):
 SK_IDX_MIN, SK_IDX_MAX, SK_IDX_NULL_COUNT, SK_IDX_SUM = range(4)           # blocksstable::ObSkipIndexColType
 BOOL_MASK_UNCERTAIN, BOOL_MASK_ALWAYS_TRUE, BOOL_MASK_ALWAYS_FALSE = range(3)  # sql::ObBoolMaskType
 AGG_COUNT, AGG_SUM, AGG_SUM_PRODUCT, AGG_MIN, AGG_MAX = range(5)
+GROUP_PATH_DICT, GROUP_PATH_CELLS = 1, 2   # obgpu_result_group_by_any's *path
 DF_NOT_EXIST, DF_LOCK, DF_UPDATE, DF_INSERT, DF_DELETE = range(5)  # blocksstable::ObDmlFlag
 
 
@@ -187,6 +188,7 @@ def declared_signatures():
         "obgpu_pipeline_plan": (C.c_int, [P(HostScanSpec), P(i32), P(i64)]),
         "obgpu_pipeline_scan": (C.c_int, [vp, P(HostScanSpec), P(HostScanResult)]),
         "obgpu_pipeline_group_by": (C.c_int, [vp, P(HostScanSpec), vp, i32, vp, i32, P(HostScanResult), P(vp)]),
+        "obgpu_pipeline_group_by_any": (C.c_int, [vp, P(HostScanSpec), vp, i32, vp, i32, P(HostScanResult), P(vp), P(i32)]),
         "obgpu_pipeline_top_rows": (C.c_int, [vp, P(HostScanSpec), vp, i32, vp, i32, i64, P(HostScanResult), P(i64), P(i64)]),
         "obgpu_pipeline_fetch_top_rows": (C.c_int, [vp, vp, vp, vp, vp, vp]),
         "obgpu_batch_open": (C.c_int, [vp, vp, i64, vp, vp, i32, i32, vp, P(vp)]),
@@ -237,6 +239,7 @@ def declared_signatures():
         "obgpu_result_fetch_groups": (C.c_int, [vp, vp, vp, vp]),
         "obgpu_result_group_by_columns": (C.c_int, [vp, vp, i32, vp, i32, P(i64), P(i64)]),
         "obgpu_result_fetch_group_columns": (C.c_int, [vp, vp, vp, vp, vp]),
+        "obgpu_result_group_by_any": (C.c_int, [vp, vp, i32, vp, i32, P(i64), P(i64), P(i32)]),
         "obgpu_result_top_rows": (C.c_int, [vp, vp, i32, vp, i32, i64, P(i64), P(i64)]),
         "obgpu_result_fetch_top_rows": (C.c_int, [vp, vp, vp, vp, vp, vp]),
         "obgpu_groups_create": (C.c_int, [vp, i32, vp, i32, P(vp)]),

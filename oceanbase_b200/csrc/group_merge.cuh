@@ -485,60 +485,71 @@ int obgpu_groups_info(obgpu_groups *g, int64_t *n_groups, int64_t *key_bytes, in
 
 namespace gmerge {
 
+// the n groups of s in tuple order, as a new GroupBuf (*gv, allocated here on ctx's stream): a CUB merge sort of the group
+// indices by TupleLess, the string lengths in that order scanned into offsets, then gather_kernel. col_bytes[c]: string column
+// c's key bytes over the n groups. The accumulator's fetch and the hash fold over decoded cells (gcells) both end here.
+static int sorted_groups(obgpu_ctx *ctx, const Store &s, int64_t n, const int32_t *kind, uint32_t sgn_key, uint32_t sgn_agg,
+                         const int64_t *col_bytes, void **gv) {
+  int64_t kb = 0;
+  for (int c = 0; c < s.n_cols; ++c) kb += col_bytes[c];
+  const gvals::GroupBuf lay(n, s.n_cols, s.n_aggs, kb);
+  Scratch out(ctx);
+  CUDA_TRY(ctx, out.alloc(lay.end));
+  CUDA_TRY(ctx, cudaMemsetAsync(out.p, 0, lay.out, ctx->stream));   // no group: offsets {0}; integer columns' last slot 0
+  if (n > 0) {
+    size_t t_sort = 0, t_scan = 0;
+    CUDA_TRY(ctx, cub::DeviceMergeSort::SortKeys(nullptr, t_sort, (uint32_t *)nullptr, n, TupleLess{s}, ctx->stream));
+    if (s.str_mask) CUDA_TRY(ctx, cub::DeviceScan::ExclusiveSum(nullptr, t_scan, (const int64_t *)nullptr, (int64_t *)nullptr, n, ctx->stream));
+    // [order][string lengths, offsets: n_cols x n][sort temporaries][scan temporaries]
+    Scratch tmp(ctx);
+    const size_t o_order = tmp.take((size_t)n * 4), o_slen = tmp.take((size_t)s.n_cols * n * 8), o_soff = tmp.take((size_t)s.n_cols * n * 8);
+    const size_t o_sort = tmp.take(t_sort), o_scan = tmp.take(t_scan);
+    CUDA_TRY(ctx, tmp.alloc());
+    uint32_t *order = tmp.at<uint32_t>(o_order);
+    int64_t *slen = tmp.at<int64_t>(o_slen), *soff = tmp.at<int64_t>(o_soff);
+    const unsigned grid = (unsigned)((n + kThreads - 1) / kThreads);
+    gvals::iota_kernel<<<grid, kThreads, 0, ctx->stream>>>(order, (int)n);
+    CUDA_TRY(ctx, cub::DeviceMergeSort::SortKeys(tmp.p + o_sort, t_sort, order, n, TupleLess{s}, ctx->stream));
+    GatherArgs p{};
+    if (s.str_mask) {
+      sorted_lens_kernel<<<grid, kThreads, 0, ctx->stream>>>(s, order, n, slen);
+      ctx->launches++;
+      for (int c = 0; c < s.n_cols; ++c)
+        if ((s.str_mask >> c) & 1u) CUDA_TRY(ctx, cub::DeviceScan::ExclusiveSum(tmp.p + o_scan, t_scan, slen + c * n, soff + c * n, n, ctx->stream));
+    }
+    int64_t base = 0;
+    for (int c = 0; c < s.n_cols; ++c) {   // each string column's bytes follow the previous one's
+      p.base[c] = base;
+      base += col_bytes[c];
+    }
+    p.s = s;
+    p.order = order;
+    p.n = n;
+    for (int k = 0; k < s.n_aggs; ++k) p.kind[k] = kind[k];
+    p.sgn_key = sgn_key;
+    p.sgn_agg = sgn_agg;
+    p.soff = soff;
+    p.keys = out.at<int64_t>(0);
+    p.out = out.at<int64_t>(lay.out);
+    p.nulls = out.at<uint8_t>(lay.nulls);
+    p.heap = out.at<uint8_t>(lay.heap);
+    gather_kernel<<<grid, kThreads, 0, ctx->stream>>>(p);
+    ctx->launches += 2;
+    CUDA_TRY(ctx, cudaGetLastError());
+  }
+  *gv = out.release();
+  return OBGPU_SUCCESS;
+}
+
 // obgpu_groups_fetch on the accumulator's own stream (errors and launches land in g->own)
 static int fetch(obgpu_groups *g, int64_t *host_keys, uint8_t *host_key_nulls, void *host_key_heap, int64_t *host_out) {
   obgpu_ctx *ctx = &g->own;
-  const int64_t n = g->n;
-  const gvals::GroupBuf lay(n, g->n_cols, g->n_aggs, g->heap_used);
-  if (!g->d_gv) {
-    Scratch out(ctx);
-    CUDA_TRY(ctx, out.alloc(lay.end));
-    CUDA_TRY(ctx, cudaMemsetAsync(out.p, 0, lay.out, ctx->stream));   // no group: offsets {0}; integer columns' last slot 0
-    if (n > 0) {
-      const gmerge::Store s = gmerge::store_of(g, g->d_store, g->cap, g->d_heap);
-      size_t t_sort = 0, t_scan = 0;
-      CUDA_TRY(ctx, cub::DeviceMergeSort::SortKeys(nullptr, t_sort, (uint32_t *)nullptr, n, gmerge::TupleLess{s}, ctx->stream));
-      if (g->str_mask) CUDA_TRY(ctx, cub::DeviceScan::ExclusiveSum(nullptr, t_scan, (const int64_t *)nullptr, (int64_t *)nullptr, n, ctx->stream));
-      // [order][string lengths, offsets: n_cols x n][sort temporaries][scan temporaries]
-      Scratch tmp(ctx);
-      const size_t o_order = tmp.take((size_t)n * 4), o_slen = tmp.take((size_t)g->n_cols * n * 8), o_soff = tmp.take((size_t)g->n_cols * n * 8);
-      const size_t o_sort = tmp.take(t_sort), o_scan = tmp.take(t_scan);
-      CUDA_TRY(ctx, tmp.alloc());
-      uint32_t *order = tmp.at<uint32_t>(o_order);
-      int64_t *slen = tmp.at<int64_t>(o_slen), *soff = tmp.at<int64_t>(o_soff);
-      const unsigned grid = (unsigned)((n + gmerge::kThreads - 1) / gmerge::kThreads);
-      gvals::iota_kernel<<<grid, gmerge::kThreads, 0, ctx->stream>>>(order, (int)n);
-      CUDA_TRY(ctx, cub::DeviceMergeSort::SortKeys(tmp.p + o_sort, t_sort, order, n, gmerge::TupleLess{s}, ctx->stream));
-      gmerge::GatherArgs p{};
-      if (g->str_mask) {
-        gmerge::sorted_lens_kernel<<<grid, gmerge::kThreads, 0, ctx->stream>>>(s, order, n, slen);
-        ctx->launches++;
-        for (int c = 0; c < g->n_cols; ++c)
-          if ((g->str_mask >> c) & 1u) CUDA_TRY(ctx, cub::DeviceScan::ExclusiveSum(tmp.p + o_scan, t_scan, slen + c * n, soff + c * n, n, ctx->stream));
-      }
-      int64_t base = 0;
-      for (int c = 0; c < g->n_cols; ++c) {   // each string column's bytes follow the previous one's
-        p.base[c] = base;
-        base += g->col_bytes[c];
-      }
-      p.s = s;
-      p.order = order;
-      p.n = n;
-      for (int k = 0; k < g->n_aggs; ++k) p.kind[k] = g->kind[k];
-      p.sgn_key = g->sgn_key;
-      p.sgn_agg = g->sgn_agg;
-      p.soff = soff;
-      p.keys = out.at<int64_t>(0);
-      p.out = out.at<int64_t>(lay.out);
-      p.nulls = out.at<uint8_t>(lay.nulls);
-      p.heap = out.at<uint8_t>(lay.heap);
-      gmerge::gather_kernel<<<grid, gmerge::kThreads, 0, ctx->stream>>>(p);
-      ctx->launches += 2;
-      CUDA_TRY(ctx, cudaGetLastError());
-    }
-    g->d_gv = out.release();
-  }
-  return gvals::copy_groups(ctx, (const uint8_t *)g->d_gv, n, g->n_cols, g->n_aggs, g->heap_used, host_keys, host_key_nulls, host_key_heap,
+  if (!g->d_gv)
+    if (const int ret = sorted_groups(ctx, store_of(g, g->d_store, g->cap, g->d_heap), g->n, g->kind, g->sgn_key, g->sgn_agg, g->col_bytes,
+                                      &g->d_gv);
+        ret != OBGPU_SUCCESS)
+      return ret;
+  return gvals::copy_groups(ctx, (const uint8_t *)g->d_gv, g->n, g->n_cols, g->n_aggs, g->heap_used, host_keys, host_key_nulls, host_key_heap,
                             host_out);
 }
 

@@ -52,6 +52,9 @@ constexpr uint32_t kHashGroups = 1u << 22;        // the most distinct ids the h
 enum : int { ST_LONG_KEY = 8 };                   // a string entry of 65 536 bytes or more: no key (bcodes::key_of keeps 16 bits)
 enum : int { ONE_INT, ONE_STR, MULTI };           // fold_kernel's group columns: one integer, one string, or 1..4 of any kind
 enum : int { PATH_SHARED, PATH_GLOBAL, PATH_HASH_INSERT, PATH_HASH_FOLD };
+// why group_by_columns refused with OBGPU_NOT_SUPPORTED: WHY_OTHER for the refusals every GROUP BY shares (class, aggregates);
+// the others are limits of the dictionary fold that the hash fold over decoded cells (group_cells.cuh) does not have
+enum : int { WHY_OTHER, WHY_NOT_DICT, WHY_VALUE_CAP, WHY_LONG_KEY, WHY_IMAGE, WHY_TUPLE_CAP };
 
 // the order-preserving key of an integer value: its compare image, sign bit flipped for signed and narrow classes (the MIN / MAX key)
 __device__ __forceinline__ uint64_t order_key(const ColDesc &d, uint64_t v) {
@@ -428,12 +431,19 @@ struct ColStage {
   explicit ColStage(obgpu_ctx *c) : mem(c) {}
 };
 
-static int column_stages(obgpu_ctx *ctx, obgpu_batch *b, int32_t col, ColStage &cs) {
+// the order key of a group column of obj_type t has its sign bit flipped (gvals::order_key)
+static bool key_sgn(uint8_t t) { return obf::store_class_of(t) == 1 || obf::datum_len_of(t) < 8; }
+
+static int column_stages(obgpu_ctx *ctx, obgpu_batch *b, int32_t col, ColStage &cs, int *why) {
   const uint8_t gt = b->col_types[(size_t)col];
   const int gsc = gt == 0xff ? 0 : obf::store_class_of(gt);
   if (gsc != 1 && gsc != 2 && gsc != 5) { ctx->err = "group-by column is not an integer or string column in every micro block"; return OBGPU_NOT_SUPPORTED; }
   const bool str = gsc == 5;
-  if (str && b->image_size >= (int64_t)1 << 37) { ctx->err = "string group keys address images below 2^37 bytes"; return OBGPU_NOT_SUPPORTED; }
+  if (str && b->image_size >= (int64_t)1 << 37) {
+    *why = WHY_IMAGE;
+    ctx->err = "string group keys address images below 2^37 bytes";
+    return OBGPU_NOT_SUPPORTED;
+  }
   const int n = b->n_blocks;
   size_t t_sort = 0;   // cub's temporaries, sized for the most keys
   if (str)
@@ -466,10 +476,18 @@ static int column_stages(obgpu_ctx *ctx, obgpu_batch *b, int32_t col, ColStage &
   CUDA_TRY(ctx, cudaMemcpyAsync(hs, d_status, 4, cudaMemcpyDeviceToHost, ctx->stream));
   CUDA_TRY(ctx, cudaMemcpyAsync(hs + 1, ctr, 8, cudaMemcpyDeviceToHost, ctx->stream));
   CUDA_TRY(ctx, cudaStreamSynchronize(ctx->stream));
-  if (hs[0] & ST_UNSUPPORTED) { ctx->err = "group-by column is not dictionary coded in every micro block"; return OBGPU_NOT_SUPPORTED; }
-  if (hs[0] & ST_LONG_KEY) { ctx->err = "group-by string of 65536 bytes or more"; return OBGPU_NOT_SUPPORTED; }
+  if (hs[0] & ST_UNSUPPORTED) {
+    *why = WHY_NOT_DICT;
+    ctx->err = "group-by column is not dictionary coded in every micro block";
+    return OBGPU_NOT_SUPPORTED;
+  }
+  if (hs[0] & ST_LONG_KEY) { *why = WHY_LONG_KEY; ctx->err = "group-by string of 65536 bytes or more"; return OBGPU_NOT_SUPPORTED; }
   if (hs[0]) return check_status(ctx, hs[0]);
-  if (hs[2] || (uint32_t)hs[1] > (uint32_t)bcodes::kMaxCodes) { ctx->err = "more than 65536 distinct group-by values in the batch"; return OBGPU_NOT_SUPPORTED; }
+  if (hs[2] || (uint32_t)hs[1] > (uint32_t)bcodes::kMaxCodes) {
+    *why = WHY_VALUE_CAP;
+    ctx->err = "more than 65536 distinct group-by values in the batch";
+    return OBGPU_NOT_SUPPORTED;
+  }
   const int n_keys = hs[1];
   uint32_t *code_rank = tmp.at<uint32_t>(o_rank);
   uint64_t *rank_key = tmp.at<uint64_t>(o_rkey);
@@ -491,7 +509,7 @@ static int column_stages(obgpu_ctx *ctx, obgpu_batch *b, int32_t col, ColStage &
   }
   cs.dev = GroupCol{table, tmp.at<uint16_t>(o_slot), code_rank, (uint32_t)n_keys, col, str};
   cs.rank_key = rank_key;
-  cs.sgn_key = gsc == 1 || obf::datum_len_of(gt) < 8;
+  cs.sgn_key = key_sgn(gt);
   return OBGPU_SUCCESS;
 }
 
@@ -505,6 +523,46 @@ struct GroupBuf {
     end = heap + (size_t)key_bytes + 16;
   }
 };
+
+// the result's group slot <- groups in the GroupBuf layout at gv (the slot takes gv over)
+static void set_groups(obgpu_result *r, void *gv, int64_t ng, int64_t kb, const int32_t *cols, int n_cols, const obgpu_group_agg *aggs,
+                       int n_aggs, uint32_t str_mask, uint32_t sgn_agg) {
+  const obgpu_batch *b = r->batch;
+  r->d_gv = gv;
+  r->gv_groups = ng;
+  r->gv_key_bytes = kb;
+  r->gv_n_aggs = n_aggs;
+  r->gv_n_cols = n_cols;
+  r->gv_str_mask = str_mask;
+  for (int k = 0; k < n_aggs; ++k) {
+    r->gv_kind[k] = aggs[k].kind;
+    r->gv_agg_col[k] = aggs[k].col;
+    r->gv_agg_type[k] = aggs[k].col >= 0 ? b->col_types[(size_t)aggs[k].col] : -1;
+  }
+  r->gv_sgn_key = 0;
+  for (int c = 0; c < n_cols; ++c) {
+    r->gv_key_type[c] = b->col_types[(size_t)cols[c]];
+    if (key_sgn((uint8_t)r->gv_key_type[c])) r->gv_sgn_key |= 1u << c;
+  }
+  r->gv_sgn_agg = sgn_agg;
+}
+
+// the aggregates every GROUP BY folds: COUNT / SUM / MIN / MAX over integer-class columns or COUNT(*); *sgn_agg: bit k when
+// aggregate k's MIN / MAX key has its sign bit flipped
+static int check_aggs(obgpu_ctx *ctx, const obgpu_batch *b, const obgpu_group_agg *aggs, int32_t n_aggs, uint32_t *sgn_agg) {
+  *sgn_agg = 0;
+  for (int k = 0; k < n_aggs; ++k) {
+    if (aggs[k].kind < OBGPU_AGG_COUNT || aggs[k].kind > OBGPU_AGG_MAX || aggs[k].kind == OBGPU_AGG_SUM_PRODUCT) return OBGPU_NOT_SUPPORTED;
+    if (aggs[k].col >= (int32_t)b->max_cols || (aggs[k].col < 0 && aggs[k].kind != OBGPU_AGG_COUNT)) return OBGPU_INVALID_ARGUMENT;
+    if (aggs[k].col >= 0) {
+      const uint8_t t = b->col_types[(size_t)aggs[k].col];
+      const int sc = t == 0xff ? 0 : obf::store_class_of(t);
+      if (sc != 1 && sc != 2) { ctx->err = "aggregates fold integer-class columns only"; return OBGPU_NOT_SUPPORTED; }
+      if (obf::store_class_of(t) == 1 || obf::datum_len_of(t) < 8) *sgn_agg |= 1u << k;
+    }
+  }
+  return OBGPU_SUCCESS;
+}
 
 // the scan's own status first, then the previous call's groups dropped: a refused call leaves none
 static int begin_groups(obgpu_result *r) {
@@ -520,9 +578,10 @@ static int begin_groups(obgpu_result *r) {
 }
 
 // GROUP BY the tuple of cols[0..n_cols) (arguments checked by the caller but the aggregates); *has_null: the last group's first
-// key is NULL
+// key is NULL; *why: the reason of an OBGPU_NOT_SUPPORTED (WHY_*)
 static int group_by_columns(obgpu_result *r, const int32_t *cols, int n_cols, const obgpu_group_agg *aggs, int32_t n_aggs, int64_t *n_groups,
-                            int64_t *key_bytes, int32_t *has_null) {
+                            int64_t *key_bytes, int32_t *has_null, int *why) {
+  *why = WHY_OTHER;
   obgpu_batch *b = r->batch;
   obgpu_ctx *ctx = r->ctx;
   FoldAggs ga{};
@@ -531,15 +590,8 @@ static int group_by_columns(obgpu_result *r, const int32_t *cols, int n_cols, co
   ga.col[0] = -1;
   GatherArgs gp{};
   gp.n_aggs = n_aggs;
+  if (const int ret = check_aggs(ctx, b, aggs, n_aggs, &gp.sgn_agg); ret != OBGPU_SUCCESS) return ret;
   for (int k = 0; k < n_aggs; ++k) {
-    if (aggs[k].kind < OBGPU_AGG_COUNT || aggs[k].kind > OBGPU_AGG_MAX || aggs[k].kind == OBGPU_AGG_SUM_PRODUCT) return OBGPU_NOT_SUPPORTED;
-    if (aggs[k].col >= (int32_t)b->max_cols || (aggs[k].col < 0 && aggs[k].kind != OBGPU_AGG_COUNT)) return OBGPU_INVALID_ARGUMENT;
-    if (aggs[k].col >= 0) {
-      const uint8_t t = b->col_types[(size_t)aggs[k].col];
-      const int sc = t == 0xff ? 0 : obf::store_class_of(t);
-      if (sc != 1 && sc != 2) { ctx->err = "aggregates fold integer-class columns only"; return OBGPU_NOT_SUPPORTED; }
-      if (obf::store_class_of(t) == 1 || obf::datum_len_of(t) < 8) gp.sgn_agg |= 1u << k;
-    }
     ga.kind[k + 1] = gp.kind[k] = aggs[k].kind;
     ga.col[k + 1] = aggs[k].col;
   }
@@ -549,12 +601,12 @@ static int group_by_columns(obgpu_result *r, const int32_t *cols, int n_cols, co
   uint32_t str_mask = 0;
   for (int c = 0; c < n_cols; ++c) {
     st[c] = std::make_unique<ColStage>(ctx);
-    if (const int ret = column_stages(ctx, b, cols[c], *st[c]); ret != OBGPU_SUCCESS) return ret;
+    if (const int ret = column_stages(ctx, b, cols[c], *st[c], why); ret != OBGPU_SUCCESS) return ret;
     fp.gc[c] = st[c]->dev;
     gp.k.kc[c] = KeyCol{st[c]->rank_key, (uint64_t)st[c]->dev.n_keys + 1, 0, st[c]->dev.str, st[c]->sgn_key};
     if (st[c]->dev.str) str_mask |= 1u << c;
     P *= (uint64_t)st[c]->dev.n_keys + 1;
-    if (P >= (unsigned __int128)~0ull) { ctx->err = "2^64 - 1 or more composite group ids"; return OBGPU_NOT_SUPPORTED; }
+    if (P >= (unsigned __int128)~0ull) { *why = WHY_TUPLE_CAP; ctx->err = "2^64 - 1 or more composite group ids"; return OBGPU_NOT_SUPPORTED; }
   }
   gp.k.n_cols = n_cols;
   const int path = (uint64_t)P <= kDenseGroups && (uint64_t)P * (uint64_t)ga.n * 16 <= kSharedAccBudget ? PATH_SHARED
@@ -609,7 +661,11 @@ static int group_by_columns(obgpu_result *r, const int32_t *cols, int n_cols, co
     CUDA_TRY(ctx, cudaMemcpyAsync(hc + 2, d_status, 4, cudaMemcpyDeviceToHost, ctx->stream));
     CUDA_TRY(ctx, cudaStreamSynchronize(ctx->stream));
     if (hc[2]) return check_status(ctx, (int)hc[2]);
-    if (hc[1] || hc[0] > kHashGroups) { ctx->err = "more than 4194304 distinct group-by tuples in the selected rows"; return OBGPU_NOT_SUPPORTED; }
+    if (hc[1] || hc[0] > kHashGroups) {
+      *why = WHY_TUPLE_CAP;
+      ctx->err = "more than 4194304 distinct group-by tuples in the selected rows";
+      return OBGPU_NOT_SUPPORTED;
+    }
     G = hc[0];
     if (G > 0) {
       int end_bit = 0;
@@ -706,23 +762,7 @@ static int group_by_columns(obgpu_result *r, const int32_t *cols, int n_cols, co
       return OBGPU_ERR_SYS;
     }
   }
-  r->d_gv = gv;
-  r->gv_groups = ng;
-  r->gv_key_bytes = kb;
-  r->gv_n_aggs = n_aggs;
-  r->gv_n_cols = n_cols;
-  r->gv_str_mask = str_mask;
-  for (int k = 0; k < n_aggs; ++k) {
-    r->gv_kind[k] = aggs[k].kind;
-    r->gv_agg_col[k] = aggs[k].col;
-    r->gv_agg_type[k] = aggs[k].col >= 0 ? b->col_types[(size_t)aggs[k].col] : -1;
-  }
-  r->gv_sgn_key = 0;
-  for (int c = 0; c < n_cols; ++c) {
-    r->gv_key_type[c] = b->col_types[(size_t)cols[c]];
-    if (st[c]->sgn_key) r->gv_sgn_key |= 1u << c;
-  }
-  r->gv_sgn_agg = gp.sgn_agg;
+  set_groups(r, gv, ng, kb, cols, n_cols, aggs, n_aggs, str_mask, gp.sgn_agg);
   *n_groups = ng;
   *key_bytes = kb;
   if (has_null) *has_null = null_last;
@@ -753,7 +793,8 @@ int obgpu_result_group_by_values(obgpu_result *r, int32_t group_col, const obgpu
   if (group_col < 0 || (uint32_t)group_col >= r->batch->max_cols || n_aggs < 1 || n_aggs > 16 || !aggs || !n_groups || !key_bytes ||
       !has_null_group)
     return OBGPU_INVALID_ARGUMENT;
-  return gvals::group_by_columns(r, &group_col, 1, aggs, n_aggs, n_groups, key_bytes, has_null_group);
+  int why = 0;
+  return gvals::group_by_columns(r, &group_col, 1, aggs, n_aggs, n_groups, key_bytes, has_null_group, &why);
 }
 
 int obgpu_result_group_by_columns(obgpu_result *r, const int32_t *group_cols, int32_t n_group_cols, const obgpu_group_agg *aggs,
@@ -763,7 +804,8 @@ int obgpu_result_group_by_columns(obgpu_result *r, const int32_t *group_cols, in
     return OBGPU_INVALID_ARGUMENT;
   for (int c = 0; c < n_group_cols; ++c)
     if (group_cols[c] < 0 || (uint32_t)group_cols[c] >= r->batch->max_cols) return OBGPU_INVALID_ARGUMENT;
-  return gvals::group_by_columns(r, group_cols, n_group_cols, aggs, n_aggs, n_groups, key_bytes, nullptr);
+  int why = 0;
+  return gvals::group_by_columns(r, group_cols, n_group_cols, aggs, n_aggs, n_groups, key_bytes, nullptr, &why);
 }
 
 int obgpu_result_fetch_groups(obgpu_result *r, int64_t *host_keys, void *host_key_heap, int64_t *host_out) {

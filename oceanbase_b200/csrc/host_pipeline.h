@@ -382,8 +382,15 @@ int obgpu_pipeline_scan(obgpu_pipeline *p, const obgpu_host_scan_spec *s, obgpu_
   return first_err.load();
 }
 
-int obgpu_pipeline_group_by(obgpu_pipeline *p, const obgpu_host_scan_spec *s, const int32_t *group_cols, int32_t n_group_cols,
-                            const obgpu_group_agg *aggs, int32_t n_aggs, obgpu_host_scan_result *res, obgpu_groups **out) {
+}  // extern "C"
+
+namespace obpipe {
+
+// GROUP BY through the pipeline: each worker opens its batch, scans it with nothing projected, groups it with
+// group_batch(result, &n_groups, &key_bytes) and adds the groups to one accumulator under the mutex
+template <class GroupBatch>
+static int group_by(obgpu_pipeline *p, const obgpu_host_scan_spec *s, const int32_t *group_cols, int32_t n_group_cols,
+                    const obgpu_group_agg *aggs, int32_t n_aggs, obgpu_host_scan_result *res, obgpu_groups **out, GroupBatch group_batch) {
   if (!p || !s || !res || !out || s->n_blocks <= 0 || !s->image || !s->offsets || !s->sizes || !group_cols || n_group_cols < 1 ||
       n_group_cols > gvals::kMaxGroupCols || !aggs || n_aggs < 1 || n_aggs > 16)
     return OBGPU_INVALID_ARGUMENT;
@@ -434,7 +441,7 @@ int obgpu_pipeline_group_by(obgpu_pipeline *p, const obgpu_host_scan_spec *s, co
       }
       if (ret == OBGPU_SUCCESS) ret = obgpu_result_info_get(r, &info);
       int64_t ng = 0, kb = 0;
-      if (ret == OBGPU_SUCCESS) ret = obgpu_result_group_by_columns(r, group_cols, n_group_cols, aggs, n_aggs, &ng, &kb);
+      if (ret == OBGPU_SUCCESS) ret = group_batch(r, &ng, &kb);
       if (ret == OBGPU_SUCCESS) {
         std::lock_guard<std::mutex> g(mu);
         if (first_err.load() == OBGPU_SUCCESS) ret = obgpu_groups_add(acc, r);
@@ -471,6 +478,31 @@ int obgpu_pipeline_group_by(obgpu_pipeline *p, const obgpu_host_scan_spec *s, co
   }
   *out = acc;
   return OBGPU_SUCCESS;
+}
+
+}  // namespace obpipe
+
+extern "C" {
+
+int obgpu_pipeline_group_by(obgpu_pipeline *p, const obgpu_host_scan_spec *s, const int32_t *group_cols, int32_t n_group_cols,
+                            const obgpu_group_agg *aggs, int32_t n_aggs, obgpu_host_scan_result *res, obgpu_groups **out) {
+  return obpipe::group_by(p, s, group_cols, n_group_cols, aggs, n_aggs, res, out, [&](obgpu_result *r, int64_t *ng, int64_t *kb) {
+    return obgpu_result_group_by_columns(r, group_cols, n_group_cols, aggs, n_aggs, ng, kb);
+  });
+}
+
+int obgpu_pipeline_group_by_any(obgpu_pipeline *p, const obgpu_host_scan_spec *s, const int32_t *group_cols, int32_t n_group_cols,
+                                const obgpu_group_agg *aggs, int32_t n_aggs, obgpu_host_scan_result *res, obgpu_groups **out,
+                                int32_t *cells_batches) {
+  std::atomic<int32_t> cells{0};
+  const int ret = obpipe::group_by(p, s, group_cols, n_group_cols, aggs, n_aggs, res, out, [&](obgpu_result *r, int64_t *ng, int64_t *kb) {
+    int32_t path = 0;
+    const int gr = obgpu_result_group_by_any(r, group_cols, n_group_cols, aggs, n_aggs, ng, kb, &path);
+    if (path == OBGPU_GROUP_PATH_CELLS) cells.fetch_add(1);
+    return gr;
+  });
+  if (cells_batches) *cells_batches = ret == OBGPU_SUCCESS ? cells.load() : 0;
+  return ret;
 }
 
 int obgpu_pipeline_top_rows(obgpu_pipeline *p, const obgpu_host_scan_spec *s, const obgpu_sort_key *keys, int32_t n_keys,

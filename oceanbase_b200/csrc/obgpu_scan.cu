@@ -3447,6 +3447,7 @@ int obgpu_project_datums(obgpu_batch *batch, int32_t block, int32_t col, const i
 #include "group_values.cuh"   // GROUP BY over a scan, one group per distinct value of the batch
 #include "group_merge.cuh"    // the groups of several scans merged by value on the device (obgpu_groups)
 #include "top_rows.cuh"       // ORDER BY ... LIMIT k over a scan: the first k selected rows in key order
+#include "group_cells.cuh"    // GROUP BY columns of any encoding: a hash fold over decoded cells
 
 // ---- major-compaction merge (include/obgpu_compaction.h) -----------------------------------------
 #include "../../include/obgpu_compaction.h"

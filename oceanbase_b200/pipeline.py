@@ -338,6 +338,20 @@ class HostScanPipeline:
         and its groups merged on the device (obgpu_pipeline_group_by). aggs: (kind, store col or -1) as
         ScanResult.group_by_columns takes them. Returns (keys, out, GroupByStats); keys and out are exactly what
         ScanResult.group_by_columns returns over the whole table as one batch. blocks_per_batch 0: n_blocks / 12."""
+        keys, out, stats, _ = self._group_by("obgpu_pipeline_group_by", table, filter, group_cols, aggs, blocks_per_batch, ramp, compressor,
+                                             zero_copy, agg_rows, agg_off)
+        return keys, out, stats
+
+    def group_by_any(self, table: TableImage, filter, group_cols: Sequence[int], aggs: Sequence[tuple], blocks_per_batch: int = 0,
+                     ramp: int = 0, compressor: int = 0, zero_copy: bool = False, agg_rows: Optional[np.ndarray] = None,
+                     agg_off: Optional[np.ndarray] = None):
+        """group_by for group columns of any encoding (obgpu_pipeline_group_by_any): each batch grouped by
+        ScanResult.group_by_any's path. Returns (keys, out, GroupByStats, cells_batches): keys and out are exactly what
+        ScanResult.group_by_any returns over the whole table as one batch; cells_batches how many batches took the cells path."""
+        return self._group_by("obgpu_pipeline_group_by_any", table, filter, group_cols, aggs, blocks_per_batch, ramp, compressor, zero_copy,
+                              agg_rows, agg_off)
+
+    def _group_by(self, entry, table, filter, group_cols, aggs, blocks_per_batch, ramp, compressor, zero_copy, agg_rows, agg_off):
         spec, keep = self._spec(table, filter, [], blocks_per_batch, 1.0, ramp, 0, agg_rows, agg_off)
         spec.no_row_output = 1
         spec.compressor_type = int(compressor)
@@ -353,10 +367,14 @@ class HostScanPipeline:
         res.batch_row_begin, res.batch_rows, res.batch_block_begin = row_begin.ctypes.data, rows.ctypes.data, blk_begin.ctypes.data
         res.n_batches_cap = nb.value
         h = C.c_void_p()
-        code = lib.obgpu_pipeline_group_by(self._h, C.byref(spec), cols.ctypes.data, len(cols), gspec.ctypes.data if len(aggs) else None,
-                                           len(aggs), C.byref(res), C.byref(h))
+        args = [self._h, C.byref(spec), cols.ctypes.data, len(cols), gspec.ctypes.data if len(aggs) else None, len(aggs), C.byref(res),
+                C.byref(h)]
+        cells = C.c_int32(0)
+        if entry == "obgpu_pipeline_group_by_any":
+            args.append(C.byref(cells))
+        code = getattr(lib, entry)(*args)
         if code != capi.OB_SUCCESS:
-            raise capi.ObGpuError(code, "obgpu_pipeline_group_by", (lib.obgpu_pipeline_last_error(self._h) or b"").decode())
+            raise capi.ObGpuError(code, entry, (lib.obgpu_pipeline_last_error(self._h) or b"").decode())
         self.launch_count += res.kernel_launches
         acc = GroupAccumulator(h, len(cols), len(aggs), self)
         try:
@@ -366,7 +384,7 @@ class HostScanPipeline:
         n = res.n_batches
         stats = GroupByStats(n, blk_begin[:n + 1].copy(), rows[:n].copy(), int(res.total_rows), int(res.selected_rows), int(res.h2d_bytes),
                              int(res.d2h_bytes), int(res.kernel_launches))
-        return keys, out, stats
+        return keys, out, stats, cells.value
 
     def top_rows(self, table: TableImage, filter, keys, out_cols: Sequence[int], k: int, blocks_per_batch: int = 0, ramp: int = 0,
                  compressor: int = 0, zero_copy: bool = False, agg_rows: Optional[np.ndarray] = None, agg_off: Optional[np.ndarray] = None):

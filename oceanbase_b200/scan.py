@@ -596,11 +596,26 @@ class ScanResult:
         ng, kb = C.c_int64(0), C.c_int64(0)
         check(lib.obgpu_result_group_by_columns(self._h, cols.ctypes.data, len(cols), spec.ctypes.data, len(aggs), C.byref(ng), C.byref(kb)),
               "obgpu_result_group_by_columns", self.batch.ctx._h)
-        n, nc = ng.value, len(cols)
+        return self._fetch_group_columns(cols, len(aggs), ng.value, kb.value)
+
+    def group_by_any(self, group_cols, aggs):
+        """GROUP BY group_cols of any encoding (obgpu_result_group_by_any): returns (keys, out, path), keys and out as
+        group_by_columns returns them (and byte for byte its groups wherever it accepts the batch), path capi.GROUP_PATH_DICT
+        or capi.GROUP_PATH_CELLS: the fold the library chose."""
+        cols = np.array(list(group_cols), dtype=np.int32)
+        spec = np.array([(k, c) for k, c in aggs], dtype=np.int32).reshape(-1, 2)
+        ng, kb, path = C.c_int64(0), C.c_int64(0), C.c_int32(0)
+        check(lib.obgpu_result_group_by_any(self._h, cols.ctypes.data, len(cols), spec.ctypes.data, len(aggs), C.byref(ng), C.byref(kb),
+                                            C.byref(path)), "obgpu_result_group_by_any", self.batch.ctx._h)
+        keys, out = self._fetch_group_columns(cols, len(aggs), ng.value, kb.value)
+        return keys, out, path.value
+
+    def _fetch_group_columns(self, cols, n_aggs, n, key_bytes):
+        nc = len(cols)
         keys = np.zeros((nc, n + 1), dtype=np.int64)
         nulls = np.zeros((nc, max(n, 1)), dtype=np.uint8)
-        heap = np.zeros(max(kb.value, 1), dtype=np.uint8)
-        out = np.zeros((len(aggs), max(n, 1), 2), dtype=np.int64)
+        heap = np.zeros(max(key_bytes, 1), dtype=np.uint8)
+        out = np.zeros((n_aggs, max(n, 1), 2), dtype=np.int64)
         check(lib.obgpu_result_fetch_group_columns(self._h, keys.ctypes.data, nulls.ctypes.data, heap.ctypes.data, out.ctypes.data),
               "obgpu_result_fetch_group_columns", self.batch.ctx._h)
         types = []
